@@ -625,8 +625,10 @@ void lane_set_tuning(int clen, int halo, int variant) { g_tune.clen = clen; g_tu
 // Scratch of the lane engine, one buffer per device (grow-only, zero-initialised when (re)allocated):
 //     [stats 64 B][group counters: cap_groups ints][chunk records: 5 per (chunk, fiber)]
 // The counters must be zero between launches (the last warp of a group resets its counter), so their region has a FIXED size per
-// allocation -- it must never overlap what an earlier launch with fewer groups used for records.
-struct LaneScratch { void* p = nullptr; size_t cap = 0; long long cap_groups = 0; };
+// allocation -- it must never overlap what an earlier launch with fewer groups used for records.  A launch bakes the split (records
+// at group_count + cap_groups) into its arguments, and a regrown buffer may come back at the same address with a larger counter
+// region: `gen` counts the allocations, so that a captured graph can tell a stale layout from the current one (solver.cu: DrGraphKey).
+struct LaneScratch { void* p = nullptr; size_t cap = 0; long long cap_groups = 0; unsigned long long gen = 0; };
 static LaneScratch g_scr[64];
 static long long lane_scratch_bytes(long long groups_cap, long long nf, int len) {
     const long long nfp = (nf + 31) / 32 * 32 + 32 * 64;
@@ -774,9 +776,13 @@ void* lane_scratch(long long nf, int len) {
     if (need > s.cap || groups > s.cap_groups) {
         if (s.p) { cudaDeviceSynchronize(); cudaFree(s.p); s.p = nullptr; s.cap = 0; }
         if (cudaMalloc(&s.p, need) != cudaSuccess) { cudaGetLastError(); s.p = nullptr; s.cap_groups = 0; return nullptr; }
-        cudaMemset(s.p, 0, need); s.cap = need; s.cap_groups = gcap;
+        cudaMemset(s.p, 0, need); s.cap = need; s.cap_groups = gcap; s.gen++;
     }
     return s.p;
+}
+unsigned long long lane_scratch_generation() {
+    int d = 0; if (cudaGetDevice(&d) != cudaSuccess || d < 0 || d >= 64) return 0;
+    return g_scr[d].gen;
 }
 unsigned long long lane_read_stats(int reset) {
     int d = 0; if (cudaGetDevice(&d) != cudaSuccess || d < 0 || d >= 64 || !g_scr[d].p) return 0;

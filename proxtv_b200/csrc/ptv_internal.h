@@ -123,6 +123,7 @@ template <typename T>
 cudaError_t lane_prox(int op, const T* A, const T* B, const T* C, T* X, long long nf, int len, long long inc, T lam, void* scratch,
                       cudaStream_t st, T* X2 = nullptr);
 void* lane_scratch(long long nf, int len);          // per-device records / counters (allocates: call outside stream capture)
+unsigned long long lane_scratch_generation();       // per device: allocations of that buffer so far (its layout changes with each)
 bool lane_shape_ok(long long nf, int len, long long inc, size_t elem, const void* const* ptrs, int nptrs);
 void lane_set_tuning(int clen, int halo, int variant);
 void lane_set_tasklog(unsigned long long* dev, long long cap_tasks);

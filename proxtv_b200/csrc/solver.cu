@@ -266,11 +266,13 @@ template <typename T>
 int dr2_tspace_body(size_t M, size_t N, int batch, const T* Y, T w1, T w2, T* out, int maxit, void* ws, double* scratch, cudaStream_t st,
                     bool plain_transposes);
 
+// aux, aux_gen: the lane engine's scratch and its allocation count -- a regrown scratch can reuse the address with another layout
+// (records after a larger counter region), which the kernel arguments baked into the graph would not follow
 struct DrGraphKey {
-    size_t tsize, M, N; const void* Y; void* out; void* ws; double w1, w2; int maxit; const void* aux;      // aux: the lane engine's scratch
+    size_t tsize, M, N; const void* Y; void* out; void* ws; double w1, w2; int maxit; const void* aux; unsigned long long aux_gen;
     bool operator==(const DrGraphKey& o) const {
         return tsize == o.tsize && M == o.M && N == o.N && Y == o.Y && out == o.out && ws == o.ws && w1 == o.w1 && w2 == o.w2 &&
-               maxit == o.maxit && aux == o.aux;
+               maxit == o.maxit && aux == o.aux && aux_gen == o.aux_gen;
     }
 };
 struct DrGraph { cudaGraphExec_t exec = nullptr; DrGraphKey key{}; long long launches[KC_COUNT] = {0, 0, 0}; };
@@ -330,7 +332,7 @@ int dr2_device(size_t M, size_t N, int batch, int row_major, const T* Y, T w1, T
                           : dr2_piped_body<T>(M, N, Y, w1, w2, out, maxit, t, s, x, scr, scratch, gc, n, eng == ENGINE_AUTO && sizeof(T) == 8, bs);
         };
         DrGraphKey key{sizeof(T) + (tspace ? 100u : 0u) + (tpose ? 200u : 0u) + (eng == ENGINE_AUTO ? 400u : 0u) + (lane ? 800u : 0u) + (lane && lane_t ? 50u : 0u) + (row_major ? 25u : 0u) + 1000u * (size_t)batch, M, N, (const void*)Y, (void*)out, ws, (double)w1,
-                       (double)w2, maxit, lane ? lscr : nullptr};
+                       (double)w2, maxit, lane ? lscr : nullptr, lane ? ptvl::lane_scratch_generation() : 0ull};
         int rc = -1;
         if (!profile_is_enabled()) {
             DrGraph& G = g_dr_graph;

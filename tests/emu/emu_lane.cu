@@ -2,7 +2,7 @@
 // scan steps, window management, sweep, chunk records, verification and repair) on the CPU, one warp task at a time, the 32
 // lanes of a warp in a plain loop (lanes only interact through the warp collectives, which the host Env computes over the
 // loop).  Feed and Drain are the host stand-ins of the kernel's TMA feeder / row drain: same window contents, same calls.
-// Not part of the product; built by tests/test_lane_emulation.py with g++ (host code only; the CUDA headers only supply the
+// Not part of the product; built by tests/lane_emu.py with g++ (host code only; the CUDA headers only supply the
 // __host__ __device__ macros).
 #include "../../proxtv_b200/csrc/lane_core.cuh"
 #include <vector>
@@ -156,6 +156,18 @@ static int run_all(int opkind, const T* A, const T* B, const T* C, T* X, T* X2, 
     return 0;
 }
 
+// the same scan over every fiber of the (nf, len, inc) slicing rule (inc == 1: fiber j is in[j * len ..]; inc > 1: fiber j = (slab s,
+// column c) has sample r at (s * inc * len) + r * inc + c) -- the sequential reference of the lane engine's output, whatever its chunking,
+// windowing or repairs.  The float32 form reads float, scans in double (as the kernel does) and rounds the results to float.
+template <typename T>
+static void slope_fibers(const T* in, T* out, long long nf, int len, long long inc, T lam) {
+    for (long long j = 0; j < nf; j++) {
+        const long long base = inc > 1 ? (j / inc) * inc * len + j % inc : j * (long long)len, st = inc > 1 ? inc : 1;
+        slope_seq<T>(len, lam, 0, LK_BEGIN, [&](int i) { return in[base + (long long)i * st]; },
+                     [&](int f, int e, T v, int) { for (int r = f; r <= e; r++) out[base + (long long)r * st] = v; return false; });
+    }
+}
+
 extern "C" {
 // config: 0 -> W=64,TITER=16,R=8 ; 1 -> W=32,TITER=8,R=8 ; 2 -> W=128,TITER=16,R=16 (float) ...
 int emu_lane_f64(int opkind, const double* A, const double* B, const double* C, double* X, double* X2, long long nf, int len, long long inc,
@@ -205,4 +217,6 @@ void emu_slope_seq_f64(const double* y, int n, double lam, double* x, long long*
                       [&](int f, int e, double v, int) { for (int r = f; r <= e; r++) x[r] = v; return false; });
     if (steps) *steps = st;
 }
+void emu_slope_fibers_f64(const double* in, double* out, long long nf, int len, long long inc, double lam) { slope_fibers<double>(in, out, nf, len, inc, lam); }
+void emu_slope_fibers_f32(const float* in, float* out, long long nf, int len, long long inc, float lam) { slope_fibers<float>(in, out, nf, len, inc, lam); }
 }

@@ -10,37 +10,17 @@ repair path takes over), the boxed drain of the contiguous layout, partial fiber
 alternating / integer-valued data, lambda from 0 to 1e4, float32 storage, and the fused Douglas-Rachford pass arithmetic driven
 through a complete DR2_TV solve against the oracle."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-EMU_DIR = os.path.join(HERE, "emu")
-dp = C.POINTER(C.c_double)
-fp = C.POINTER(C.c_float)
+import lane_emu
+from lane_emu import dp, fp, slope_fibers
 
 
 @pytest.fixture(scope="module")
 def emu():
-    so = os.path.join(EMU_DIR, "libptv_emu_lane.so")
-    src = os.path.join(EMU_DIR, "emu_lane.cu")
-    core = os.path.join(HERE, "..", "proxtv_b200", "csrc", "lane_core.cuh")
-    if not os.path.exists(so) or any(os.path.getmtime(f) > os.path.getmtime(so) for f in (src, core)):
-        cuda_inc = "/usr/local/cuda/include"
-        if not os.path.isdir(cuda_inc):
-            pytest.skip("CUDA headers not available")
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-I" + cuda_inc, "-fPIC", "-ffp-contract=off", "-shared", "-x", "c++", src, "-o", so])
-    lib = C.CDLL(so)
-    lib.emu_lane_f64.argtypes = [C.c_int, dp, dp, dp, dp, dp, C.c_longlong, C.c_int, C.c_longlong, C.c_double, C.c_int, C.c_int, C.c_int, C.c_int,
-                                 C.POINTER(C.c_longlong)]
-    lib.emu_lane_f32.argtypes = [C.c_int, fp, fp, fp, fp, fp, C.c_longlong, C.c_int, C.c_longlong, C.c_float, C.c_int, C.c_int, C.c_int, C.c_int,
-                                 C.POINTER(C.c_longlong)]
-    lib.emu_slope_seq_f64.argtypes = [dp, C.c_int, C.c_double, dp, C.POINTER(C.c_longlong)]
-    lib.emu_plan.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
-    lib.emu_taskplan.argtypes = [C.c_int, C.c_longlong, C.c_longlong]; lib.emu_taskplan.restype = C.c_longlong
-    return lib
+    return lane_emu.load()
 
 
 def _p(a, t=dp):
@@ -222,3 +202,32 @@ def test_transposed_result_ops(emu, port):
     u = lane(emu, 3, A, Bv, Cv, M, N, M, 0.3, clen=32, halo=16, X2=X2)[0]
     d = Cv - x
     assert np.array_equal(X2, T(d)) and np.array_equal(u, T(Bv - (2.0 * d - Cv)))
+
+
+def test_lane_output_is_the_sequential_scan_bit_for_bit(emu):
+    """The lane engine's output is a pure function of its input: whatever the window (32 / 64 / 128 rows), the epoch length, the
+    chunking, the halo (0: every chunk boundary is repaired), the drain (direct or boxed) or the layout, every fiber equals the plain
+    sequential slope-form scan of that fiber (emu_slope_fibers_*) BIT FOR BIT, in float64 and in float32 storage (scanned in double,
+    rounded once).  This is the bar the GPU tests of the lane kernels (test_gpu_lane.py) hold the device code to."""
+    rng = np.random.default_rng(21)
+    nf, ln = 70, 300                                          # a partial last fiber group; chunks of 32..64 rows
+    blocks = np.repeat(rng.normal(0, 1, (nf, ln // 16 + 1)), 16, axis=1)[:, :ln] + rng.normal(0, 0.3, (nf, ln))
+    ties = np.round(rng.normal(0, 3, (nf, ln)))
+    ramp = np.tile(np.linspace(-3, 3, ln), (nf, 1)) + rng.normal(0, 0.01, (nf, 1))
+    plateau = rng.normal(0, 1, (nf, ln)); plateau[:, 60:250] = 0.3
+    repairs = 0
+    for dt in (np.float64, np.float32):
+        for data, lam in ((blocks, 0.2), (ties, 1.0), (ramp, 5.0), (plateau, 0.5), (blocks, 50.0)):
+            lam = dt(lam)
+            for inc in (nf, 1):                               # fibers adjacent in memory / contiguous fibers
+                A = np.ascontiguousarray((data.T if inc > 1 else data).astype(dt)).ravel()
+                want = slope_fibers(emu, A, nf, ln, inc, lam)
+                for cfg in (0, 1, 2):
+                    for clen, halo in ((0, 32), (64, 32), (48, 16), (32, 8), (64, 0)):
+                        for boxed in (0, 1):
+                            X, st = lane(emu, 0, A, None, None, nf, ln, inc, lam, clen=clen, halo=halo, boxed=boxed, config=cfg)
+                            assert np.array_equal(X, want), (dt.__name__, float(lam), inc, cfg, clen, halo, boxed)
+                            if clen and halo == 0:
+                                assert st["repairs"] >= nf
+                            repairs += st["repairs"]
+    assert repairs > 10000                                    # the repair path was exercised, not just the fast path
