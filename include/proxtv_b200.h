@@ -119,6 +119,20 @@ int proxtv_prox_fibers_dev_f64(const double *in, double *out, long long nf, int 
                                const double *lamv, void *stream);
 int proxtv_prox_fibers_dev_f32(const float *in, float *out, long long nf, int len, long long inc, float lam,
                                const float *lamv, void *stream);
+/* Backward pass (vector-Jacobian product) of proxtv_prox_fibers_dev_*: y = the forward's output, g = the upstream gradient, gx = the
+ * gradient with respect to the input, all laid out like the fibers; gw (may be NULL) = the gradient with respect to the per-edge
+ * weights, laid out like lamv (len-1 samples per fiber; with lamv == NULL its sum over a fiber is the gradient of lam).  Exactly,
+ * per fiber, in double and rounded once when stored: edge e is fused iff y[e] == y[e+1] and its weight (lamv[e], or lam) is > 0;
+ * every sample gets the mean of g over its run of fused edges, summed left to right from 0.0; gw[e] = sgn(y[e+1] - y[e]) *
+ * (gx[e] - gx[e+1]) on unfused edges, +0 on fused ones.  The result does not depend on how the work is split.  Outputs must not
+ * overlap inputs (not checked).  Returns 1 ok / 0 error; refused without writing anything: nf < 0, len < 0, inc < 1, y, g or gx
+ * NULL, lamv == NULL with lam < 0.  nf == 0 or len == 0: returns 1, does nothing. */
+int proxtv_prox_fibers_vjp_dev_f64(const double *y, const double *g, double *gx, double *gw, long long nf, int len, long long inc,
+                                   double lam, const double *lamv, void *stream);
+int proxtv_prox_fibers_vjp_dev_f32(const float *y, const float *g, float *gx, float *gw, long long nf, int len, long long inc,
+                                   float lam, const float *lamv, void *stream);
+/* tests: chunk length of the backward pass's work split (0 = automatic; whole fibers when it is >= len) */
+void proxtv_vjp_tuning(int chunk_len);
 /* host-pointer form of the above (pageable or pinned memory); synchronous. */
 int proxtv_prox_fibers_f64(const double *in, double *out, long long nf, int len, long long inc, double lam,
                            const double *lamv);

@@ -8,7 +8,8 @@ device the calls raise.
 
 Extensions the reference lacks (SURVEY.md section 8b): a leading batch dimension (``tv1_1d_batched``,
 ``tv1w_1d_batched``, ``tv1_2d_batched``), float32, and torch CUDA tensors as inputs (device-resident path: no PCIe
-traffic, no host transposes -- a C-ordered tensor is handled by swapping the kernels' stride roles).
+traffic, no host transposes -- a C-ordered tensor is handled by swapping the kernels' stride roles).  The batched 1D functions
+are differentiable on torch tensors (exact backward kernel, ``tv1_1d_batched``).
 """
 import ctypes as C
 
@@ -26,7 +27,7 @@ ENGINES = {"auto": 0, "seq": 1, "chunked": 2, "chunked-strided": 3, "pipelined":
 
 def set_engine(name):
     """Select the kernel family / DR schedule ('auto' | 'seq' | 'chunked' | 'chunked-strided' | 'pipelined' | 'tspace' |
-    'tpose', see include/proxtv_b200.h); returns the previous one.  Only measurements and tests need this."""
+    'tpose' | 'lane' | 'lane-t', see include/proxtv_b200.h); returns the previous one.  Only measurements and tests need this."""
     prev = load().proxtv_set_engine(ENGINES[name])
     return [k for k, v in ENGINES.items() if v == prev][0]
 
@@ -168,8 +169,72 @@ def tv1w_1d(x, w, method="tautstring", sigma=0.05):
     return y
 
 
+def _prox_rows_torch(xt, w, wt):
+    """The device prox of every row of the contiguous float32/float64 CUDA tensor xt (B, L); penalty w, or weights wt (B, L-1)."""
+    import torch
+    out = torch.empty_like(xt)
+    B, L = xt.shape
+    lib = require_device()
+    st = C.c_void_p(torch.cuda.current_stream(xt.device).cuda_stream)
+    fn = lib.proxtv_prox_fibers_dev_f32 if xt.dtype == torch.float32 else lib.proxtv_prox_fibers_dev_f64
+    with torch.cuda.device(xt.device):
+        _check(fn(C.c_void_p(xt.data_ptr()), C.c_void_p(out.data_ptr()), B, L, 1, float(w),
+                  C.c_void_p(wt.data_ptr()) if wt is not None else None, st), "batched 1D prox")
+    return out
+
+
+_PROX_ROWS_FN = None
+
+
+def _prox_rows_fn():
+    """torch.autograd.Function around _prox_rows_torch (made on first use, so that numpy users never import torch).
+
+    forward(x, w, w_t, wt): x (B, L) contiguous, w the penalty as a float, w_t the 0-dim tensor it came from (or None; only receives
+    the gradient), wt (B, L-1) weights or None.  backward: proxtv_prox_fibers_vjp_dev_* on the current stream -- gx = segment means of
+    the upstream gradient, gw per edge; the gradient of w_t is gw summed in float64."""
+    global _PROX_ROWS_FN
+    if _PROX_ROWS_FN is not None:
+        return _PROX_ROWS_FN
+    import torch
+    from torch.autograd.function import once_differentiable
+
+    class ProxRows(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, x, w, w_t, wt):
+            y = _prox_rows_torch(x, w, wt)
+            ctx.save_for_backward(y, wt)
+            ctx.w = w
+            ctx.w_t_meta = (w_t.dtype, w_t.device) if w_t is not None else None
+            return y
+
+        @staticmethod
+        @once_differentiable
+        def backward(ctx, gy):
+            y, wt = ctx.saved_tensors
+            need_x, _, need_wt_scalar, need_wt = ctx.needs_input_grad
+            B, L = y.shape
+            g = gy.to(dtype=y.dtype).contiguous()
+            gx = torch.empty_like(y)
+            gw = torch.empty((B, max(L - 1, 0)), dtype=y.dtype, device=y.device) if (need_wt_scalar or need_wt) else None
+            lib = require_device()
+            st = C.c_void_p(torch.cuda.current_stream(y.device).cuda_stream)
+            fn = lib.proxtv_prox_fibers_vjp_dev_f32 if y.dtype == torch.float32 else lib.proxtv_prox_fibers_vjp_dev_f64
+            with torch.cuda.device(y.device):
+                _check(fn(C.c_void_p(y.data_ptr()), C.c_void_p(g.data_ptr()), C.c_void_p(gx.data_ptr()),
+                          C.c_void_p(gw.data_ptr()) if gw is not None else None, B, L, 1, ctx.w,
+                          C.c_void_p(wt.data_ptr()) if wt is not None else None, st), "batched 1D prox backward")
+            g_scalar = None
+            if need_wt_scalar:
+                w_t = ctx.w_t_meta
+                g_scalar = gw.sum(dtype=torch.float64).to(dtype=w_t[0], device=w_t[1]).reshape(())
+            return (gx if need_x else None), None, g_scalar, (gw if need_wt else None)
+
+    _PROX_ROWS_FN = ProxRows
+    return ProxRows
+
+
 def _batched_1d(x, w, weights):
-    """x: (B, L) numpy array or torch CUDA tensor, row-contiguous signals."""
+    """x: (B, L) numpy array or torch CUDA tensor, row-contiguous signals.  w: float, or (torch path) a 0-dim tensor."""
     if _is_torch(x):
         import torch
         assert x.is_cuda and x.dim() == 2
@@ -177,19 +242,17 @@ def _batched_1d(x, w, weights):
         f32 = xt.dtype == torch.float32
         if not f32 and xt.dtype != torch.float64:
             xt = xt.double()
-        out = torch.empty_like(xt)
         B, L = xt.shape
         wt = None
         if weights is not None:
             wt = weights.to(dtype=xt.dtype, device=xt.device).contiguous()
             assert tuple(wt.shape) == (B, L - 1)
-        lib = require_device()
-        st = C.c_void_p(torch.cuda.current_stream(xt.device).cuda_stream)
-        fn = lib.proxtv_prox_fibers_dev_f32 if f32 else lib.proxtv_prox_fibers_dev_f64
-        with torch.cuda.device(xt.device):
-            _check(fn(C.c_void_p(xt.data_ptr()), C.c_void_p(out.data_ptr()), B, L, 1, float(w),
-                      C.c_void_p(wt.data_ptr()) if wt is not None else None, st), "batched 1D prox")
-        return out
+        w_t = w if _is_torch(w) else None
+        wf = float(w_t.detach()) if w_t is not None else float(w)
+        if torch.is_grad_enabled() and (xt.requires_grad or (wt is not None and wt.requires_grad)
+                                        or (w_t is not None and w_t.requires_grad)):
+            return _prox_rows_fn().apply(xt, wf, w_t, wt)
+        return _prox_rows_torch(xt, wf, wt)
     x = np.asarray(x)
     assert x.ndim == 2
     f32 = x.dtype == np.float32
@@ -209,13 +272,23 @@ def _batched_1d(x, w, weights):
 
 
 def tv1_1d_batched(x, w):
-    """``tv1_1d`` on every row of a (B, L) array (numpy float64/float32, or a torch CUDA tensor)."""
+    """``tv1_1d`` on every row of a (B, L) array (numpy float64/float32, or a torch CUDA tensor).
+
+    torch: differentiable.  With grad mode on and ``x`` or ``w`` requiring grad, the result carries a ``grad_fn`` whose backward is the
+    exact vector-Jacobian product of the prox (proxtv_prox_fibers_vjp_dev_*: every sample gets the mean of the upstream gradient over
+    its constant segment), run on the current CUDA stream; double backward is not supported.  ``w`` may be a float or a 0-dim tensor;
+    a tensor's gradient is the sum of the per-edge gradients, accumulated in float64.  The forward result is the same either way.
+    """
     assert w >= 0
-    return _batched_1d(x, float(w), None)
+    return _batched_1d(x, w if _is_torch(w) else float(w), None)
 
 
 def tv1w_1d_batched(x, w):
-    """``tv1w_1d`` on every row of x (B, L) with per-edge weights w (B, L-1)  -- BASELINE config 3."""
+    """``tv1w_1d`` on every row of x (B, L) with per-edge weights w (B, L-1)  -- BASELINE config 3.
+
+    torch: differentiable with respect to ``x`` and the weights tensor ``w`` (see ``tv1_1d_batched``); a zero weight never fuses its
+    edge, so its gradient is the signed difference of the two sides' gradients like any other edge between segments.
+    """
     return _batched_1d(x, 0.0, w)
 
 

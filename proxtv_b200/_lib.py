@@ -43,6 +43,9 @@ SIGNATURES = {
     "proxtv_set_engine": (C.c_int, [C.c_int]),
     "proxtv_prox_fibers_dev_f64": (C.c_int, [_vp, _vp, C.c_longlong, C.c_int, C.c_longlong, C.c_double, _vp, _vp]),
     "proxtv_prox_fibers_dev_f32": (C.c_int, [_vp, _vp, C.c_longlong, C.c_int, C.c_longlong, C.c_float, _vp, _vp]),
+    "proxtv_prox_fibers_vjp_dev_f64": (C.c_int, [_vp, _vp, _vp, _vp, C.c_longlong, C.c_int, C.c_longlong, C.c_double, _vp, _vp]),
+    "proxtv_prox_fibers_vjp_dev_f32": (C.c_int, [_vp, _vp, _vp, _vp, C.c_longlong, C.c_int, C.c_longlong, C.c_float, _vp, _vp]),
+    "proxtv_vjp_tuning": (None, [C.c_int]),
     "proxtv_prox_fibers_f64": (C.c_int, [_vp, _vp, C.c_longlong, C.c_int, C.c_longlong, C.c_double, _vp]),
     "proxtv_prox_fibers_f32": (C.c_int, [_vp, _vp, C.c_longlong, C.c_int, C.c_longlong, C.c_float, _vp]),
     "proxtv_DR2_TV_dev_f64": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, C.c_int, _vp, C.c_double, C.c_double, _vp, C.c_int, _vp, _vp]),

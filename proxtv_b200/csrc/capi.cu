@@ -192,6 +192,22 @@ template <typename T> static T* dev_scratch(long long nf, int len, long long inc
     return (T*)g_ws.get(al((size_t)strided_scratch_elems(nf, len) * sizeof(T)));
 }
 
+// Backward pass of proxtv_prox_fibers_dev_*: refused calls write nothing; the scratch (chunked work only) comes from the workspace.
+template <typename T>
+static int dev_vjp(const char* fn, const T* y, const T* g, T* gx, T* gw, long long nf, int len, long long inc, T lam, const T* lamv,
+                   void* stream) {
+    if (nf < 0 || len < 0 || inc < 1) { fail(fn, "invalid fiber geometry (need nf >= 0, len >= 0, inc >= 1)", nullptr); return 0; }
+    if (nf == 0 || len == 0) return 1;
+    if (!y || !g || !gx) { fail(fn, "NULL array", nullptr); return 0; }
+    if (!lamv && !(lam >= 0)) { fail(fn, "negative penalty", nullptr); return 0; }
+    if (!have_device(fn, nullptr)) return 0;
+    WsGuard guard((cudaStream_t)stream);
+    const size_t sb = ptvv::vjp_scratch_bytes(nf, len);
+    void* scr = sb ? g_ws.get(sb) : nullptr;
+    if (sb && !scr) { fail(fn, "out of device memory", nullptr); return 0; }
+    return cuda_ok(fn, ptvv::vjp_fibers<T>(y, g, gx, gw, nf, len, inc, lam, lamv, scr, (cudaStream_t)stream), nullptr);
+}
+
 template <typename T>
 static int dev_dr2(const char* fn, size_t M, size_t N, int batch, int row_major, const T* Y, T W1, T W2, T* out, int maxit, double* info, void* stream) {
     if (!have_device(fn, info)) return 0;
@@ -342,6 +358,15 @@ int proxtv_prox_fibers_dev_f32(const float* in, float* out, long long nf, int le
     return cuda_ok("proxtv_prox_fibers_dev_f32", prox_fibers<float>(in, nullptr, IN_A, out, 0, FiberGeom{nf, len, inc}, lam, lamv, eng, dev_scratch<float>(nf, len, inc), (cudaStream_t)stream,
                                                                  (inc == 1 && len > 16384) ? lf_scratch_elems(nf, len) : (inc != 1 ? strided_scratch_elems(nf, len) : 0)), nullptr);
 }
+int proxtv_prox_fibers_vjp_dev_f64(const double* y, const double* g, double* gx, double* gw, long long nf, int len, long long inc, double lam,
+                                   const double* lamv, void* stream) {
+    return dev_vjp<double>("proxtv_prox_fibers_vjp_dev_f64", y, g, gx, gw, nf, len, inc, lam, lamv, stream);
+}
+int proxtv_prox_fibers_vjp_dev_f32(const float* y, const float* g, float* gx, float* gw, long long nf, int len, long long inc, float lam,
+                                   const float* lamv, void* stream) {
+    return dev_vjp<float>("proxtv_prox_fibers_vjp_dev_f32", y, g, gx, gw, nf, len, inc, lam, lamv, stream);
+}
+void proxtv_vjp_tuning(int chunk_len) { ptvv::vjp_set_tuning(chunk_len); }
 int proxtv_prox_fibers_f64(const double* in, double* out, long long nf, int len, long long inc, double lam, const double* lamv) {
     return host_prox_fibers<double>("proxtv_prox_fibers_f64", in, out, nf, len, inc, lam, lamv);
 }

@@ -129,3 +129,15 @@ void lane_set_tuning(int clen, int halo, int variant);
 void lane_set_tasklog(unsigned long long* dev, long long cap_tasks);
 unsigned long long lane_read_stats(int reset);
 }  // namespace ptvl
+
+// ---- backward pass of the batched 1D prox (vjp.cu, contract in vjp_core.cuh) ----
+namespace ptvv {
+// gx (and gw unless nullptr) from the forward output y and the upstream gradient g over the fibers (nf, len, inc); weights as in
+// prox_fibers.  scratch: vjp_scratch_bytes(nf, len) bytes (0: none needed).  Outputs must not overlap inputs.
+template <typename T>
+cudaError_t vjp_fibers(const T* y, const T* g, T* gx, T* gw, long long nf, int len, long long inc, T lam, const T* lamv, void* scratch,
+                       cudaStream_t st);
+size_t vjp_scratch_bytes(long long nf, int len);
+int vjp_chunk_len(long long nf, int len);
+void vjp_set_tuning(int clen);
+}  // namespace ptvv
