@@ -133,6 +133,22 @@ int proxtv_prox_fibers_vjp_dev_f32(const float *y, const float *g, float *gx, fl
                                    float lam, const float *lamv, void *stream);
 /* tests: chunk length of the backward pass's work split (0 = automatic; whole fibers when it is >= len) */
 void proxtv_vjp_tuning(int chunk_len);
+/* Segmentation tape of y (the forward's output) over the fibers (nf, len, inc), nf a multiple of inc: what the backward pass above
+ * needs of y, in 2 bits per element.  F and U are bitsets over the nf * len elements in storage order, ceil(nf * len / 32) uint32
+ * words each (bit i: word i / 32, bit i % 32), the words up to the next multiple of 256 bytes written as 0.  Bit i describes element
+ * i and its successor i + inc along its fiber: (F, U) = (1, 0) fused (equal as stored and weight > 0), (0, 1) the successor is
+ * greater, (0, 0) it is smaller -- also every fiber's last sample --, (1, 1) equal with a zero weight (not fused, sign 0).  Refused
+ * without writing anything: nf < 0, len < 0, inc < 1, nf not a multiple of inc, y, F or U NULL, lamv == NULL with lam < 0. */
+int proxtv_fiber_tape_dev_f64(const double *y, long long nf, int len, long long inc, double lam, const double *lamv, unsigned *F,
+                              unsigned *U, void *stream);
+int proxtv_fiber_tape_dev_f32(const float *y, long long nf, int len, long long inc, float lam, const float *lamv, unsigned *F,
+                              unsigned *U, void *stream);
+/* proxtv_prox_fibers_vjp_dev_* driven by a tape instead of (y, lam, lamv): given the tape of (y, lam, lamv), the same gx and gw bit
+ * for bit.  Refusals as above (F, U, g or gx NULL; nf not a multiple of inc). */
+int proxtv_prox_fibers_vjp_tape_dev_f64(const unsigned *F, const unsigned *U, const double *g, double *gx, double *gw, long long nf,
+                                        int len, long long inc, void *stream);
+int proxtv_prox_fibers_vjp_tape_dev_f32(const unsigned *F, const unsigned *U, const float *g, float *gx, float *gw, long long nf,
+                                        int len, long long inc, void *stream);
 /* host-pointer form of the above (pageable or pinned memory); synchronous. */
 int proxtv_prox_fibers_f64(const double *in, double *out, long long nf, int len, long long inc, double lam,
                            const double *lamv);
@@ -146,6 +162,25 @@ int proxtv_DR2_TV_dev_f64(size_t M, size_t N, int batch, int row_major, const do
                           double *info, void *stream);
 int proxtv_DR2_TV_dev_f32(size_t M, size_t N, int batch, int row_major, const float *Y, float W1, float W2, float *out, int maxit,
                           double *info, void *stream);
+/* Exact backward pass of DR2_TV (DESIGN.md section 11).  The gradient is the one of the function computed: the lane engine's fixed
+ * schedule of K = maxit iterations (0: 35) and the final projection, every prox pass with the Jacobian of proxtv_prox_fibers_vjp_dev_*.
+ * record: DR2_TV as proxtv_DR2_TV_dev_* computes it (bit for bit whenever that call takes a lane schedule; within rounding
+ * otherwise), with plain prox passes, writing into the device buffer `tape` (at least proxtv_DR2_TV_tape_bytes() bytes) a 256-byte
+ * header and the segmentation tapes (proxtv_fiber_tape_dev_*) of the 2K + 1 passes after the first column pass.  Returns 1 ok / 0
+ * error (info[2] = 3 too); refused without writing anything: M, N or batch < 1, Y, out or tape NULL, a negative weight, tape_bytes
+ * too small.  vjp: from the tape alone, gY = the gradient with respect to Y for the upstream gradient gout (both laid out like out)
+ * and, unless glam is NULL, glam = 2 * batch doubles, per image [W1, W2] -- the gradients of the two penalties.  Deterministic (no
+ * atomics); synchronises the stream once (reads the tape's header).  Returns 1 ok / 0 error; refused without writing anything: M, N
+ * or batch < 1, tape, gout or gY NULL, a header that does not match the arguments (dtype, shape, batch, row_major, maxit). */
+size_t proxtv_DR2_TV_tape_bytes(size_t M, size_t N, int batch, int maxit);
+int proxtv_DR2_TV_record_dev_f64(size_t M, size_t N, int batch, int row_major, const double *Y, double W1, double W2, double *out,
+                                 int maxit, void *tape, size_t tape_bytes, double *info, void *stream);
+int proxtv_DR2_TV_record_dev_f32(size_t M, size_t N, int batch, int row_major, const float *Y, float W1, float W2, float *out,
+                                 int maxit, void *tape, size_t tape_bytes, double *info, void *stream);
+int proxtv_DR2_TV_vjp_dev_f64(size_t M, size_t N, int batch, int row_major, int maxit, const void *tape, const double *gout,
+                              double *gY, double *glam, void *stream);
+int proxtv_DR2_TV_vjp_dev_f32(size_t M, size_t N, int batch, int row_major, int maxit, const void *tape, const float *gout,
+                              float *gY, double *glam, void *stream);
 int proxtv_DR2_TV_batched_f64(size_t M, size_t N, int batch, const double *Y, double W1, double W2, double *out, int maxit,
                               double *info);
 int proxtv_DR2_TV_batched_f32(size_t M, size_t N, int batch, const float *Y, float W1, float W2, float *out, int maxit,

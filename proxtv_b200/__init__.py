@@ -9,7 +9,7 @@ device the calls raise.
 Extensions the reference lacks (SURVEY.md section 8b): a leading batch dimension (``tv1_1d_batched``,
 ``tv1w_1d_batched``, ``tv1_2d_batched``), float32, and torch CUDA tensors as inputs (device-resident path: no PCIe
 traffic, no host transposes -- a C-ordered tensor is handled by swapping the kernels' stride roles).  The batched 1D functions
-are differentiable on torch tensors (exact backward kernel, ``tv1_1d_batched``).
+and ``tv1_2d`` / ``tv1_2d_batched`` are differentiable on torch tensors (exact backward kernels).
 """
 import ctypes as C
 
@@ -306,6 +306,11 @@ def tv1_2d(x, w, n_threads=1, max_iters=0, method="dr"):
     reference methods are slower CPU baselines for the same problem and are not provided.  ``n_threads`` is ignored.
     numpy input: returns a Fortran-ordered float64 array like the reference.  torch CUDA tensor input (2D, float64 or
     float32): stays on the device and returns a tensor of the same dtype/layout.
+
+    torch: differentiable with respect to ``x`` and ``w`` given as a 0-dim tensor.  With grad mode on and one of them requiring
+    grad, the forward records a segmentation tape of every prox pass (2 bits per element per pass, kept on the device until the
+    backward) and the backward is the exact vector-Jacobian product of the fixed 35-iteration splitting that is computed
+    (proxtv_DR2_TV_vjp_dev_*, DESIGN.md section 11), run on the current CUDA stream; double backward is not supported.
     """
     assert w >= 0
     assert method in _TV1_2D_METHODS
@@ -313,7 +318,7 @@ def tv1_2d(x, w, n_threads=1, max_iters=0, method="dr"):
         raise NotImplementedError("proxtv_b200 implements the 'dr' and 'pd' 2D solvers (the GPU hot path); got %r" % method)
     if _is_torch(x):
         assert method == "dr", "torch path implements the DR solver"
-        return _dr2_torch(x, float(w), max_iters, batched=False)
+        return _dr2_torch_entry(x, w, max_iters, batched=False)
     x = np.asfortranarray(x, dtype="float64")
     assert x.ndim == 2
     w = force_float_scalar(w)
@@ -379,7 +384,9 @@ def _drw_torch(x, w_col, w_row, max_iters):
     return out.t()
 
 
-def _dr2_torch(x, w, max_iters, batched):
+def _dr2_layout(x, batched):
+    """(M, N, batch, row_major, xin) of a 2D / batched 3D CUDA tensor: either memory order of the trailing two dims is taken as it
+    is, anything else is copied to C order."""
     import torch
     assert x.is_cuda and x.dtype in (torch.float64, torch.float32)
     assert x.dim() == (3 if batched else 2)
@@ -392,6 +399,12 @@ def _dr2_torch(x, w, max_iters, batched):
         row_major, xin = 0, x
     else:
         row_major, xin = 1, x.contiguous()
+    return M, N, batch, row_major, xin
+
+
+def _dr2_torch(x, w, max_iters, batched):
+    import torch
+    M, N, batch, row_major, xin = _dr2_layout(x, batched)
     out = torch.empty_strided(xin.shape, xin.stride(), dtype=xin.dtype, device=xin.device)
     info = np.zeros(_N_INFO)
     lib = require_device()
@@ -404,15 +417,88 @@ def _dr2_torch(x, w, max_iters, batched):
     return out
 
 
+_DR2_FN = None
+
+
+def _dr2_fn():
+    """torch.autograd.Function around DR2_TV on the device (made on first use, so that numpy users never import torch).
+
+    forward(x, w, w_t, max_iters, batched): proxtv_DR2_TV_record_dev_* -- the solve of _dr2_torch with the lane engine's schedule in
+    plain passes, keeping the segmentation tape of every prox pass (a uint8 CUDA tensor, proxtv_DR2_TV_tape_bytes() long) on ctx.
+    backward: proxtv_DR2_TV_vjp_dev_* on the current stream -- the exact vector-Jacobian product of the unrolled iteration; the
+    gradient of w_t is glam (per image and axis) summed in float64."""
+    global _DR2_FN
+    if _DR2_FN is not None:
+        return _DR2_FN
+    import torch
+    from torch.autograd.function import once_differentiable
+
+    class DR2(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, x, w, w_t, max_iters, batched):
+            M, N, batch, row_major, xin = _dr2_layout(x, batched)
+            lib = require_device()
+            out = torch.empty_strided(xin.shape, xin.stride(), dtype=xin.dtype, device=xin.device)
+            tape = torch.empty(int(lib.proxtv_DR2_TV_tape_bytes(M, N, batch, int(max_iters))), dtype=torch.uint8, device=xin.device)
+            info = np.zeros(_N_INFO)
+            st = C.c_void_p(torch.cuda.current_stream(xin.device).cuda_stream)
+            fn = lib.proxtv_DR2_TV_record_dev_f32 if xin.dtype == torch.float32 else lib.proxtv_DR2_TV_record_dev_f64
+            with torch.cuda.device(xin.device):
+                ok = fn(M, N, batch, row_major, C.c_void_p(xin.data_ptr()), w, w, C.c_void_p(out.data_ptr()), int(max_iters),
+                        C.c_void_p(tape.data_ptr()), tape.numel(), _ptr(info), st)
+            _check(ok, "DR2_TV (recorded, device)")
+            ctx.save_for_backward(tape)
+            ctx.geom = (M, N, batch, row_major, int(max_iters), tuple(out.shape), out.stride(), out.dtype)
+            ctx.w_t_meta = (w_t.dtype, w_t.device) if w_t is not None else None
+            return out
+
+        @staticmethod
+        @once_differentiable
+        def backward(ctx, gout):
+            (tape,) = ctx.saved_tensors
+            M, N, batch, row_major, max_iters, shape, stride, dt = ctx.geom
+            need_x, _, need_w_t, _, _ = ctx.needs_input_grad
+            dev = tape.device
+            g = torch.empty_strided(shape, stride, dtype=dt, device=dev)      # the upstream gradient in the output's layout
+            g.copy_(gout)
+            gY = torch.empty_strided(shape, stride, dtype=dt, device=dev)
+            glam = torch.empty(2 * batch, dtype=torch.float64, device=dev) if need_w_t else None
+            lib = require_device()
+            st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            fn = lib.proxtv_DR2_TV_vjp_dev_f32 if dt == torch.float32 else lib.proxtv_DR2_TV_vjp_dev_f64
+            with torch.cuda.device(dev):
+                _check(fn(M, N, batch, row_major, max_iters, C.c_void_p(tape.data_ptr()), C.c_void_p(g.data_ptr()),
+                          C.c_void_p(gY.data_ptr()), C.c_void_p(glam.data_ptr()) if glam is not None else None, st),
+                       "DR2_TV backward (device)")
+            g_w = None
+            if need_w_t:
+                g_w = glam.sum(dtype=torch.float64).to(dtype=ctx.w_t_meta[0], device=ctx.w_t_meta[1]).reshape(())
+            return (gY if need_x else None), None, g_w, None, None
+
+    _DR2_FN = DR2
+    return DR2
+
+
+def _dr2_torch_entry(x, w, max_iters, batched):
+    """The torch path of tv1_2d / tv1_2d_batched: differentiable when grad mode is on and x, or w given as a 0-dim tensor, requires
+    grad; otherwise exactly _dr2_torch."""
+    import torch
+    w_t = w if _is_torch(w) else None
+    wf = float(w_t.detach()) if w_t is not None else float(w)
+    if torch.is_grad_enabled() and (x.requires_grad or (w_t is not None and w_t.requires_grad)):
+        return _dr2_fn().apply(x, wf, w_t, max_iters, batched)
+    return _dr2_torch(x, wf, max_iters, batched)
+
+
 def tv1_2d_batched(x, w, max_iters=0):
     """``tv1_2d(method='dr')`` on every image of x (B, H, W)  -- BASELINE config 5.
 
     numpy: float64 or float32, C-ordered (B, H, W); torch: CUDA tensor (B, H, W).  Each image is solved independently with
-    exactly the single-image iteration (its own 2*mean initialisation).
+    exactly the single-image iteration (its own 2*mean initialisation).  torch: differentiable like ``tv1_2d``.
     """
     assert w >= 0
     if _is_torch(x):
-        return _dr2_torch(x, float(w), max_iters, batched=True)
+        return _dr2_torch_entry(x, w, max_iters, batched=True)
     x = np.asarray(x)
     assert x.ndim == 3
     f32 = x.dtype == np.float32

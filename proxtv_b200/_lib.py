@@ -46,12 +46,23 @@ SIGNATURES = {
     "proxtv_prox_fibers_vjp_dev_f64": (C.c_int, [_vp, _vp, _vp, _vp, C.c_longlong, C.c_int, C.c_longlong, C.c_double, _vp, _vp]),
     "proxtv_prox_fibers_vjp_dev_f32": (C.c_int, [_vp, _vp, _vp, _vp, C.c_longlong, C.c_int, C.c_longlong, C.c_float, _vp, _vp]),
     "proxtv_vjp_tuning": (None, [C.c_int]),
+    "proxtv_fiber_tape_dev_f64": (C.c_int, [_vp, C.c_longlong, C.c_int, C.c_longlong, C.c_double, _vp, _vp, _vp, _vp]),
+    "proxtv_fiber_tape_dev_f32": (C.c_int, [_vp, C.c_longlong, C.c_int, C.c_longlong, C.c_float, _vp, _vp, _vp, _vp]),
+    "proxtv_prox_fibers_vjp_tape_dev_f64": (C.c_int, [_vp, _vp, _vp, _vp, _vp, C.c_longlong, C.c_int, C.c_longlong, _vp]),
+    "proxtv_prox_fibers_vjp_tape_dev_f32": (C.c_int, [_vp, _vp, _vp, _vp, _vp, C.c_longlong, C.c_int, C.c_longlong, _vp]),
     "proxtv_prox_fibers_f64": (C.c_int, [_vp, _vp, C.c_longlong, C.c_int, C.c_longlong, C.c_double, _vp]),
     "proxtv_prox_fibers_f32": (C.c_int, [_vp, _vp, C.c_longlong, C.c_int, C.c_longlong, C.c_float, _vp]),
     "proxtv_DR2_TV_dev_f64": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, C.c_int, _vp, C.c_double, C.c_double, _vp, C.c_int, _vp, _vp]),
     "proxtv_DR2_TV_dev_f32": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, C.c_int, _vp, C.c_float, C.c_float, _vp, C.c_int, _vp, _vp]),
     "proxtv_DR2L1W_TV_dev_f64": (C.c_int, [C.c_size_t, C.c_size_t, _vp, _vp, _vp, _vp, C.c_int, _vp, _vp]),
     "proxtv_DR2L1W_TV_dev_f32": (C.c_int, [C.c_size_t, C.c_size_t, _vp, _vp, _vp, _vp, C.c_int, _vp, _vp]),
+    "proxtv_DR2_TV_tape_bytes": (C.c_size_t, [C.c_size_t, C.c_size_t, C.c_int, C.c_int]),
+    "proxtv_DR2_TV_record_dev_f64": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, C.c_int, _vp, C.c_double, C.c_double, _vp, C.c_int, _vp,
+                                               C.c_size_t, _vp, _vp]),
+    "proxtv_DR2_TV_record_dev_f32": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, C.c_int, _vp, C.c_float, C.c_float, _vp, C.c_int, _vp,
+                                               C.c_size_t, _vp, _vp]),
+    "proxtv_DR2_TV_vjp_dev_f64": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp]),
+    "proxtv_DR2_TV_vjp_dev_f32": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp]),
     "proxtv_DR2_TV_batched_f64": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, _vp, C.c_double, C.c_double, _vp, C.c_int, _vp]),
     "proxtv_DR2_TV_batched_f32": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, _vp, C.c_float, C.c_float, _vp, C.c_int, _vp]),
     "proxtv_PD2_TV_dev_f64": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, _vp]),

@@ -217,6 +217,65 @@ static int dev_dr2(const char* fn, size_t M, size_t N, int batch, int row_major,
     return dr2_device<T>(M, N, batch, row_major, Y, W1, W2, out, maxit, info, ws, (Engine)g_engine, (cudaStream_t)stream);
 }
 
+// Segmentation tape of y over the fibers (nf, len, inc) (nf a multiple of inc); refused calls write nothing.
+template <typename T>
+static int dev_tape(const char* fn, const T* y, long long nf, int len, long long inc, T lam, const T* lamv, uint32_t* F, uint32_t* U,
+                    void* stream) {
+    if (nf < 0 || len < 0 || inc < 1 || (nf > 0 && nf % inc != 0)) {
+        fail(fn, "invalid fiber geometry (need nf >= 0, len >= 0, inc >= 1, nf a multiple of inc)", nullptr); return 0; }
+    if (nf == 0 || len == 0) return 1;
+    if (!y || !F || !U) { fail(fn, "NULL array", nullptr); return 0; }
+    if (!lamv && !(lam >= 0)) { fail(fn, "negative penalty", nullptr); return 0; }
+    if (!have_device(fn, nullptr)) return 0;
+    WsGuard guard((cudaStream_t)stream);
+    return cuda_ok(fn, ptvv::fiber_tape<T>(y, nf, len, inc, lam, lamv, F, U, (cudaStream_t)stream), nullptr);
+}
+
+template <typename T>
+static int dev_vjp_tape(const char* fn, const uint32_t* F, const uint32_t* U, const T* g, T* gx, T* gw, long long nf, int len, long long inc,
+                        void* stream) {
+    if (nf < 0 || len < 0 || inc < 1 || (nf > 0 && nf % inc != 0)) {
+        fail(fn, "invalid fiber geometry (need nf >= 0, len >= 0, inc >= 1, nf a multiple of inc)", nullptr); return 0; }
+    if (nf == 0 || len == 0) return 1;
+    if (!F || !U || !g || !gx) { fail(fn, "NULL array", nullptr); return 0; }
+    if (!have_device(fn, nullptr)) return 0;
+    WsGuard guard((cudaStream_t)stream);
+    const size_t sb = ptvv::vjp_scratch_bytes(nf, len);
+    void* scr = sb ? g_ws.get(sb) : nullptr;
+    if (sb && !scr) { fail(fn, "out of device memory", nullptr); return 0; }
+    return cuda_ok(fn, ptvv::vjp_fibers_tape<T>(F, U, g, gx, gw, nf, len, inc, scr, (cudaStream_t)stream), nullptr);
+}
+
+template <typename T>
+static int dev_dr2_record(const char* fn, size_t M, size_t N, int batch, int row_major, const T* Y, T W1, T W2, T* out, int maxit, void* tape,
+                          size_t tape_bytes, double* info, void* stream) {
+    if (M < 1 || N < 1 || batch < 1) { fail(fn, "invalid shape (need M, N, batch >= 1)", info); return 0; }
+    if (!Y || !out || !tape) { fail(fn, "NULL array", info); return 0; }
+    if (!(W1 >= 0) || !(W2 >= 0)) { fail(fn, "negative penalty", info); return 0; }
+    if (tape_bytes < dr2_tape_bytes(M, N, batch, maxit)) { fail(fn, "tape_bytes smaller than proxtv_DR2_TV_tape_bytes()", info); return 0; }
+    if (!have_device(fn, info)) return 0;
+    WsGuard guard((cudaStream_t)stream);
+    void* ws = g_ws.get(ws_bytes_dr2_record<T>(M, N, batch));
+    if (!ws) { fail(fn, "out of memory", info); return 0; }
+    if (!cuda_ok(fn, dr2_record_device<T>(M, N, batch, row_major, Y, W1, W2, out, maxit, tape, ws, (Engine)g_engine, (cudaStream_t)stream), info))
+        return 0;
+    if (info) { info[INFO_ITERS] = maxit <= 0 ? MAX_ITERS_DR : maxit; info[INFO_RC] = RC_OK; }
+    return 1;
+}
+
+template <typename T>
+static int dev_dr2_vjp(const char* fn, size_t M, size_t N, int batch, int row_major, int maxit, const void* tape, const T* gout, T* gY,
+                       double* glam, void* stream) {
+    if (M < 1 || N < 1 || batch < 1) { fail(fn, "invalid shape (need M, N, batch >= 1)", nullptr); return 0; }
+    if (!tape || !gout || !gY) { fail(fn, "NULL array", nullptr); return 0; }
+    if (!have_device(fn, nullptr)) return 0;
+    WsGuard guard((cudaStream_t)stream);
+    if (const char* why = dr2_tape_check(tape, sizeof(T), M, N, batch, row_major, maxit, (cudaStream_t)stream)) { fail(fn, why, nullptr); return 0; }
+    void* ws = g_ws.get(ws_bytes_dr2_vjp<T>(M, N, batch));
+    if (!ws) { fail(fn, "out of memory", nullptr); return 0; }
+    return cuda_ok(fn, dr2_vjp_device<T>(M, N, batch, row_major, maxit, tape, gout, gY, glam, ws, (cudaStream_t)stream), nullptr);
+}
+
 }  // namespace
 
 extern "C" {
@@ -367,6 +426,22 @@ int proxtv_prox_fibers_vjp_dev_f32(const float* y, const float* g, float* gx, fl
     return dev_vjp<float>("proxtv_prox_fibers_vjp_dev_f32", y, g, gx, gw, nf, len, inc, lam, lamv, stream);
 }
 void proxtv_vjp_tuning(int chunk_len) { ptvv::vjp_set_tuning(chunk_len); }
+int proxtv_fiber_tape_dev_f64(const double* y, long long nf, int len, long long inc, double lam, const double* lamv, unsigned* F, unsigned* U,
+                              void* stream) {
+    return dev_tape<double>("proxtv_fiber_tape_dev_f64", y, nf, len, inc, lam, lamv, F, U, stream);
+}
+int proxtv_fiber_tape_dev_f32(const float* y, long long nf, int len, long long inc, float lam, const float* lamv, unsigned* F, unsigned* U,
+                              void* stream) {
+    return dev_tape<float>("proxtv_fiber_tape_dev_f32", y, nf, len, inc, lam, lamv, F, U, stream);
+}
+int proxtv_prox_fibers_vjp_tape_dev_f64(const unsigned* F, const unsigned* U, const double* g, double* gx, double* gw, long long nf, int len,
+                                        long long inc, void* stream) {
+    return dev_vjp_tape<double>("proxtv_prox_fibers_vjp_tape_dev_f64", F, U, g, gx, gw, nf, len, inc, stream);
+}
+int proxtv_prox_fibers_vjp_tape_dev_f32(const unsigned* F, const unsigned* U, const float* g, float* gx, float* gw, long long nf, int len,
+                                        long long inc, void* stream) {
+    return dev_vjp_tape<float>("proxtv_prox_fibers_vjp_tape_dev_f32", F, U, g, gx, gw, nf, len, inc, stream);
+}
 int proxtv_prox_fibers_f64(const double* in, double* out, long long nf, int len, long long inc, double lam, const double* lamv) {
     return host_prox_fibers<double>("proxtv_prox_fibers_f64", in, out, nf, len, inc, lam, lamv);
 }
@@ -378,6 +453,19 @@ int proxtv_DR2_TV_dev_f64(size_t M, size_t N, int batch, int row_major, const do
     return dev_dr2<double>("proxtv_DR2_TV_dev_f64", M, N, batch, row_major, Y, W1, W2, out, maxit, info, stream); }
 int proxtv_DR2_TV_dev_f32(size_t M, size_t N, int batch, int row_major, const float* Y, float W1, float W2, float* out, int maxit, double* info, void* stream) {
     return dev_dr2<float>("proxtv_DR2_TV_dev_f32", M, N, batch, row_major, Y, W1, W2, out, maxit, info, stream); }
+size_t proxtv_DR2_TV_tape_bytes(size_t M, size_t N, int batch, int maxit) { return batch < 1 ? 0 : dr2_tape_bytes(M, N, batch, maxit); }
+int proxtv_DR2_TV_record_dev_f64(size_t M, size_t N, int batch, int row_major, const double* Y, double W1, double W2, double* out, int maxit,
+                                 void* tape, size_t tape_bytes, double* info, void* stream) {
+    return dev_dr2_record<double>("proxtv_DR2_TV_record_dev_f64", M, N, batch, row_major, Y, W1, W2, out, maxit, tape, tape_bytes, info, stream); }
+int proxtv_DR2_TV_record_dev_f32(size_t M, size_t N, int batch, int row_major, const float* Y, float W1, float W2, float* out, int maxit,
+                                 void* tape, size_t tape_bytes, double* info, void* stream) {
+    return dev_dr2_record<float>("proxtv_DR2_TV_record_dev_f32", M, N, batch, row_major, Y, W1, W2, out, maxit, tape, tape_bytes, info, stream); }
+int proxtv_DR2_TV_vjp_dev_f64(size_t M, size_t N, int batch, int row_major, int maxit, const void* tape, const double* gout, double* gY,
+                              double* glam, void* stream) {
+    return dev_dr2_vjp<double>("proxtv_DR2_TV_vjp_dev_f64", M, N, batch, row_major, maxit, tape, gout, gY, glam, stream); }
+int proxtv_DR2_TV_vjp_dev_f32(size_t M, size_t N, int batch, int row_major, int maxit, const void* tape, const float* gout, float* gY,
+                              double* glam, void* stream) {
+    return dev_dr2_vjp<float>("proxtv_DR2_TV_vjp_dev_f32", M, N, batch, row_major, maxit, tape, gout, gY, glam, stream); }
 int proxtv_DR2_TV_batched_f64(size_t M, size_t N, int batch, const double* Y, double W1, double W2, double* out, int maxit, double* info) {
     return host_dr2<double>("proxtv_DR2_TV_batched_f64", M, N, batch, Y, W1, W2, out, maxit, info); }
 int proxtv_DR2_TV_batched_f32(size_t M, size_t N, int batch, const float* Y, float W1, float W2, float* out, int maxit, double* info) {

@@ -1,0 +1,313 @@
+// dr2_vjp.cu -- the exact backward pass of DR2_TV (DESIGN.md section 11): a recorded forward that writes the segmentation tape of every
+// prox pass, and the unrolled vector-Jacobian product driven by that tape.
+//
+// DR2_TV is a fixed, unconverged splitting (35 iterations and a final projection), so the gradient is the one of the function actually
+// computed: the lane engine's schedule (solver.cu: dr2_lane_body), per image, storage type T, column prox P_c (axis 0, penalty w1) and
+// row prox P_r (axis 1, w2):
+//     t_0 = 2 mean(Y)                     k = 0: x1 = t_0 (the prox of a constant), k >= 1: x1 = P_c(t_k)
+//     d = t_k - x1 ;  u = Y - (2 d - t_k) ;  x2 = P_r(u) ;  t_{k+1} = d + x2                       k = 0 .. K-1
+//     final: x1 = P_c(t_K) ;  d = t_K - x1 ;  out = P_r(Y - d)
+// Every prox has the Jacobian of vjp_core.cuh: the mean over each constant segment, S_p(g) for pass p.  For an upstream gradient G:
+//     final:      a = S_R(G) ; gY = a ; g_t = S_C(a) - a
+//     k = K-1..0: G = g_t ; a = S_R(G) ; gY = gY + a ; h = G - 2 a ; g_t = (a + h) - S_C(h)
+//     start:      gY = (T)((double)gY + (2.0 * sum_image(g_t)) / (M N))
+// (k = 0: S_C is the column mean when w1 > 0 and M > 1, else the identity -- the Jacobian of the prox at a constant image).  All
+// combines in T with exactly these associations (-fmad=false); sum_image is a double sum in the fixed two-stage order below.
+//
+// Tape: a 256-byte header (Dr2TapeHeader), then 2K + 1 passes in execution order -- p = 0: row pass of k = 0; p = 2k - 1 / 2k: column /
+// row pass of iteration k (k = K: the final pair) -- each two bitsets F, U (vjp_core.cuh) of vjp_tape_set_bytes(n) bytes.  The first
+// column pass (a constant) is not recorded.
+//
+// Penalty gradients (glam, per image [cols, rows]): a pass's gw (vjp_core.cuh rule 4 for its upstream gradient) summed per image in
+// double (two-stage: fixed blocks, then one block per image) and added to the image's accumulator in backward execution order; the
+// column passes' upstream gradient is -h, so their sums enter negated; the k = 0 column pass contributes 0.  No atomics: a call's
+// result does not depend on timing.
+#include "ptv_internal.h"
+#include "vjp_core.cuh"
+#include <string.h>
+
+namespace ptv {
+
+static inline size_t al256(size_t b) { return (b + 255) & ~(size_t)255; }
+static constexpr size_t DR2V_SCRATCH = (REDUCE_BLOCKS + 8) * sizeof(double);
+
+struct Dr2TapeHeader {
+    uint64_t magic;
+    int64_t elem, M, N, batch, row_major, K, w1pos, w2pos;
+    int64_t pad[23];
+};
+static_assert(sizeof(Dr2TapeHeader) == 256, "tape header is 256 bytes");
+static constexpr uint64_t DR2_TAPE_MAGIC = 0x3150415432524432ull;          // "2DR2TAP1"
+
+size_t dr2_tape_bytes(size_t M, size_t N, int batch, int maxit) {
+    const int K = maxit <= 0 ? MAX_ITERS_DR : maxit;
+    return 256 + (size_t)(2 * K + 1) * 2 * ptvv::vjp_tape_set_bytes((long long)(M * N * (size_t)batch));
+}
+template <typename T> size_t ws_bytes_dr2_record(size_t M, size_t N, int batch) {
+    return 8 * al256(M * N * (size_t)batch * sizeof(T)) + DR2V_SCRATCH;      // t, d, u, x + 4 arrays of staging for prox_fibers
+}
+template <typename T> size_t ws_bytes_dr2_vjp(size_t M, size_t N, int batch) {
+    const long long n = (long long)(M * N * (size_t)batch);
+    const size_t s1 = ptvv::vjp_scratch_bytes((long long)N * batch, (int)M), s2 = ptvv::vjp_scratch_bytes((long long)M * batch, (int)N);
+    return 6 * al256((size_t)n * sizeof(T)) + al256(s1 > s2 ? s1 : s2) + DR2V_SCRATCH + al256((size_t)batch * sizeof(double));
+}
+
+static unsigned ew_grid(long long n) {
+    long long b = (n + 1023) / 1024;
+    if (b < 1) b = 1;
+    if (b > 132LL * 32) b = 132LL * 32;
+    return (unsigned)b;
+}
+#define GRID_STRIDE(q, n) for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < (n); q += (long long)gridDim.x * blockDim.x)
+
+// ---------------------------------------------------------------- recorded forward: combines that write the tape of the pass they read
+// One warp per 32-element tape word; lane j handles element 32 q + j.  The pass output x is read at i and at its successor i + inc.
+// Column pass (FINAL = false): d = t - x1 ; u = Y - (2 d - t)     (FINAL): d = t - x1 ; u = Y - d        tape of x1, column geometry
+template <typename T, bool FINAL>
+__global__ void k_rec_cols(const T* __restrict__ x1, const T* __restrict__ t, const T* __restrict__ Y, T* __restrict__ d, T* __restrict__ u,
+                           long long n, int len, long long inc, double lam, uint32_t* __restrict__ F, uint32_t* __restrict__ U, long long nwords) {
+    const int lane = threadIdx.x & 31;
+    const long long w0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5, ws = ((long long)gridDim.x * blockDim.x) >> 5;
+    for (long long q = w0; q < nwords; q += ws) {
+        const long long i = q * 32 + lane;
+        uint32_t f = 0, uu = 0;
+        if (i < n) {
+            ptvv::vjp_tape_edge<T>(x1, i, len, inc, lam, (const T*)nullptr, f, uu);
+            const T tv = t[i];
+            const T dv = tv - x1[i];
+            d[i] = dv;
+            u[i] = FINAL ? Y[i] - dv : Y[i] - (T(2) * dv - tv);
+        }
+        const uint32_t bf = __ballot_sync(0xffffffffu, f), bu = __ballot_sync(0xffffffffu, uu);
+        if (lane == 0) { F[q] = bf; U[q] = bu; }
+    }
+}
+// Row pass: t' = d + x2 ; tape of x2, row geometry
+template <typename T>
+__global__ void k_rec_rows(const T* __restrict__ x2, const T* __restrict__ d, T* __restrict__ tn, long long n, int len, long long inc,
+                           double lam, uint32_t* __restrict__ F, uint32_t* __restrict__ U, long long nwords) {
+    const int lane = threadIdx.x & 31;
+    const long long w0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5, ws = ((long long)gridDim.x * blockDim.x) >> 5;
+    for (long long q = w0; q < nwords; q += ws) {
+        const long long i = q * 32 + lane;
+        uint32_t f = 0, uu = 0;
+        if (i < n) {
+            ptvv::vjp_tape_edge<T>(x2, i, len, inc, lam, (const T*)nullptr, f, uu);
+            tn[i] = d[i] + x2[i];
+        }
+        const uint32_t bf = __ballot_sync(0xffffffffu, f), bu = __ballot_sync(0xffffffffu, uu);
+        if (lane == 0) { F[q] = bf; U[q] = bu; }
+    }
+}
+
+static void dr2_geoms(size_t M, size_t N, int batch, int row_major, FiberGeom& gc, FiberGeom& gr) {
+    gc = row_major ? FiberGeom{(long long)N * batch, (int)M, (long long)N} : FiberGeom{(long long)N * batch, (int)M, 1};
+    gr = row_major ? FiberGeom{(long long)M * batch, (int)N, 1} : FiberGeom{(long long)M * batch, (int)N, (long long)M};
+}
+
+template <typename T>
+cudaError_t dr2_record_device(size_t M, size_t N, int batch, int row_major, const T* Y, T w1, T w2, T* out, int maxit, void* tape, void* ws,
+                              Engine eng, cudaStream_t st) {
+    const long long n = (long long)(M * N * (size_t)batch);
+    const int K = maxit <= 0 ? MAX_ITERS_DR : maxit;
+    const size_t ab = al256((size_t)n * sizeof(T)), sb = ptvv::vjp_tape_set_bytes(n);
+    char* w = (char*)ws;
+    T* t = (T*)w; w += ab;
+    T* d = (T*)w; w += ab;
+    T* u = (T*)w; w += ab;
+    T* x = (T*)w; w += ab;
+    T* scr = (T*)w; w += 4 * ab;
+    double* scratch = (double*)w;
+    FiberGeom gc, gr;
+    dr2_geoms(M, N, batch, row_major, gc, gr);
+    // the engine and the lane decision of dr2_device for the same arguments
+    eng = lane_guard<T>(eng, Y, n, (double)(w1 > w2 ? w1 : w2), st);
+    void* lscr = nullptr;
+    const bool lane = dr2_lane_pick<T>(M, N, batch, row_major, Y, out, ws, w1, w2, eng, &lscr) != 0;
+    auto prox = [&](const T* in, T* o, bool col) -> cudaError_t {
+        const FiberGeom& g = col ? gc : gr;
+        const T lam = col ? w1 : w2;
+        if (lane) {
+            KernelSpan sp(g.inc == 1 ? KC_PROX_CONTIG : KC_PROX_STRIDED, 1, st);
+            return ptvl::lane_prox<T>(ptvl::LANE_PLAIN, in, nullptr, nullptr, o, g.nf, g.len, g.inc, lam, lscr, st);
+        }
+        return prox_fibers<T>(in, nullptr, IN_A, o, 0, g, lam, nullptr, eng, scr, st, 4 * n);
+    };
+    auto Fp = [&](int p) { return (uint32_t*)((char*)tape + 256 + (size_t)p * 2 * sb); };
+    auto Up = [&](int p) { return (uint32_t*)((char*)tape + 256 + (size_t)p * 2 * sb + sb); };
+    const long long nwords = (long long)(sb / 4);
+    const unsigned gw = ew_grid(nwords * 32);
+#define RTRY(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) return e__; } while (0)
+    Dr2TapeHeader h;
+    memset(&h, 0, sizeof(h));
+    h.magic = DR2_TAPE_MAGIC; h.elem = (int64_t)sizeof(T); h.M = (int64_t)M; h.N = (int64_t)N; h.batch = batch; h.row_major = row_major ? 1 : 0;
+    h.K = K; h.w1pos = w1 > T(0); h.w2pos = w2 > T(0);
+    RTRY(cudaMemcpyAsync(tape, &h, sizeof(h), cudaMemcpyHostToDevice, st));
+    RTRY(ew_image_means_x2<T>(Y, (long long)(M * N), batch, t, scratch, st));          // t = 2 mean
+    RTRY(ew_dr_first<T>(Y, t, u, d, n, st));                                           // k = 0: d = t - t ; u = Y - (2 d - t)
+    for (int k = 0; k <= K; k++) {
+        const bool final = k == K;
+        if (k > 0) {
+            RTRY(prox(t, x, true));
+            KernelSpan sp(KC_ELEMENTWISE, 1, st);
+            if (final) k_rec_cols<T, true><<<gw, 256, 0, st>>>(x, t, Y, d, u, n, gc.len, gc.inc, (double)w1, Fp(2 * k - 1), Up(2 * k - 1), nwords);
+            else k_rec_cols<T, false><<<gw, 256, 0, st>>>(x, t, Y, d, u, n, gc.len, gc.inc, (double)w1, Fp(2 * k - 1), Up(2 * k - 1), nwords);
+            RTRY(cudaGetLastError());
+        }
+        if (final) {
+            RTRY(prox(u, out, false));
+            RTRY(ptvv::fiber_tape<T>(out, gr.nf, gr.len, gr.inc, w2, nullptr, Fp(2 * k), Up(2 * k), st));
+        } else {
+            RTRY(prox(u, x, false));
+            KernelSpan sp(KC_ELEMENTWISE, 1, st);
+            k_rec_rows<T><<<gw, 256, 0, st>>>(x, d, t, n, gr.len, gr.inc, (double)w2, Fp(2 * k), Up(2 * k), nwords);
+            RTRY(cudaGetLastError());
+        }
+    }
+    return cudaSuccess;
+}
+
+const char* dr2_tape_check(const void* tape, size_t elem, size_t M, size_t N, int batch, int row_major, int maxit, cudaStream_t st) {
+    Dr2TapeHeader h;
+    if (cudaMemcpyAsync(&h, tape, sizeof(h), cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) {
+        cudaGetLastError(); return "cannot read the tape header";
+    }
+    const int K = maxit <= 0 ? MAX_ITERS_DR : maxit;
+    if (h.magic != DR2_TAPE_MAGIC) return "not a DR2_TV tape";
+    if (h.elem != (int64_t)elem) return "tape recorded with another dtype";
+    if (h.M != (int64_t)M || h.N != (int64_t)N || h.batch != batch) return "tape recorded for another shape";
+    if (h.row_major != (row_major ? 1 : 0)) return "tape recorded for another storage order";
+    if (h.K != K) return "tape recorded with another iteration count";
+    return nullptr;
+}
+
+// ---------------------------------------------------------------- backward
+__device__ __forceinline__ double dr2v_block_sum(double v) {
+    __shared__ double sm[32];
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+    const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+    if (l == 0) sm[w] = v;
+    __syncthreads();
+    const int nw = (blockDim.x + 31) >> 5;
+    v = (threadIdx.x < nw) ? sm[threadIdx.x] : 0.0;
+    if (w == 0) for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+    __syncthreads();
+    return v;   // valid in thread 0
+}
+// per-image sums, stage 1: block x of image y sums a grid-stride slice of the image into partial[y][x]
+template <typename T>
+__global__ void k_img_partial(const T* __restrict__ a, long long per, double* __restrict__ partial) {
+    const T* img = a + (long long)blockIdx.y * per;
+    double acc = 0.0;
+    for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < per; q += (long long)gridDim.x * blockDim.x) acc += (double)img[q];
+    acc = dr2v_block_sum(acc);
+    if (threadIdx.x == 0) partial[(long long)blockIdx.y * gridDim.x + blockIdx.x] = acc;
+}
+// stage 2: one block per image sums its nblk partials; glam != nullptr: glam[2 b + axis] += sign * sum, else sums[b] = sum
+__global__ void k_img_final(const double* __restrict__ partial, int nblk, int b0, double* __restrict__ sums, double* __restrict__ glam, int axis,
+                            double sign) {
+    double acc = 0.0;
+    for (int q = threadIdx.x; q < nblk; q += blockDim.x) acc += partial[(long long)blockIdx.x * nblk + q];
+    acc = dr2v_block_sum(acc);
+    if (threadIdx.x == 0) {
+        const int b = b0 + blockIdx.x;
+        if (glam) glam[2 * b + axis] = glam[2 * b + axis] + sign * acc;
+        else sums[b] = acc;
+    }
+}
+template <typename T>
+static cudaError_t img_sums(const T* a, long long per, int batch, double* scratch, double* sums, double* glam, int axis, double sign,
+                            cudaStream_t st) {
+    if (per <= 0) return cudaSuccess;
+    int nblk = (int)((per + 2047) / 2048);
+    if (nblk > REDUCE_BLOCKS) nblk = REDUCE_BLOCKS;
+    const int share = REDUCE_BLOCKS / (batch < REDUCE_BLOCKS ? batch : REDUCE_BLOCKS);
+    if (nblk > share) nblk = share < 1 ? 1 : share;
+    int per_launch = REDUCE_BLOCKS / nblk; if (per_launch < 1) per_launch = 1;
+    KernelSpan span(KC_ELEMENTWISE, 2 * ((batch + per_launch - 1) / per_launch), st);
+    for (int b0 = 0; b0 < batch; b0 += per_launch) {
+        const int nb = batch - b0 < per_launch ? batch - b0 : per_launch;
+        k_img_partial<T><<<dim3(nblk, nb), 256, 0, st>>>(a + (long long)b0 * per, per, scratch);
+        k_img_final<<<nb, 256, 0, st>>>(scratch, nblk, b0, sums, glam, axis, sign);
+    }
+    return cudaGetLastError();
+}
+
+template <typename T> __global__ void k_b_final(const T* __restrict__ a, const T* __restrict__ sc, T* __restrict__ gY, T* __restrict__ g, long long n) {
+    GRID_STRIDE(q, n) { const T av = a[q]; gY[q] = av; g[q] = sc[q] - av; }
+}
+template <typename T> __global__ void k_b_mid1(const T* __restrict__ G, const T* __restrict__ a, T* __restrict__ gY, T* __restrict__ h, long long n) {
+    GRID_STRIDE(q, n) { const T av = a[q]; gY[q] = gY[q] + av; h[q] = G[q] - T(2) * av; }
+}
+template <typename T> __global__ void k_b_mid2(const T* __restrict__ a, const T* __restrict__ h, const T* __restrict__ sc, T* __restrict__ g, long long n) {
+    GRID_STRIDE(q, n) g[q] = (a[q] + h[q]) - sc[q];
+}
+template <typename T> __global__ void k_b_start(T* __restrict__ gY, const double* __restrict__ sums, long long per, long long n) {
+    GRID_STRIDE(q, n) gY[q] = (T)((double)gY[q] + (2.0 * sums[q / per]) / (double)per);
+}
+
+template <typename T>
+cudaError_t dr2_vjp_device(size_t M, size_t N, int batch, int row_major, int maxit, const void* tape, const T* gout, T* gY, double* glam,
+                           void* ws, cudaStream_t st) {
+    const long long n = (long long)(M * N * (size_t)batch), per = (long long)(M * N);
+    const int K = maxit <= 0 ? MAX_ITERS_DR : maxit;
+    const size_t ab = al256((size_t)n * sizeof(T)), sb = ptvv::vjp_tape_set_bytes(n);
+    const size_t s1 = ptvv::vjp_scratch_bytes((long long)N * batch, (int)M), s2 = ptvv::vjp_scratch_bytes((long long)M * batch, (int)N);
+    char* w = (char*)ws;
+    T* g = (T*)w; w += ab;
+    T* a = (T*)w; w += ab;
+    T* h = (T*)w; w += ab;
+    T* sc = (T*)w; w += ab;
+    T* gwb = (T*)w; w += ab;
+    T* zero = (T*)w; w += ab;
+    void* vscr = w; w += al256(s1 > s2 ? s1 : s2);
+    double* scratch = (double*)w; w += DR2V_SCRATCH;
+    double* sums = (double*)w;
+    FiberGeom gc, gr;
+    dr2_geoms(M, N, batch, row_major, gc, gr);
+    Dr2TapeHeader hd;                                  // read by the caller's check; the flags are needed here too
+    RTRY(cudaMemcpyAsync(&hd, tape, sizeof(hd), cudaMemcpyDeviceToHost, st));
+    RTRY(cudaStreamSynchronize(st));
+    const long long ec = gc.nf / batch * (gc.len - 1), er = gr.nf / batch * (gr.len - 1);     // edges per image of either pass
+    const char* tb = (const char*)tape + 256;
+    auto Fp = [&](int p) { return (const uint32_t*)(tb + (size_t)p * 2 * sb); };
+    auto Up = [&](int p) { return (const uint32_t*)(tb + (size_t)p * 2 * sb + sb); };
+    T* gw = glam ? gwb : nullptr;
+    const unsigned ge = ew_grid(n);
+    auto vjp = [&](int p, const T* gin, T* gx, bool col, double sign) -> cudaError_t {
+        const FiberGeom& G = col ? gc : gr;
+        RTRY(ptvv::vjp_fibers_tape<T>(Fp(p), Up(p), gin, gx, gw, G.nf, G.len, G.inc, vscr, st));
+        if (glam) RTRY(img_sums<T>(gw, col ? ec : er, batch, scratch, nullptr, glam, col ? 0 : 1, sign, st));
+        return cudaSuccess;
+    };
+    if (glam) RTRY(cudaMemsetAsync(glam, 0, 2 * (size_t)batch * sizeof(double), st));
+    // final pair: out = P_r(Y - d), d = t_K - P_c(t_K)
+    RTRY(vjp(2 * K, gout, a, false, 1.0));
+    RTRY(vjp(2 * K - 1, a, sc, true, 1.0));                 // upstream of the final column prox: +a
+    { KernelSpan sp(KC_ELEMENTWISE, 1, st); k_b_final<T><<<ge, 256, 0, st>>>(a, sc, gY, g, n); RTRY(cudaGetLastError()); }
+    for (int k = K - 1; k >= 0; k--) {
+        RTRY(vjp(2 * k, g, a, false, 1.0));
+        { KernelSpan sp(KC_ELEMENTWISE, 1, st); k_b_mid1<T><<<ge, 256, 0, st>>>(g, a, gY, h, n); RTRY(cudaGetLastError()); }
+        if (k > 0) RTRY(vjp(2 * k - 1, h, sc, true, -1.0));  // upstream of the column prox: -h
+        else {
+            // the prox of the constant start image: every column one segment (w1 > 0), or the identity (w1 == 0); M == 1 is one sample
+            RTRY(cudaMemsetAsync(zero, 0, (size_t)n * sizeof(T), st));
+            RTRY(ptvv::vjp_fibers<T>(zero, h, sc, nullptr, gc.nf, gc.len, gc.inc, hd.w1pos ? T(1) : T(0), nullptr, vscr, st));
+        }
+        { KernelSpan sp(KC_ELEMENTWISE, 1, st); k_b_mid2<T><<<ge, 256, 0, st>>>(a, h, sc, g, n); RTRY(cudaGetLastError()); }
+    }
+    RTRY(img_sums<T>(g, per, batch, scratch, sums, nullptr, 0, 0.0, st));
+    { KernelSpan sp(KC_ELEMENTWISE, 1, st); k_b_start<T><<<ge, 256, 0, st>>>(gY, sums, per, n); RTRY(cudaGetLastError()); }
+    return cudaSuccess;
+#undef RTRY
+}
+
+#define INST(T) \
+    template size_t ws_bytes_dr2_record<T>(size_t, size_t, int); \
+    template size_t ws_bytes_dr2_vjp<T>(size_t, size_t, int); \
+    template cudaError_t dr2_record_device<T>(size_t, size_t, int, int, const T*, T, T, T*, int, void*, void*, Engine, cudaStream_t); \
+    template cudaError_t dr2_vjp_device<T>(size_t, size_t, int, int, int, const void*, const T*, T*, double*, void*, cudaStream_t);
+INST(double)
+INST(float)
+
+}  // namespace ptv

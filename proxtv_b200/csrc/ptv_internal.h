@@ -108,6 +108,23 @@ template <typename T> int pd_device(const T* y, const double* lambdas_scaled, co
 // lane engine, else eng.  One small kernel and one stream synchronisation per call (the data behind a pointer changes between calls).
 template <typename T> Engine lane_guard(Engine eng, const T* y, long long n, double lam, cudaStream_t st);
 int lane_guard_last();           // tools / tests: last decision on this device (1 lane suits, 0 it does not, -1 none taken)
+// The lane schedule dr2_device takes for these arguments and engine (already through lane_guard): 0 none, 1 staged (dr2_lane_body),
+// 2 transposed (dr2_lane_t_body).  A lane schedule gets the lane engine's scratch in *lscr (allocates: call outside stream capture).
+template <typename T> int dr2_lane_pick(size_t M, size_t N, int batch, int row_major, const T* Y, const T* out, const void* ws, T w1, T w2,
+                                        Engine eng, void** lscr);
+
+// ---- exact backward pass of DR2_TV (dr2_vjp.cu, DESIGN.md section 11) ----
+size_t dr2_tape_bytes(size_t M, size_t N, int batch, int maxit);          // header + (2K + 1) passes x two bitsets
+template <typename T> size_t ws_bytes_dr2_record(size_t M, size_t N, int batch);
+template <typename T> size_t ws_bytes_dr2_vjp(size_t M, size_t N, int batch);
+// DR2_TV with the schedule of the lane engine in plain passes, writing the segmentation tape of every pass but the first column pass.
+// The tape's size (dr2_tape_bytes) is checked by the caller.  Returns a CUDA error (cudaErrorInvalidConfiguration: a lane pass refused).
+template <typename T> cudaError_t dr2_record_device(size_t M, size_t N, int batch, int row_major, const T* Y, T w1, T w2, T* out, int maxit,
+                                                    void* tape, void* ws, Engine eng, cudaStream_t st);
+// Validates a tape's header against the arguments (host; reads it back with one stream synchronisation): nullptr ok, else the reason.
+const char* dr2_tape_check(const void* tape, size_t elem, size_t M, size_t N, int batch, int row_major, int maxit, cudaStream_t st);
+template <typename T> cudaError_t dr2_vjp_device(size_t M, size_t N, int batch, int row_major, int maxit, const void* tape, const T* gout,
+                                                 T* gY, double* glam, void* ws, cudaStream_t st);
 
 // PDR_TV (src/TVNDopt.cpp:280-500): parallel Douglas-Rachford, fixed iteration count; same workspace as pd_device
 template <typename T> int pdr_device(const T* y, const double* lambdas_scaled, const double* dims, T* x, double* info,
@@ -137,6 +154,13 @@ namespace ptvv {
 template <typename T>
 cudaError_t vjp_fibers(const T* y, const T* g, T* gx, T* gw, long long nf, int len, long long inc, T lam, const T* lamv, void* scratch,
                        cudaStream_t st);
+// The same, with "fused" and the edge signs read from a segmentation tape (vjp_core.cuh) of y instead of y and the weights.
+template <typename T>
+cudaError_t vjp_fibers_tape(const uint32_t* F, const uint32_t* U, const T* g, T* gx, T* gw, long long nf, int len, long long inc,
+                            void* scratch, cudaStream_t st);
+// The segmentation tape of y over the fibers (nf, len, inc), nf a multiple of inc: F and U of vjp_tape_set_bytes(nf * len) bytes each.
+template <typename T>
+cudaError_t fiber_tape(const T* y, long long nf, int len, long long inc, T lam, const T* lamv, uint32_t* F, uint32_t* U, cudaStream_t st);
 size_t vjp_scratch_bytes(long long nf, int len);
 int vjp_chunk_len(long long nf, int len);
 void vjp_set_tuning(int clen);

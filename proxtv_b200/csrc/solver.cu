@@ -286,6 +286,23 @@ template <typename T> size_t ws_bytes_dr2(size_t M, size_t N, int batch) {
 }
 
 template <typename T>
+int dr2_lane_pick(size_t M, size_t N, int batch, int row_major, const T* Y, const T* out, const void* ws, T w1, T w2, Engine eng,
+                  void** lscr) {
+    *lscr = nullptr;
+    const void* lane_ptrs[3] = {Y, out, ws};
+    const bool lane_t = eng == ENGINE_LANE_T || row_major;
+    bool lane = (eng == ENGINE_AUTO || eng == ENGINE_LANE || eng == ENGINE_LANE_T) && w1 > T(0) && w2 > T(0) && M >= 2 && N >= 2 && g_pipe.init() &&
+                ptvl::lane_shape_ok((long long)N * batch, (int)M, lane_t ? (long long)N : 1, sizeof(T), lane_ptrs, 3) &&
+                ptvl::lane_shape_ok((long long)M * batch, (int)N, (long long)M, sizeof(T), lane_ptrs, 3) &&
+                (!lane_t || (((long long)M * sizeof(T)) % 16 == 0 && ((long long)N * sizeof(T)) % 16 == 0));
+    if (lane) {
+        void* a1 = ptvl::lane_scratch((long long)N * batch, (int)M); void* a2 = ptvl::lane_scratch((long long)M * batch, (int)N);
+        *lscr = a2; lane = a1 && a2;                // the second call returns the (possibly grown) buffer both passes use
+    }
+    return lane ? (lane_t ? 2 : 1) : 0;
+}
+
+template <typename T>
 int dr2_device(size_t M, size_t N, int batch, int row_major, const T* Y, T w1, T w2, T* out, int maxit, double* info, void* ws,
                Engine eng, cudaStream_t st) {
     const long long n = (long long)M * (long long)N * batch;
@@ -313,17 +330,9 @@ int dr2_device(size_t M, size_t N, int batch, int row_major, const T* Y, T w1, T
                        (size_t)((M > N ? M : N) * sizeof(T)) <= 96 * 1024 && g_pipe.init();
     // lane-per-fiber engine: images whose row pitch suits TMA tiling, positive weights.  Column-major: the staged schedule (column
     // pass over contiguous fibers) or, engine lane-t, the transposed one; row-major: only the transposed schedule applies.
-    const void* lane_ptrs[3] = {Y, out, ws};
     void* lscr = nullptr;
-    const bool lane_t = eng == ENGINE_LANE_T || row_major;
-    bool lane = (eng == ENGINE_AUTO || eng == ENGINE_LANE || eng == ENGINE_LANE_T) && w1 > T(0) && w2 > T(0) && M >= 2 && N >= 2 && g_pipe.init() &&
-                ptvl::lane_shape_ok((long long)N * batch, (int)M, lane_t ? (long long)N : 1, sizeof(T), lane_ptrs, 3) &&
-                ptvl::lane_shape_ok((long long)M * batch, (int)N, (long long)M, sizeof(T), lane_ptrs, 3) &&
-                (!lane_t || (((long long)M * sizeof(T)) % 16 == 0 && ((long long)N * sizeof(T)) % 16 == 0));
-    if (lane) {
-        void* a1 = ptvl::lane_scratch((long long)N * batch, (int)M); void* a2 = ptvl::lane_scratch((long long)M * batch, (int)N);
-        lscr = a2; lane = a1 && a2;                 // the second call returns the (possibly grown) buffer both passes use
-    }
+    const int lane_sched = dr2_lane_pick<T>(M, N, batch, row_major, Y, out, ws, w1, w2, eng, &lscr);
+    const bool lane = lane_sched != 0, lane_t = lane_sched == 2;
     if (lane || tspace || piped) {
         auto body = [&](cudaStream_t bs) -> int {
             if (lane) return lane_t ? dr2_lane_t_body<T>(M, N, batch, row_major, Y, w1, w2, out, maxit, t, s, x, scr, scratch, lscr, bs)
@@ -603,6 +612,7 @@ int pdr_device(const T* y, const double* lam, const double* dims, T* x, double* 
 #define INST(T) \
     template size_t ws_bytes_dr2<T>(size_t, size_t, int); \
     template int dr2_device<T>(size_t, size_t, int, int, const T*, T, T, T*, int, double*, void*, Engine, cudaStream_t); \
+    template int dr2_lane_pick<T>(size_t, size_t, int, int, const T*, const T*, const void*, T, T, Engine, void**); \
     template int drw_device<T>(size_t, size_t, const T*, const T*, const T*, T*, int, double*, void*, Engine, cudaStream_t); \
     template size_t ws_bytes_pd<T>(long long, int); \
     template int pd2_device<T>(const T*, const double*, const double*, T*, double*, const int*, int, int, int, void*, Engine, cudaStream_t); \

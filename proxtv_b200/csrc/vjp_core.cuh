@@ -45,6 +45,38 @@ struct VjpMeans { double head, tail; };   // pass 2: (T-rounded) means of the op
 
 PTV_HD double vjp_sgn(double d) { return d > 0.0 ? 1.0 : (d < 0.0 ? -1.0 : 0.0); }
 
+// Segmentation tape of one prox pass (what the backward needs of a forward output y, without y): two bitsets F, U over the linear
+// elements of the array in storage order; bit i describes element i and its successor along the pass's fibers (the (nf, len, inc)
+// slicing rule: the successor of element i is i + inc, except at the last sample of a fiber):
+//     (F, U) = (1, 0) fused (rule 1 above: equal as stored, weight > 0)      (0, 1) unfused, the successor is greater
+//              (0, 0) unfused, the successor is smaller; also every fiber's last sample      (1, 1) unfused and equal (zero weight): sign 0
+// Each bitset is ceil(n / 32) uint32 words (bit i: word i / 32, bit i % 32), zero-padded to a multiple of 256 bytes.
+PTV_HD size_t vjp_tape_set_bytes(long long n) { return ((size_t)((n + 31) / 32) * 4 + 255) & ~(size_t)255; }
+PTV_HD void vjp_tape_encode(bool last, bool eq, bool gt, bool wpos, uint32_t& f, uint32_t& u) {
+    f = (!last && eq) ? 1u : 0u;
+    u = (!last && (gt || (eq && !wpos))) ? 1u : 0u;
+}
+// (F, U) bits of linear element i of y under the slicing rule (nf, len, inc) (weights: w laid out with len-1 samples per fiber, or
+// the uniform penalty lam when w is NULL)
+template <typename T>
+PTV_HD void vjp_tape_edge(const T* y, long long i, int len, long long inc, double lam, const T* w, uint32_t& f, uint32_t& u) {
+    const long long slab = i / (inc * (long long)len), in = i - slab * inc * (long long)len;
+    const long long r = in / inc, c = in - r * inc;
+    const bool last = r == (long long)len - 1;
+    if (last) { f = 0; u = 0; return; }
+    const T a = y[i], b = y[i + inc];
+    const bool wpos = w ? w[slab * inc * (long long)(len - 1) + r * inc + c] > T(0) : lam > 0.0;
+    vjp_tape_encode(false, b == a, b > a, wpos, f, u);
+}
+// element i's edge: fused? and its sign (meaningful on unfused edges that are not a fiber's last sample)
+PTV_HD bool vjp_tape_fused(const uint32_t* F, const uint32_t* U, long long i) {
+    return ((F[i >> 5] >> (i & 31)) & 1u) && !((U[i >> 5] >> (i & 31)) & 1u);
+}
+PTV_HD double vjp_tape_sgn(const uint32_t* F, const uint32_t* U, long long i) {
+    const bool f = (F[i >> 5] >> (i & 31)) & 1u, u = (U[i >> 5] >> (i & 31)) & 1u;
+    return u ? (f ? 0.0 : 1.0) : -1.0;
+}
+
 // Pass 1, one row at a time.  The caller feeds row i with g[i], y[i+1] (ignored at i == len-1) and whether edge i's weight is > 0.
 // S: out.gx(row, value), out.gw(edge, value) (a no-op when gw is not wanted).
 template <typename T> struct VjpScan {
@@ -61,9 +93,15 @@ template <typename T> struct VjpScan {
         open_left = open_left_; pend = false; fused_last = false; yc = y0;
     }
     template <class S> PTV_HD void row(int i, T gi, T yn, bool wpos, S& out) {
+        const bool last = (i == len - 1);
+        step(i, gi, !last && yn == yc && wpos, [&]() { return vjp_sgn((double)yn - (double)yc); }, out);
+        if (!last) yc = yn;
+    }
+    // The same row with "fused" and the sign of the edge (called only when the edge is not fused and not the fiber's last) given by the
+    // caller: row() derives them from y, the tape-driven kernels (vjp_tape_bits) from a pass's segmentation tape.
+    template <class S, class SG> PTV_HD void step(int i, T gi, bool fu, SG sgn, S& out) {
         s = s + (double)gi;
         const bool last = (i == len - 1);
-        const bool fu = !last && yn == yc && wpos;
         if (fu) {
             out.gw(i, T(0));
         } else {
@@ -78,10 +116,9 @@ template <typename T> struct VjpScan {
             }
             if (head_end < 0) head_end = i;
             pend = mine && !last;           // edge i waits for the next segment's mean (never consumed at the chunk's end: pass 3)
-            if (!last) { psg = vjp_sgn((double)yn - (double)yc); pm = mt; }
+            if (!last) { psg = sgn(); pm = mt; }
             s = 0.0; st = i + 1;
         }
-        if (!last) yc = yn;
         fused_last = fu;
     }
     PTV_HD void finish(VjpRec& r) const {
@@ -121,8 +158,15 @@ PTV_HD double vjp_first_mean(const VjpRec& r, const VjpMeans& m) { return r.head
 // Pass 3, one chunk: gx of its open parts, then gw of the edges pass 1 left: after an open head, before an open tail, and the chunk's
 // last edge when it ends a segment (its right side is the next chunk's first segment, m_next = vjp_first_mean of that chunk).
 // Y: y(row) -> T, X: gx(row) -> T (reads back what passes 1 and 3 stored in this chunk), W: wpos(edge) is not needed (unfused edges only).
+// vjp_fix_chunk_sg: the same with the sign of an unfused edge given by the caller, SG: sg(edge) -> double (tape-driven kernels).
+template <typename T, class S, class SG, class X>
+PTV_HD void vjp_fix_chunk_sg(const VjpRec& r, const VjpMeans& mm, int c0, int c1, int len, double m_next, bool want_gw, SG sg, X gx, S& out);
 template <typename T, class S, class Y, class X>
 PTV_HD void vjp_fix_chunk(const VjpRec& r, const VjpMeans& mm, int c0, int c1, int len, double m_next, bool want_gw, Y y, X gx, S& out) {
+    vjp_fix_chunk_sg<T>(r, mm, c0, c1, len, m_next, want_gw, [&](int e) { return vjp_sgn((double)y(e + 1) - (double)y(e)); }, gx, out);
+}
+template <typename T, class S, class SG, class X>
+PTV_HD void vjp_fix_chunk_sg(const VjpRec& r, const VjpMeans& mm, int c0, int c1, int len, double m_next, bool want_gw, SG sg, X gx, S& out) {
     const bool ol = r.flags & VJP_OPEN_LEFT, orr = r.flags & VJP_OPEN_RIGHT;
     const bool inside = ol && r.head_end < 0;
     if (ol) { const int e = inside ? c1 - 1 : r.head_end; for (int k = c0; k <= e; k++) out.gx(k, (T)mm.head); }
@@ -130,7 +174,7 @@ PTV_HD void vjp_fix_chunk(const VjpRec& r, const VjpMeans& mm, int c0, int c1, i
     if (!want_gw || inside) return;
     auto edge = [&](int e) {
         const double l = (double)gx(e), rr = (e == c1 - 1) ? m_next : (double)gx(e + 1);
-        out.gw(e, (T)(vjp_sgn((double)y(e + 1) - (double)y(e)) * (l - rr)));
+        out.gw(e, (T)(sg(e) * (l - rr)));
     };
     if (ol && r.head_end < c1 - 1) edge(r.head_end);
     if (orr && r.tail_start > c0 && !(ol && r.head_end == r.tail_start - 1)) edge(r.tail_start - 1);
