@@ -191,6 +191,26 @@ int proxtv_DR2L1W_TV_dev_f64(size_t M, size_t N, const double *Y, const double *
                              double *info, void *stream);
 int proxtv_DR2L1W_TV_dev_f32(size_t M, size_t N, const float *Y, const float *W1, const float *W2, float *out, int maxit,
                              double *info, void *stream);
+/* Exact backward pass of DR2L1W_TV (DESIGN.md section 12): the gradient of the function computed, K = maxit (0: 35) iterations and
+ * the final pair, every prox pass with the Jacobian of proxtv_prox_fibers_vjp_dev_*.  Layouts as proxtv_DR2L1W_TV_dev_*.
+ * record: proxtv_DR2L1W_TV_dev_* bit for bit, with plain prox passes, writing into the device buffer `tape` (at least
+ * proxtv_DR2L1W_TV_tape_bytes() bytes) a 256-byte header and the segmentation tapes (proxtv_fiber_tape_dev_*) of all 2K + 2 passes.
+ * Weights must be >= 0 (not checked on the device).  Returns 1 ok / 0 error (info[2] = 3 too); refused without writing anything:
+ * M or N < 1, Y, out or tape NULL, W1 NULL with M > 1, W2 NULL with N > 1, tape_bytes too small.  vjp: from the tape alone, gY =
+ * the gradient with respect to Y for the upstream gradient gout (both laid out like out) and, unless NULL, gW1 / gW2 = the gradients
+ * of the per-edge weights (laid out like W1 / W2; each edge's passes summed in double in backward order, rounded once).
+ * Deterministic (no atomics); synchronises the stream once (reads the tape's header).  Returns 1 ok / 0 error; refused without
+ * writing anything: M or N < 1, tape, gout or gY NULL, a header that does not match the arguments (dtype, shape, maxit) -- a
+ * DR2_TV tape included. */
+size_t proxtv_DR2L1W_TV_tape_bytes(size_t M, size_t N, int maxit);
+int proxtv_DR2L1W_TV_record_dev_f64(size_t M, size_t N, const double *Y, const double *W1, const double *W2, double *out, int maxit,
+                                    void *tape, size_t tape_bytes, double *info, void *stream);
+int proxtv_DR2L1W_TV_record_dev_f32(size_t M, size_t N, const float *Y, const float *W1, const float *W2, float *out, int maxit,
+                                    void *tape, size_t tape_bytes, double *info, void *stream);
+int proxtv_DR2L1W_TV_vjp_dev_f64(size_t M, size_t N, int maxit, const void *tape, const double *gout, double *gY, double *gW1,
+                                 double *gW2, void *stream);
+int proxtv_DR2L1W_TV_vjp_dev_f32(size_t M, size_t N, int maxit, const void *tape, const float *gout, float *gY, float *gW1,
+                                 float *gW2, void *stream);
 
 /* PD2_TV / PD_TV with device arrays y, x (lambdas, dims, ns, info stay on the host).  Synchronous (the stop test needs
  * one 8-byte read-back per iteration).  proxtv_PD_TV_* scale lambdas in place like PD_TV. */

@@ -342,11 +342,18 @@ def tv1w_2d(x, w_col, w_row, max_iters=0, n_threads=1):
 
     ``w_col``: (M-1, N) weights of the differences along columns, ``w_row``: (M, N-1) along rows.  Same fixed-iteration
     scheme as ``tv1_2d(method='dr')`` (35 iterations unless ``max_iters`` > 0).  ``n_threads`` is ignored.
-    numpy input: Fortran-ordered float64 result like the reference.  torch CUDA tensors (float64 / float32, all three on
-    the same device): computed on the device, returns a tensor shaped and typed like ``x``.
+    numpy input: Fortran-ordered float64 result like the reference.  torch CUDA tensors (float64 / float32, weights of any
+    floating dtype on any device): computed on x's device, returns a tensor shaped and typed like ``x``.
+
+    torch: differentiable with respect to ``x``, ``w_col`` and ``w_row``.  With grad mode on and one of them requiring grad, the
+    forward records a segmentation tape of every prox pass (2 bits per element per pass, kept on the device until the backward) and
+    the backward is the exact vector-Jacobian product of the fixed-iteration splitting that is computed (proxtv_DR2L1W_TV_vjp_dev_*,
+    DESIGN.md section 12), run on the current CUDA stream; each edge weight gets its own gradient.  Weights of another dtype or
+    device, and expanded weights (``w.expand(M - 1, N)``), get theirs through ordinary autograd.  The forward result is the same
+    either way; double backward is not supported.
     """
     if _is_torch(x):
-        return _drw_torch(x, w_col, w_row, max_iters)
+        return _drw_torch_entry(x, w_col, w_row, max_iters)
     assert np.all(np.asarray(w_col) >= 0)
     assert np.all(np.asarray(w_row) >= 0)
     M, N = np.shape(x)
@@ -382,6 +389,78 @@ def _drw_torch(x, w_col, w_row, max_iters):
            int(max_iters), _ptr(info), st)
     _check(info[2] != 3, "DR2L1W_TV (device)")
     return out.t()
+
+
+_DRW_FN = None
+
+
+def _drw_fn():
+    """torch.autograd.Function around DR2L1W_TV on the device (made on first use, so that numpy users never import torch).
+
+    forward(Y, W1, W2, max_iters): Y (N, M), W1 (N, M-1), W2 (N-1, M) contiguous, x's dtype and device -- the column-major buffers
+    of the solver.  proxtv_DR2L1W_TV_record_dev_* -- the solve of _drw_torch, keeping the segmentation tape of every prox pass (a
+    uint8 CUDA tensor, proxtv_DR2L1W_TV_tape_bytes() long) on ctx.  backward: proxtv_DR2L1W_TV_vjp_dev_* on the current stream, with
+    NULL for a weight map whose input does not need its gradient."""
+    global _DRW_FN
+    if _DRW_FN is not None:
+        return _DRW_FN
+    import torch
+    from torch.autograd.function import once_differentiable
+
+    class DRW(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, Y, W1, W2, max_iters):
+            N, M = int(Y.shape[0]), int(Y.shape[1])
+            lib = require_device()
+            out = torch.empty_like(Y)
+            tape = torch.empty(int(lib.proxtv_DR2L1W_TV_tape_bytes(M, N, int(max_iters))), dtype=torch.uint8, device=Y.device)
+            info = np.zeros(_N_INFO)
+            st = C.c_void_p(torch.cuda.current_stream(Y.device).cuda_stream)
+            fn = lib.proxtv_DR2L1W_TV_record_dev_f32 if Y.dtype == torch.float32 else lib.proxtv_DR2L1W_TV_record_dev_f64
+            with torch.cuda.device(Y.device):
+                ok = fn(M, N, C.c_void_p(Y.data_ptr()), C.c_void_p(W1.data_ptr()), C.c_void_p(W2.data_ptr()), C.c_void_p(out.data_ptr()),
+                        int(max_iters), C.c_void_p(tape.data_ptr()), tape.numel(), _ptr(info), st)
+            _check(ok, "DR2L1W_TV (recorded, device)")
+            ctx.save_for_backward(tape)
+            ctx.geom = (M, N, int(max_iters))
+            return out
+
+        @staticmethod
+        @once_differentiable
+        def backward(ctx, gout):
+            (tape,) = ctx.saved_tensors
+            M, N, max_iters = ctx.geom
+            need_y, need_w1, need_w2, _ = ctx.needs_input_grad
+            dev, dt = tape.device, gout.dtype
+            g = gout.contiguous()
+            gY = torch.empty((N, M), dtype=dt, device=dev)
+            gW1 = torch.empty((N, M - 1), dtype=dt, device=dev) if need_w1 else None
+            gW2 = torch.empty((N - 1, M), dtype=dt, device=dev) if need_w2 else None
+            lib = require_device()
+            st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            fn = lib.proxtv_DR2L1W_TV_vjp_dev_f32 if dt == torch.float32 else lib.proxtv_DR2L1W_TV_vjp_dev_f64
+            p = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None          # noqa: E731
+            with torch.cuda.device(dev):
+                _check(fn(M, N, max_iters, p(tape), p(g), p(gY), p(gW1), p(gW2), st), "DR2L1W_TV backward (device)")
+            return (gY if need_y else None), gW1, gW2, None
+
+    _DRW_FN = DRW
+    return DRW
+
+
+def _drw_torch_entry(x, w_col, w_row, max_iters):
+    """The torch path of tv1w_2d: differentiable when grad mode is on and x, w_col or w_row requires grad; otherwise exactly
+    _drw_torch.  The transposes and casts to the solver's column-major buffers are ordinary autograd ops outside the Function."""
+    import torch
+    if not (torch.is_grad_enabled() and any(_is_torch(t) and t.requires_grad for t in (x, w_col, w_row))):
+        return _drw_torch(x, w_col, w_row, max_iters)
+    assert x.is_cuda and x.dtype in (torch.float64, torch.float32) and x.dim() == 2
+    M, N = int(x.shape[0]), int(x.shape[1])
+    assert tuple(w_col.shape) == (M - 1, N) and tuple(w_row.shape) == (M, N - 1)
+    xt = x.t().contiguous()
+    w1 = w_col.to(device=x.device, dtype=x.dtype).t().contiguous()
+    w2 = w_row.to(device=x.device, dtype=x.dtype).t().contiguous()
+    return _drw_fn().apply(xt, w1, w2, int(max_iters)).t()
 
 
 def _dr2_layout(x, batched):

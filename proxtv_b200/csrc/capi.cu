@@ -276,6 +276,33 @@ static int dev_dr2_vjp(const char* fn, size_t M, size_t N, int batch, int row_ma
     return cuda_ok(fn, dr2_vjp_device<T>(M, N, batch, row_major, maxit, tape, gout, gY, glam, ws, (cudaStream_t)stream), nullptr);
 }
 
+template <typename T>
+static int dev_drw_record(const char* fn, size_t M, size_t N, const T* Y, const T* W1, const T* W2, T* out, int maxit, void* tape,
+                          size_t tape_bytes, double* info, void* stream) {
+    if (M < 1 || N < 1) { fail(fn, "invalid shape (need M, N >= 1)", info); return 0; }
+    if (!Y || !out || !tape || (M > 1 && !W1) || (N > 1 && !W2)) { fail(fn, "NULL array", info); return 0; }
+    if (tape_bytes < drw_tape_bytes(M, N, maxit)) { fail(fn, "tape_bytes smaller than proxtv_DR2L1W_TV_tape_bytes()", info); return 0; }
+    if (!have_device(fn, info)) return 0;
+    WsGuard guard((cudaStream_t)stream);
+    void* ws = g_ws.get(ws_bytes_drw_record<T>(M, N));
+    if (!ws) { fail(fn, "out of memory", info); return 0; }
+    if (!cuda_ok(fn, drw_record_device<T>(M, N, Y, W1, W2, out, maxit, tape, ws, (Engine)g_engine, (cudaStream_t)stream), info)) return 0;
+    if (info) { info[INFO_ITERS] = maxit <= 0 ? MAX_ITERS_DR : maxit; info[INFO_RC] = RC_OK; }
+    return 1;
+}
+
+template <typename T>
+static int dev_drw_vjp(const char* fn, size_t M, size_t N, int maxit, const void* tape, const T* gout, T* gY, T* gW1, T* gW2, void* stream) {
+    if (M < 1 || N < 1) { fail(fn, "invalid shape (need M, N >= 1)", nullptr); return 0; }
+    if (!tape || !gout || !gY) { fail(fn, "NULL array", nullptr); return 0; }
+    if (!have_device(fn, nullptr)) return 0;
+    WsGuard guard((cudaStream_t)stream);
+    if (const char* why = drw_tape_check(tape, sizeof(T), M, N, maxit, (cudaStream_t)stream)) { fail(fn, why, nullptr); return 0; }
+    void* ws = g_ws.get(ws_bytes_drw_vjp<T>(M, N));
+    if (!ws) { fail(fn, "out of memory", nullptr); return 0; }
+    return cuda_ok(fn, drw_vjp_device<T>(M, N, maxit, tape, gout, gY, gW1, gW2, ws, (cudaStream_t)stream), nullptr);
+}
+
 }  // namespace
 
 extern "C" {
@@ -475,6 +502,19 @@ int proxtv_DR2L1W_TV_dev_f64(size_t M, size_t N, const double* Y, const double* 
     return run_drw<double>("proxtv_DR2L1W_TV_dev_f64", false, M, N, Y, W1, W2, out, maxit, info, (cudaStream_t)stream); }
 int proxtv_DR2L1W_TV_dev_f32(size_t M, size_t N, const float* Y, const float* W1, const float* W2, float* out, int maxit, double* info, void* stream) {
     return run_drw<float>("proxtv_DR2L1W_TV_dev_f32", false, M, N, Y, W1, W2, out, maxit, info, (cudaStream_t)stream); }
+size_t proxtv_DR2L1W_TV_tape_bytes(size_t M, size_t N, int maxit) { return drw_tape_bytes(M, N, maxit); }
+int proxtv_DR2L1W_TV_record_dev_f64(size_t M, size_t N, const double* Y, const double* W1, const double* W2, double* out, int maxit, void* tape,
+                                    size_t tape_bytes, double* info, void* stream) {
+    return dev_drw_record<double>("proxtv_DR2L1W_TV_record_dev_f64", M, N, Y, W1, W2, out, maxit, tape, tape_bytes, info, stream); }
+int proxtv_DR2L1W_TV_record_dev_f32(size_t M, size_t N, const float* Y, const float* W1, const float* W2, float* out, int maxit, void* tape,
+                                    size_t tape_bytes, double* info, void* stream) {
+    return dev_drw_record<float>("proxtv_DR2L1W_TV_record_dev_f32", M, N, Y, W1, W2, out, maxit, tape, tape_bytes, info, stream); }
+int proxtv_DR2L1W_TV_vjp_dev_f64(size_t M, size_t N, int maxit, const void* tape, const double* gout, double* gY, double* gW1, double* gW2,
+                                 void* stream) {
+    return dev_drw_vjp<double>("proxtv_DR2L1W_TV_vjp_dev_f64", M, N, maxit, tape, gout, gY, gW1, gW2, stream); }
+int proxtv_DR2L1W_TV_vjp_dev_f32(size_t M, size_t N, int maxit, const void* tape, const float* gout, float* gY, float* gW1, float* gW2,
+                                 void* stream) {
+    return dev_drw_vjp<float>("proxtv_DR2L1W_TV_vjp_dev_f32", M, N, maxit, tape, gout, gY, gW1, gW2, stream); }
 
 int proxtv_PD2_TV_dev_f64(const double* y, double* lambdas, double* dims, double* x, double* info, int* ns, int nds, int npen, int maxIters, void* stream) {
     return run_pd<double>("proxtv_PD2_TV_dev_f64", 0, false, y, lambdas, nullptr, dims, x, info, ns, nds, npen, maxIters, (cudaStream_t)stream); }

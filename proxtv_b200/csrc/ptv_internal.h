@@ -125,6 +125,18 @@ template <typename T> cudaError_t dr2_record_device(size_t M, size_t N, int batc
 const char* dr2_tape_check(const void* tape, size_t elem, size_t M, size_t N, int batch, int row_major, int maxit, cudaStream_t st);
 template <typename T> cudaError_t dr2_vjp_device(size_t M, size_t N, int batch, int row_major, int maxit, const void* tape, const T* gout,
                                                  T* gY, double* glam, void* ws, cudaStream_t st);
+// ---- exact backward pass of DR2L1W_TV (dr2_vjp.cu, DESIGN.md section 12) ----
+size_t drw_tape_bytes(size_t M, size_t N, int maxit);                    // header + (2K + 2) passes x two bitsets
+template <typename T> size_t ws_bytes_drw_record(size_t M, size_t N);
+template <typename T> size_t ws_bytes_drw_vjp(size_t M, size_t N);
+// drw_device's iteration with plain prox passes (bit for bit the same output), writing the segmentation tape of every pass.  The
+// tape's size (drw_tape_bytes) and the arguments are checked by the caller.
+template <typename T> cudaError_t drw_record_device(size_t M, size_t N, const T* Y, const T* W1, const T* W2, T* out, int maxit, void* tape,
+                                                    void* ws, Engine eng, cudaStream_t st);
+const char* drw_tape_check(const void* tape, size_t elem, size_t M, size_t N, int maxit, cudaStream_t st);
+// gY, and per-edge gW1 / gW2 unless nullptr, from the tape alone
+template <typename T> cudaError_t drw_vjp_device(size_t M, size_t N, int maxit, const void* tape, const T* gout, T* gY, T* gW1, T* gW2,
+                                                 void* ws, cudaStream_t st);
 
 // PDR_TV (src/TVNDopt.cpp:280-500): parallel Douglas-Rachford, fixed iteration count; same workspace as pd_device
 template <typename T> int pdr_device(const T* y, const double* lambdas_scaled, const double* dims, T* x, double* info,
