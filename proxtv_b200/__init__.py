@@ -8,8 +8,8 @@ device the calls raise.
 
 Extensions the reference lacks (SURVEY.md section 8b): a leading batch dimension (``tv1_1d_batched``,
 ``tv1w_1d_batched``, ``tv1_2d_batched``), float32, and torch CUDA tensors as inputs (device-resident path: no PCIe
-traffic, no host transposes -- a C-ordered tensor is handled by swapping the kernels' stride roles).  The batched 1D functions
-and ``tv1_2d`` / ``tv1_2d_batched`` are differentiable on torch tensors (exact backward kernels).
+traffic, no host transposes -- a C-ordered tensor is handled by swapping the kernels' stride roles).  The batched 1D functions,
+``tv1_2d`` / ``tv1_2d_batched``, ``tv1w_2d`` and the N-D ``tvgen_pdr`` are differentiable on torch tensors (exact backward kernels).
 """
 import ctypes as C
 
@@ -637,18 +637,164 @@ def tvgen(x, ws, ds, ps, n_threads=1, max_iters=0):
 tvgen.last_info = None
 
 
+def _f_contiguous(x):
+    """True when the tensor's memory is the column-major (Fortran) order of its shape (axes of size 1 may have any stride)."""
+    step = 1
+    for n, st in zip(x.shape, x.stride()):
+        if n != 1 and st != step:
+            return False
+        step *= n
+    return True
+
+
+def _pdr_layout(x, ds):
+    """(ns, dims, xin) of an N-D CUDA tensor for the column-major solver: a Fortran-ordered x is taken as it is, with its shape and
+    axes; anything else is a C-ordered array (copied to C order unless it is one already), which is the column-major array of the
+    reversed shape, so axis a becomes nds + 1 - a and no transpose is made."""
+    import torch
+    assert x.is_cuda and x.dtype in (torch.float64, torch.float32) and x.dim() >= 1
+    if _f_contiguous(x) and not x.is_contiguous():
+        return [int(n) for n in x.shape], [float(d) for d in ds], x
+    xin = x.contiguous()
+    return _pdr_c_order(xin.shape, ds) + (xin,)
+
+
+def _pdr_c_order(shape, ds):
+    """(ns, dims) of the solver for a C-ordered array of this shape and 1-based axes ds: the reversed shape, axis a -> nds + 1 - a."""
+    nd = len(shape)
+    return [int(n) for n in shape][::-1], [float(nd + 1 - d) for d in ds]
+
+
+def _pdr_args(ns, dims, lam):
+    return np.array(ns, dtype=np.int32), np.array(dims, dtype=np.float64), np.array(lam, dtype=np.float64)
+
+
+def _pdr_torch(xin, ns, dims, lam, max_iters):
+    """proxtv_PDR_TV_dev_* on the current stream; lam is a float64 copy of the penalties (scaled in place by the call)."""
+    import torch
+    nsa, dsa, lama = _pdr_args(ns, dims, lam)
+    out = torch.empty_strided(xin.shape, xin.stride(), dtype=xin.dtype, device=xin.device)
+    info = np.zeros(_N_INFO)
+    lib = require_device()
+    st = C.c_void_p(torch.cuda.current_stream(xin.device).cuda_stream)
+    fn = lib.proxtv_PDR_TV_dev_f32 if xin.dtype == torch.float32 else lib.proxtv_PDR_TV_dev_f64
+    with torch.cuda.device(xin.device):
+        ok = fn(C.c_void_p(xin.data_ptr()), _ptr(lama), _ptr(dsa), C.c_void_p(out.data_ptr()), _ptr(info), _ptr(nsa), len(ns), len(lam),
+                int(max_iters), st)
+    _check(ok and info[2] != 3, "PDR_TV (device)")
+    tvgen_pdr.last_info = info
+    return out
+
+
+_PDR_FN = None
+
+
+def _pdr_fn():
+    """torch.autograd.Function around PDR_TV on the device (made on first use, so that numpy users never import torch).
+
+    forward(xin, ws_t, ns, dims, lam, max_iters): xin column-major over ns (see _pdr_layout), lam the unscaled penalties as floats,
+    ws_t the 1-D tensor they came from (or None; only receives the gradient).  proxtv_PDR_TV_record_dev_* -- the solve of _pdr_torch,
+    keeping the segmentation tape of every pass that reaches the result (a uint8 CUDA tensor, proxtv_PDR_TV_tape_bytes() long) on ctx.
+    backward: proxtv_PDR_TV_vjp_dev_* on the current stream; the gradient of ws_t is npen * glam (glam: the gradients of the scaled
+    penalties, float64)."""
+    global _PDR_FN
+    if _PDR_FN is not None:
+        return _PDR_FN
+    import torch
+    from torch.autograd.function import once_differentiable
+
+    class PDR(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, xin, ws_t, ns, dims, lam, max_iters):
+            nsa, dsa, lama = _pdr_args(ns, dims, lam)
+            lib = require_device()
+            out = torch.empty_strided(xin.shape, xin.stride(), dtype=xin.dtype, device=xin.device)
+            nb = int(lib.proxtv_PDR_TV_tape_bytes(_ptr(nsa), len(ns), len(lam), int(max_iters)))
+            tape = torch.empty(max(nb, 256), dtype=torch.uint8, device=xin.device)
+            info = np.zeros(_N_INFO)
+            st = C.c_void_p(torch.cuda.current_stream(xin.device).cuda_stream)
+            fn = lib.proxtv_PDR_TV_record_dev_f32 if xin.dtype == torch.float32 else lib.proxtv_PDR_TV_record_dev_f64
+            with torch.cuda.device(xin.device):
+                ok = fn(C.c_void_p(xin.data_ptr()), _ptr(lama), _ptr(dsa), C.c_void_p(out.data_ptr()), _ptr(info), _ptr(nsa), len(ns),
+                        len(lam), int(max_iters), C.c_void_p(tape.data_ptr()), tape.numel(), st)
+            _check(ok and info[2] != 3, "PDR_TV (recorded, device)")
+            tvgen_pdr.last_info = info
+            ctx.save_for_backward(tape)
+            ctx.geom = (nsa, dsa, int(max_iters), tuple(out.shape), out.stride(), out.dtype)
+            ctx.ws_meta = (ws_t.dtype, ws_t.device, ws_t.shape) if ws_t is not None else None
+            return out
+
+        @staticmethod
+        @once_differentiable
+        def backward(ctx, gout):
+            (tape,) = ctx.saved_tensors
+            nsa, dsa, max_iters, shape, stride, dt = ctx.geom
+            need_x, need_ws = ctx.needs_input_grad[:2]
+            npen = len(dsa)
+            dev = tape.device
+            g = torch.empty_strided(shape, stride, dtype=dt, device=dev)      # the upstream gradient in the output's layout
+            g.copy_(gout)
+            gY = torch.empty_strided(shape, stride, dtype=dt, device=dev)
+            glam = torch.empty(npen, dtype=torch.float64, device=dev) if need_ws else None
+            lib = require_device()
+            st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            fn = lib.proxtv_PDR_TV_vjp_dev_f32 if dt == torch.float32 else lib.proxtv_PDR_TV_vjp_dev_f64
+            with torch.cuda.device(dev):
+                _check(fn(_ptr(nsa), len(nsa), npen, _ptr(dsa), max_iters, C.c_void_p(tape.data_ptr()), C.c_void_p(g.data_ptr()),
+                          C.c_void_p(gY.data_ptr()), C.c_void_p(glam.data_ptr()) if glam is not None else None, st),
+                       "PDR_TV backward (device)")
+            g_ws = None
+            if need_ws:
+                dtw, devw, shw = ctx.ws_meta
+                g_ws = (glam * float(npen)).to(dtype=dtw, device=devw).reshape(shw)
+            return (gY if need_x else None), g_ws, None, None, None, None
+
+    _PDR_FN = PDR
+    return PDR
+
+
+def _pdr_torch_entry(x, ws, ds, max_iters):
+    """The torch path of tvgen_pdr: differentiable when grad mode is on and x, or ws given as a tensor, requires grad; otherwise
+    exactly _pdr_torch.  ws (list, ndarray or 1-D tensor) is read, never written."""
+    import torch
+    ws_t = ws if _is_torch(ws) else None
+    if ws_t is not None:
+        assert ws_t.dim() == 1, "ws must be a 1-D tensor of one penalty per term"
+        lam = [float(v) for v in ws_t.detach().to(device="cpu", dtype=torch.float64).numpy()]
+    else:
+        lam = [float(v) for v in np.asarray(ws, dtype=np.float64).ravel()]
+    ns, dims, xin = _pdr_layout(x, ds)
+    if torch.is_grad_enabled() and (x.requires_grad or (ws_t is not None and ws_t.requires_grad)):
+        return _pdr_fn().apply(xin, ws_t, ns, dims, lam, int(max_iters))
+    return _pdr_torch(xin, ns, dims, lam, max_iters)
+
+
 def tvgen_pdr(x, ws, ds, ps, n_threads=1, max_iters=0):
     r"""The same generalized TV prox as ``tvgen`` solved with the reference's Parallel Douglas-Rachford splitting, ``PDR_TV``
     (src/TVNDopt.cpp:280-500; reached from MATLAB only in the reference, matlab/solveTVND_PDR.cpp:89 -- SURVEY.md 8f N4).
 
     Runs exactly ``max_iters`` iterations (0: 35; the reference's loop has no stop test) and, like PD_TV, scales a float64
-    ndarray ``ws`` by ``len(ws)`` IN PLACE.  float64 only from numpy (use the C ABI's ``proxtv_PDR_TV_dev_f32`` for float32
-    device arrays); p = 1 norms only.  ``tvgen_pdr.last_info`` = [iterations, mean|x - x_last|, RC].
+    ndarray ``ws`` by ``len(ws)`` IN PLACE.  float64 only from numpy; p = 1 norms only.
+    ``tvgen_pdr.last_info`` = [iterations, mean|x - x_last|, RC].
+
+    torch: ``x`` a CUDA tensor (float32 or float64, any ndim >= 1) is solved on its device and current stream and the result is a
+    tensor of x's shape and dtype, in x's memory order when x is C- or Fortran-contiguous (no copy is made: a C-ordered tensor is the
+    column-major array of the reversed shape), else C order.  ``ds`` are 1-based axes of ``x`` as on the numpy path; an axis without
+    a term is a free batch axis.  ``ws`` may be a list, an ndarray or a 1-D tensor of any float dtype and device, and is never
+    modified on this path.  Differentiable with respect to ``x`` and a ``ws`` tensor: with grad mode on and one of them requiring
+    grad, the forward records the segmentation tape of every prox pass that reaches the result (2 bits per element per pass, kept
+    on the device until the backward: 1.6 GiB for a 512 x 512 x 256 volume with 3 terms at 35 iterations) and the backward is the
+    exact vector-Jacobian product of the fixed-iteration splitting that is computed (proxtv_PDR_TV_vjp_dev_*, DESIGN.md section 13),
+    run on the current CUDA stream; double backward is not supported.  The forward result is the same either way.
     """
     assert len(ws) == len(ds)
     assert len(ws) == len(ps)
     assert n_threads >= 1
     assert max_iters >= 0
+    if _is_torch(x):
+        if np.any(force_float_matrix(ps) != 1):
+            raise NotImplementedError("proxtv_b200 implements TV-L1 (p = 1) penalty terms only")
+        return _pdr_torch_entry(x, ws, ds, max_iters)
     info = np.zeros(_N_INFO)
     x = np.asfortranarray(x, dtype="float64")
     ws = force_float_matrix(ws)

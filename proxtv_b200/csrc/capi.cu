@@ -303,6 +303,51 @@ static int dev_drw_vjp(const char* fn, size_t M, size_t N, int maxit, const void
     return cuda_ok(fn, drw_vjp_device<T>(M, N, maxit, tape, gout, gY, gW1, gW2, ws, (cudaStream_t)stream), nullptr);
 }
 
+// Arguments of the PDR_TV tape entry points: nullptr when valid, else the reason.
+const char* pdr_args_check(const int* ns, int nds, int npen, const double* dims) {
+    if (nds < 1 || nds > PDR_TAPE_MAX_DIMS) return "invalid dimensions (need 1 <= nds <= 16)";
+    for (int i = 0; i < nds; i++) if (ns[i] < 0) return "invalid dimensions (negative size)";
+    if (npen < 1 || npen > 64) return "need 1 to 64 penalty terms";
+    long long n = 1; for (int i = 0; i < nds; i++) n *= ns[i];
+    FiberGeom g;
+    for (int i = 0; i < npen; i++) if (!geom_of(ns, nds, dims[i], n, &g)) return "invalid penalty dimensions";
+    return nullptr;
+}
+
+// PDR_TV as proxtv_PDR_TV_dev_* computes it (the same pdr_device call), writing the tape; every refusal comes before anything is
+// written, lambdas included.
+template <typename T>
+static int dev_pdr_record(const char* fn, const T* y, double* lambdas, const double* dims, T* x, double* info, const int* ns, int nds,
+                          int npen, int maxIters, void* tape, size_t tape_bytes, void* stream) {
+    if (!y || !x || !lambdas || !dims || !ns || !tape) { fail(fn, "NULL array", info); return 0; }
+    if (const char* why = pdr_args_check(ns, nds, npen, dims)) { fail(fn, why, info); return 0; }
+    for (int i = 0; i < npen; i++) if (!(lambdas[i] >= 0)) { fail(fn, "negative penalty", info); return 0; }
+    if (tape_bytes < pdr_tape_bytes(ns, nds, npen, maxIters)) { fail(fn, "tape_bytes smaller than proxtv_PDR_TV_tape_bytes()", info); return 0; }
+    if (!have_device(fn, info)) return 0;
+    WsGuard guard((cudaStream_t)stream);
+    long long n = 1; for (int i = 0; i < nds; i++) n *= ns[i];
+    void* ws = g_ws.get(ws_bytes_pd<T>(n, npen > 2 ? npen : 2));
+    if (!ws) { fail(fn, "out of memory", info); return 0; }
+    if (!cuda_ok(fn, pdr_tape_header(tape, sizeof(T), ns, nds, npen, dims, maxIters, (cudaStream_t)stream), info)) return 0;
+    for (int i = 0; i < npen; i++) lambdas[i] *= npen;                                  // as run_pd
+    if (!pdr_device<T>(y, lambdas, dims, x, info, ns, nds, npen, maxIters, ws, (Engine)g_engine, (cudaStream_t)stream, tape)) {
+        fail(fn, "device solver failed", info); return 0; }
+    return 1;
+}
+
+template <typename T>
+static int dev_pdr_vjp(const char* fn, const int* ns, int nds, int npen, const double* dims, int maxIters, const void* tape, const T* gout,
+                       T* gY, double* glam, void* stream) {
+    if (!ns || !dims || !tape || !gout || !gY) { fail(fn, "NULL array", nullptr); return 0; }
+    if (const char* why = pdr_args_check(ns, nds, npen, dims)) { fail(fn, why, nullptr); return 0; }
+    if (!have_device(fn, nullptr)) return 0;
+    WsGuard guard((cudaStream_t)stream);
+    if (const char* why = pdr_tape_check(tape, sizeof(T), ns, nds, npen, dims, maxIters, (cudaStream_t)stream)) { fail(fn, why, nullptr); return 0; }
+    void* ws = g_ws.get(ws_bytes_pdr_vjp<T>(ns, nds, npen, dims, glam != nullptr));
+    if (!ws) { fail(fn, "out of memory", nullptr); return 0; }
+    return cuda_ok(fn, pdr_vjp_device<T>(ns, nds, npen, dims, maxIters, tape, gout, gY, glam, ws, (cudaStream_t)stream), nullptr);
+}
+
 }  // namespace
 
 extern "C" {
@@ -528,6 +573,23 @@ int proxtv_PDR_TV_dev_f64(const double* y, double* lambdas, double* dims, double
     return run_pd<double>("proxtv_PDR_TV_dev_f64", 2, false, y, lambdas, nullptr, dims, x, info, ns, nds, npen, maxIters, (cudaStream_t)stream); }
 int proxtv_PDR_TV_dev_f32(const float* y, double* lambdas, double* dims, float* x, double* info, int* ns, int nds, int npen, int maxIters, void* stream) {
     return run_pd<float>("proxtv_PDR_TV_dev_f32", 2, false, y, lambdas, nullptr, dims, x, info, ns, nds, npen, maxIters, (cudaStream_t)stream); }
+size_t proxtv_PDR_TV_tape_bytes(const int* ns, int nds, int npen, int maxIters) {
+    if (!ns || nds < 1 || nds > PDR_TAPE_MAX_DIMS || npen < 1 || npen > 64) return 0;
+    for (int i = 0; i < nds; i++) if (ns[i] < 0) return 0;
+    return pdr_tape_bytes(ns, nds, npen, maxIters);
+}
+int proxtv_PDR_TV_record_dev_f64(const double* y, double* lambdas, double* dims, double* x, double* info, int* ns, int nds, int npen,
+                                 int maxIters, void* tape, size_t tape_bytes, void* stream) {
+    return dev_pdr_record<double>("proxtv_PDR_TV_record_dev_f64", y, lambdas, dims, x, info, ns, nds, npen, maxIters, tape, tape_bytes, stream); }
+int proxtv_PDR_TV_record_dev_f32(const float* y, double* lambdas, double* dims, float* x, double* info, int* ns, int nds, int npen,
+                                 int maxIters, void* tape, size_t tape_bytes, void* stream) {
+    return dev_pdr_record<float>("proxtv_PDR_TV_record_dev_f32", y, lambdas, dims, x, info, ns, nds, npen, maxIters, tape, tape_bytes, stream); }
+int proxtv_PDR_TV_vjp_dev_f64(const int* ns, int nds, int npen, const double* dims, int maxIters, const void* tape, const double* gout,
+                              double* gY, double* glam, void* stream) {
+    return dev_pdr_vjp<double>("proxtv_PDR_TV_vjp_dev_f64", ns, nds, npen, dims, maxIters, tape, gout, gY, glam, stream); }
+int proxtv_PDR_TV_vjp_dev_f32(const int* ns, int nds, int npen, const double* dims, int maxIters, const void* tape, const float* gout,
+                              float* gY, double* glam, void* stream) {
+    return dev_pdr_vjp<float>("proxtv_PDR_TV_vjp_dev_f32", ns, nds, npen, dims, maxIters, tape, gout, gY, glam, stream); }
 int proxtv_PD_TV_f32(const float* y, double* lambdas, double* dims, float* x, double* info, int* ns, int nds, int npen, int maxIters) {
     return run_pd<float>("proxtv_PD_TV_f32", 1, true, y, lambdas, nullptr, dims, x, info, ns, nds, npen, maxIters, 0); }
 

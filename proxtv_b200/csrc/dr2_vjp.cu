@@ -1,5 +1,6 @@
-// dr2_vjp.cu -- the exact backward passes of DR2_TV (DESIGN.md section 11) and of the weighted DR2L1W_TV (section 12, at the end): a
-// recorded forward that writes the segmentation tape of every prox pass, and the unrolled vector-Jacobian product driven by that tape.
+// dr2_vjp.cu -- the exact backward passes of DR2_TV (DESIGN.md section 11), of the weighted DR2L1W_TV (section 12) and of the N-D
+// PDR_TV (section 13, at the end): a recorded forward that writes the segmentation tape of every prox pass, and the unrolled
+// vector-Jacobian product driven by that tape.
 //
 // DR2_TV is a fixed, unconverged splitting (35 iterations and a final projection), so the gradient is the one of the function actually
 // computed: the lane engine's schedule (solver.cu: dr2_lane_body), per image, storage type T, column prox P_c (axis 0, penalty w1) and
@@ -518,7 +519,166 @@ cudaError_t drw_vjp_device(size_t M, size_t N, int maxit, const void* tape, cons
 #undef RTRY
 }
 
+// ================================================================ PDR_TV (DESIGN.md section 13)
+// pdr_device (solver.cu) with k = npen terms, kk = (T)k, P_i the 1D prox along axis dims[i] with the scaled penalty lam_i, in T:
+//     z_i = Y ;  j = 0..K-1:  p_i = P_i(z_i) ; q = sum_i p_i / kk ; x = sum_i z_i / kk ; z_i = z_i + ((2 q - x) - p_i)     out = x (j = K-1)
+// The last iteration's passes do not reach out, so only the (K - 1) npen passes of j = 0..K-2 are recorded (pass p = j npen + i, after
+// the 256-byte header).  Backward for the upstream gradient G, in T with exactly these associations (sums term by term, i in order):
+//     v = G / kk ; gz_i = v                                                               (k_pdrv, start)
+//     j = K-2..0:  s = (gz_0 + gz_1) + ... ; sk = s / kk ; h = 2 sk - gz_0
+//                  i = 0..k-1:  gz_i = (gz_i - sk) + S_{j,i}(h) ; h = 2 sk - gz_{i+1}   (one VJP pass, then k_pdrv; the last term's step
+//                                                                                         forms the next iteration's s, sk and h)
+//     gY = (gz_0 + gz_1) + ...
+// Penalty gradients: glam_i = 0.0 ; glam_i = glam_i + sum(gw_{j,i}) for j = K-2..0, gw_{j,i} the edge gradients (vjp_core.cuh rule 4) of
+// pass (j, i) for its upstream gradient h, each sum img_sums' fixed two-stage double sum.  No atomics.
+struct PdrTapeHeader {
+    uint64_t magic;
+    int32_t elem, K, npen, nds;
+    int32_t ns[PDR_TAPE_MAX_DIMS];
+    uint8_t axis[64];                                                       // 0-based axis of each term
+    uint8_t pad[256 - 8 - 16 - 4 * PDR_TAPE_MAX_DIMS - 64];
+};
+static_assert(sizeof(PdrTapeHeader) == 256, "tape header is 256 bytes");
+static constexpr uint64_t PDR_TAPE_MAGIC = 0x3150415452524450ull;          // "PDRRTAP1"
+
+static long long pdr_elems(const int* ns, int nds) { long long n = 1; for (int i = 0; i < nds; i++) n *= ns[i]; return n; }
+
+size_t pdr_tape_bytes(const int* ns, int nds, int npen, int maxIters) {
+    const int K = maxIters <= 0 ? MAX_ITERS_DR : maxIters;
+    return 256 + (size_t)(K - 1) * (size_t)npen * 2 * ptvv::vjp_tape_set_bytes(pdr_elems(ns, nds));
+}
+
+template <typename T> cudaError_t pdr_tape_pass(void* tape, long long n, int p, const T* y, FiberGeom g, T lam, cudaStream_t st) {
+    const size_t sb = ptvv::vjp_tape_set_bytes(n);
+    uint32_t* F = (uint32_t*)((char*)tape + 256 + (size_t)p * 2 * sb);
+    return ptvv::fiber_tape<T>(y, g.nf, g.len, g.inc, lam, nullptr, F, F + sb / 4, st);
+}
+
+static PdrTapeHeader pdr_header(size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters) {
+    PdrTapeHeader h;
+    memset(&h, 0, sizeof(h));
+    h.magic = PDR_TAPE_MAGIC; h.elem = (int32_t)elem; h.K = maxIters <= 0 ? MAX_ITERS_DR : maxIters; h.npen = npen; h.nds = nds;
+    for (int i = 0; i < nds; i++) h.ns[i] = ns[i];
+    for (int i = 0; i < npen; i++) h.axis[i] = (uint8_t)(int)(dims[i] - 1);
+    return h;
+}
+
+cudaError_t pdr_tape_header(void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters, cudaStream_t st) {
+    const PdrTapeHeader h = pdr_header(elem, ns, nds, npen, dims, maxIters);
+    return cudaMemcpyAsync(tape, &h, sizeof(h), cudaMemcpyHostToDevice, st);
+}
+
+const char* pdr_tape_check(const void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters,
+                           cudaStream_t st) {
+    PdrTapeHeader h;
+    if (cudaMemcpyAsync(&h, tape, sizeof(h), cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) {
+        cudaGetLastError(); return "cannot read the tape header";
+    }
+    const PdrTapeHeader w = pdr_header(elem, ns, nds, npen, dims, maxIters);
+    if (h.magic != w.magic) return "not a PDR_TV tape";
+    if (h.elem != w.elem) return "tape recorded with another dtype";
+    if (h.nds != w.nds || memcmp(h.ns, w.ns, sizeof(h.ns)) != 0) return "tape recorded for another shape";
+    if (h.npen != w.npen || memcmp(h.axis, w.axis, sizeof(h.axis)) != 0) return "tape recorded with other penalty terms";
+    if (h.K != w.K) return "tape recorded with another iteration count";
+    return nullptr;
+}
+
+template <typename T> size_t ws_bytes_pdr_vjp(const int* ns, int nds, int npen, const double* dims, bool want_glam) {
+    const long long n = pdr_elems(ns, nds);
+    size_t vs = 0;
+    for (int i = 0; i < npen; i++) {
+        FiberGeom g{0, 0, 1};
+        geom_of(ns, nds, dims[i], n, &g);
+        const size_t b = ptvv::vjp_scratch_bytes(g.nf, g.len);
+        if (b > vs) vs = b;
+    }
+    return (size_t)(npen + 3 + (want_glam ? 1 : 0)) * al256((size_t)n * sizeof(T)) + al256(vs) + DR2V_SCRATCH;
+}
+
+template <typename T> struct PdrvPtrs { T* gz[64]; };
+
+// start: v = G / kk, every gz_l = v.  Else the step after term i's VJP pass (result sc): gz_i = (gz_i - sk) + sc, then h = 2 sk - gz_{i+1}
+// for the next term.  After the last term (and at the start): s = (gz_0 + gz_1) + ... ; more: sk = s / kk, h = 2 sk - gz_0 ; else gY = s.
+template <typename T>
+__global__ void k_pdrv(PdrvPtrs<T> a, int npen, int i, bool start, bool more, const T* __restrict__ G, const T* __restrict__ sc,
+                       T* __restrict__ Sk, T* __restrict__ h, T* __restrict__ gY, long long n) {
+    const T kk = (T)npen;
+    GRID_STRIDE(q, n) {
+        T v;
+        if (start) {
+            v = G[q] / kk;
+            for (int l = 0; l < npen; l++) a.gz[l][q] = v;
+        } else {
+            const T sk = Sk[q];
+            v = (a.gz[i][q] - sk) + sc[q];
+            a.gz[i][q] = v;
+            if (i + 1 < npen) { h[q] = T(2) * sk - a.gz[i + 1][q]; continue; }
+        }
+        // every gz_l holds its new value here; the last term's (all of them at the start) is v
+        auto cur = [&](int l) { return (start || l == npen - 1) ? v : a.gz[l][q]; };
+        T s = cur(0);
+        for (int l = 1; l < npen; l++) s = s + cur(l);
+        if (more) {
+            const T sk = s / kk;
+            Sk[q] = sk;
+            h[q] = T(2) * sk - cur(0);
+        } else {
+            gY[q] = s;
+        }
+    }
+}
+
+template <typename T>
+cudaError_t pdr_vjp_device(const int* ns, int nds, int npen, const double* dims, int maxIters, const void* tape, const T* gout, T* gY,
+                           double* glam, void* ws, cudaStream_t st) {
+#define RTRY(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) return e__; } while (0)
+    const long long n = pdr_elems(ns, nds);
+    const int K = maxIters <= 0 ? MAX_ITERS_DR : maxIters;
+    if (glam) RTRY(cudaMemsetAsync(glam, 0, (size_t)npen * sizeof(double), st));
+    if (n == 0) return cudaSuccess;
+    const size_t ab = al256((size_t)n * sizeof(T)), sb = ptvv::vjp_tape_set_bytes(n);
+    FiberGeom g[64];
+    size_t vs = 0;
+    for (int i = 0; i < npen; i++) {
+        geom_of(ns, nds, dims[i], n, &g[i]);
+        const size_t b = ptvv::vjp_scratch_bytes(g[i].nf, g[i].len);
+        if (b > vs) vs = b;
+    }
+    char* w = (char*)ws;
+    PdrvPtrs<T> a;
+    for (int i = 0; i < npen; i++) { a.gz[i] = (T*)w; w += ab; }
+    T* Sk = (T*)w; w += ab;
+    T* h = (T*)w; w += ab;
+    T* sc = (T*)w; w += ab;
+    T* gw = nullptr;
+    if (glam) { gw = (T*)w; w += ab; }
+    void* vscr = w; w += al256(vs);
+    double* scratch = (double*)w;
+    const char* tb = (const char*)tape + 256;
+    const unsigned ge = ew_grid(n);
+    auto step = [&](bool start, int i, bool more) -> cudaError_t {
+        KernelSpan sp(KC_ELEMENTWISE, 1, st);
+        k_pdrv<T><<<ge, 256, 0, st>>>(a, npen, i, start, more, gout, sc, Sk, h, gY, n);
+        return cudaGetLastError();
+    };
+    RTRY(step(true, npen - 1, K >= 2));
+    for (int j = K - 2; j >= 0; j--) {
+        for (int i = 0; i < npen; i++) {
+            const uint32_t* F = (const uint32_t*)(tb + (size_t)(j * npen + i) * 2 * sb);
+            RTRY(ptvv::vjp_fibers_tape<T>(F, F + sb / 4, h, sc, gw, g[i].nf, g[i].len, g[i].inc, vscr, st));
+            // one "image" of all edges: img_sums adds its sum to glam[2 * 0 + i]
+            if (glam) RTRY(img_sums<T>(gw, g[i].nf * (long long)(g[i].len - 1), 1, scratch, nullptr, glam, i, 1.0, st));
+            RTRY(step(false, i, j > 0));
+        }
+    }
+    return cudaSuccess;
+#undef RTRY
+}
+
 #define INST(T) \
+    template cudaError_t pdr_tape_pass<T>(void*, long long, int, const T*, FiberGeom, T, cudaStream_t); \
+    template size_t ws_bytes_pdr_vjp<T>(const int*, int, int, const double*, bool); \
+    template cudaError_t pdr_vjp_device<T>(const int*, int, int, const double*, int, const void*, const T*, T*, double*, void*, cudaStream_t); \
     template size_t ws_bytes_dr2_record<T>(size_t, size_t, int); \
     template size_t ws_bytes_dr2_vjp<T>(size_t, size_t, int); \
     template cudaError_t dr2_record_device<T>(size_t, size_t, int, int, const T*, T, T, T*, int, void*, void*, Engine, cudaStream_t); \

@@ -138,9 +138,27 @@ const char* drw_tape_check(const void* tape, size_t elem, size_t M, size_t N, in
 template <typename T> cudaError_t drw_vjp_device(size_t M, size_t N, int maxit, const void* tape, const T* gout, T* gY, T* gW1, T* gW2,
                                                  void* ws, cudaStream_t st);
 
-// PDR_TV (src/TVNDopt.cpp:280-500): parallel Douglas-Rachford, fixed iteration count; same workspace as pd_device
+// PDR_TV (src/TVNDopt.cpp:280-500): parallel Douglas-Rachford, fixed iteration count; same workspace as pd_device.  tape: nullptr, or
+// the recorded forward's buffer (header written by the caller): the segmentation tape of every pass but the last iteration's
 template <typename T> int pdr_device(const T* y, const double* lambdas_scaled, const double* dims, T* x, double* info,
-                                     const int* ns, int nds, int npen, int maxIters, void* ws, Engine eng, cudaStream_t st);
+                                     const int* ns, int nds, int npen, int maxIters, void* ws, Engine eng, cudaStream_t st,
+                                     void* tape = nullptr);
+// the fibers of an n-element column-major array of dims ns[0..nds) along the 1-based axis `dim`; false when dim is not an axis
+bool geom_of(const int* ns, int nds, double dim, long long n, FiberGeom* g);
+// ---- exact backward pass of PDR_TV (dr2_vjp.cu, DESIGN.md section 13) ----
+constexpr int PDR_TAPE_MAX_DIMS = 16;                                    // axes the tape header holds
+size_t pdr_tape_bytes(const int* ns, int nds, int npen, int maxIters);    // header + (K - 1) npen passes x two bitsets
+// the tape of pass p (output y over the fibers g, penalty lam) into a tape of n-element passes
+template <typename T> cudaError_t pdr_tape_pass(void* tape, long long n, int p, const T* y, FiberGeom g, T lam, cudaStream_t st);
+// writes the 256-byte header (arguments checked by the caller; axes = dims - 1)
+cudaError_t pdr_tape_header(void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters, cudaStream_t st);
+// validates a tape's header against the arguments (one stream synchronisation): nullptr ok, else the reason
+const char* pdr_tape_check(const void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters,
+                           cudaStream_t st);
+template <typename T> size_t ws_bytes_pdr_vjp(const int* ns, int nds, int npen, const double* dims, bool want_glam);
+// gY, and glam[npen] (d/d of the scaled penalties) unless nullptr, from the tape alone; arguments checked by the caller
+template <typename T> cudaError_t pdr_vjp_device(const int* ns, int nds, int npen, const double* dims, int maxIters, const void* tape,
+                                                 const T* gout, T* gY, double* glam, void* ws, cudaStream_t st);
 
 }  // namespace ptv
 

@@ -467,7 +467,7 @@ template <typename T> size_t ws_bytes_pd(long long n, int npen) {
     return (size_t)arrays * align256((size_t)n * sizeof(T)) + SCRATCH_BYTES + align256(2 * 64 * sizeof(void*));
 }
 
-static bool geom_of(const int* ns, int nds, double dim, long long n, FiberGeom* g) {
+bool geom_of(const int* ns, int nds, double dim, long long n, FiberGeom* g) {
     int d = (int)(dim - 1);                                                   // TV2Dopt.cpp:171, TVNDopt.cpp:175
     if (d < 0 || d >= nds) return false;
     long long inc = 1;
@@ -568,9 +568,11 @@ int pd_device(const T* y, const double* lam, const double* dims, T* x, double* i
 // reference calls TV1D_denoise, :439 -- the same minimiser as every other exact 1D solver here) ; q = mean p_i ; x = mean z_i ;
 // z_i += 2 q - x - p_i ; stop = mean|x - x_last|.  The result x is the average of the z_i BEFORE the last update, like the
 // reference's.  info = {iters, stop, RC_ITERS if iters >= 35 else RC_OK}; the stop value is read back once, after the loop.
+// tape != nullptr (the recorded forward, dr2_vjp.cu): after each pass of the iterations but the last, the segmentation tape of its
+// output p_i is written as pass j * npen + i of the tape; nothing else changes.
 template <typename T>
 int pdr_device(const T* y, const double* lam, const double* dims, T* x, double* info, const int* ns, int nds, int npen,
-               int maxIters, void* ws, Engine eng, cudaStream_t st) {
+               int maxIters, void* ws, Engine eng, cudaStream_t st, void* tape) {
     long long n = 1; for (int i = 0; i < nds; i++) n *= ns[i];
     if (maxIters <= 0) maxIters = MAX_ITERS_DR;                                                       // :320
     if (npen > 64) { printf("PDR_TV: more than 64 penalty terms are not supported\n"); if (info) info[INFO_RC] = RC_ERROR; return 0; }
@@ -594,8 +596,10 @@ int pdr_device(const T* y, const double* lam, const double* dims, T* x, double* 
         PTV_TRY(ew_div_scalar<T>(y, x, n, (T)npen, st));                                              // :365-370
         for (int i = 0; i < npen; i++) PTV_TRY(cudaMemcpyAsync(hz[i], y, (size_t)n * sizeof(T), cudaMemcpyDeviceToDevice, st));
         while (iters < maxIters) {                                                                    // :394
-            for (int i = 0; i < npen; i++)
+            for (int i = 0; i < npen; i++) {
                 PTV_TRY(prox_fibers<T>(hz[i], nullptr, IN_A, hp[i], 0, g[i], (T)lam[i], nullptr, eng, scr, st, 3 * n));  // :409-449
+                if (tape && iters < maxIters - 1) PTV_TRY(pdr_tape_pass<T>(tape, n, iters * npen + i, hp[i], g[i], (T)lam[i], st));
+            }
             PTV_TRY(ew_pdr_combine<T>(dp, dz, hp, hz, npen, x, n, scratch, dres, st));                        // :456-475
             iters++;
         }
@@ -617,7 +621,8 @@ int pdr_device(const T* y, const double* lam, const double* dims, T* x, double* 
     template size_t ws_bytes_pd<T>(long long, int); \
     template int pd2_device<T>(const T*, const double*, const double*, T*, double*, const int*, int, int, int, void*, Engine, cudaStream_t); \
     template int pd_device<T>(const T*, const double*, const double*, T*, double*, const int*, int, int, int, void*, Engine, cudaStream_t); \
-    template int pdr_device<T>(const T*, const double*, const double*, T*, double*, const int*, int, int, int, void*, Engine, cudaStream_t);
+    template int pdr_device<T>(const T*, const double*, const double*, T*, double*, const int*, int, int, int, void*, Engine, cudaStream_t, \
+                               void*);
 INST(double)
 INST(float)
 
