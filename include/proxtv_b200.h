@@ -229,15 +229,15 @@ int proxtv_PDR_TV_dev_f32(const float *y, double *lambdas, double *dims, float *
 /* Exact backward pass of PDR_TV (DESIGN.md section 13).  The gradient is the one of the function computed: K = maxIters (0: 35)
  * iterations of npen 1D prox passes and one combine, every pass with the Jacobian of proxtv_prox_fibers_vjp_dev_*; the last
  * iteration's passes do not reach x.  tape_bytes: 256 + (K - 1) npen 2 align256(4 ceil(n / 32)) for n = prod ns, 0 for invalid
- * arguments.  record: the arguments of proxtv_PDR_TV_dev_* plus a device buffer `tape` of at least that many bytes; x and info bit
- * for bit those of proxtv_PDR_TV_dev_* (the same solve, on every engine), lambdas scaled in place like it; writes a 256-byte header
- * and the segmentation tapes (proxtv_fiber_tape_dev_*) of the (K - 1) npen passes that reach x.  Returns 1 ok / 0 error (info[2] = 3
+ * arguments or a size that does not fit in size_t (record refuses that maxIters).  record: the arguments of proxtv_PDR_TV_dev_* plus
+ * a device buffer `tape` of at least that many bytes; x and info bit for bit those of proxtv_PDR_TV_dev_* (the same solve, on every
+ * engine), lambdas scaled in place like it; writes a 256-byte header and the segmentation tapes (proxtv_fiber_tape_dev_*) of the (K - 1) npen passes that reach x.  Returns 1 ok / 0 error (info[2] = 3
  * too); refused without writing anything, lambdas included: a NULL array, nds outside 1..16, a negative size, npen outside 1..64, a
  * dims entry that is not an axis, a negative penalty, tape_bytes too small.  vjp: from the tape alone, gY = the gradient with respect
  * to y for the upstream gradient gout (both laid out like y) and, unless glam is NULL, glam = npen doubles: the gradients of the
  * SCALED penalties (npen lambdas[i] of the caller; the caller's own penalty gets npen times glam[i]).  Deterministic (no atomics);
  * synchronises the stream once (reads the header).  Returns 1 ok / 0 error; refused without writing anything: NULL arrays, invalid
- * arguments as above, a header that does not match them (dtype, ns, axes, npen, maxIters) -- a DR2_TV or DR2L1W_TV tape included --
+ * arguments as above, a header that does not match them (dtype, ns, axes, npen, maxIters) -- the tape of any other solver included --
  * and a workspace (about npen + 3 arrays like y, one more with glam) that does not fit in device memory. */
 size_t proxtv_PDR_TV_tape_bytes(const int *ns, int nds, int npen, int maxIters);
 int proxtv_PDR_TV_record_dev_f64(const double *y, double *lambdas, double *dims, double *x, double *info, int *ns, int nds, int npen,
@@ -248,6 +248,39 @@ int proxtv_PDR_TV_vjp_dev_f64(const int *ns, int nds, int npen, const double *di
                               double *gY, double *glam, void *stream);
 int proxtv_PDR_TV_vjp_dev_f32(const int *ns, int nds, int npen, const double *dims, int maxIters, const void *tape, const float *gout,
                               float *gY, double *glam, void *stream);
+/* Exact backward passes of PD_TV and PD2_TV (DESIGN.md section 14).  The gradient is the one of the function computed: K iterations,
+ * K = the count the forward ran (its info[0]); the stop test only picks K, which is locally constant almost everywhere (where a
+ * perturbation changes K the map jumps).  Every prox pass has the Jacobian of proxtv_prox_fibers_vjp_dev_*.  tape_bytes: the capacity
+ * for maxIters (0: 35) iterations, 256 + P 2 align256(4 ceil(n / 32)) for n = prod ns with P = maxIters npen (PD_TV) or 2 maxIters
+ * (PD2_TV; 1 when npen = 1), 0 for invalid arguments or a size that does not fit in size_t (record refuses that maxIters).
+ * record: the arguments of proxtv_PD*_TV_dev_* plus a device buffer `tape` of at least that many bytes; x and info bit for bit
+ * those of proxtv_PD*_TV_dev_* (the same solve, on every engine); PD_TV scales lambdas in place like its sibling, PD2_TV does not; writes the segmentation tape of every pass and, after the solve, a 256-byte header with
+ * the iteration count run.  Returns 1 ok / 0 error (info[2] = 3 too); refused without writing anything, lambdas included: a NULL
+ * array, nds outside 1..16, a negative size, npen outside 1..64 (PD_TV) or 1..2 (PD2_TV), a dims entry that is not an axis, a negative
+ * penalty, tape_bytes too small.  vjp: iters = the forward's info[0]; from the tape alone, gY = the gradient with respect to y for the
+ * upstream gradient gout (both laid out like y) and, unless glam is NULL, glam = npen doubles: PD_TV's are the gradients of the SCALED
+ * penalties (the caller's own penalty gets npen times glam[i]), PD2_TV's those of the penalties as given.  Deterministic (no
+ * atomics); synchronises the stream once (reads the header).  Returns 1 ok / 0 error; refused without writing anything: NULL arrays,
+ * invalid arguments as above, a header that does not match them (dtype, ns, axes, npen, maxIters, iters) -- the tape of any other
+ * solver included -- and a workspace (about npen + 3 arrays like y, one more with glam) that does not fit in device memory. */
+size_t proxtv_PD_TV_tape_bytes(const int *ns, int nds, int npen, int maxIters);
+size_t proxtv_PD2_TV_tape_bytes(const int *ns, int nds, int npen, int maxIters);
+int proxtv_PD_TV_record_dev_f64(const double *y, double *lambdas, double *dims, double *x, double *info, int *ns, int nds, int npen,
+                                int maxIters, void *tape, size_t tape_bytes, void *stream);
+int proxtv_PD_TV_record_dev_f32(const float *y, double *lambdas, double *dims, float *x, double *info, int *ns, int nds, int npen,
+                                int maxIters, void *tape, size_t tape_bytes, void *stream);
+int proxtv_PD2_TV_record_dev_f64(const double *y, double *lambdas, double *dims, double *x, double *info, int *ns, int nds, int npen,
+                                 int maxIters, void *tape, size_t tape_bytes, void *stream);
+int proxtv_PD2_TV_record_dev_f32(const float *y, double *lambdas, double *dims, float *x, double *info, int *ns, int nds, int npen,
+                                 int maxIters, void *tape, size_t tape_bytes, void *stream);
+int proxtv_PD_TV_vjp_dev_f64(const int *ns, int nds, int npen, const double *dims, int maxIters, int iters, const void *tape,
+                             const double *gout, double *gY, double *glam, void *stream);
+int proxtv_PD_TV_vjp_dev_f32(const int *ns, int nds, int npen, const double *dims, int maxIters, int iters, const void *tape,
+                             const float *gout, float *gY, double *glam, void *stream);
+int proxtv_PD2_TV_vjp_dev_f64(const int *ns, int nds, int npen, const double *dims, int maxIters, int iters, const void *tape,
+                              const double *gout, double *gY, double *glam, void *stream);
+int proxtv_PD2_TV_vjp_dev_f32(const int *ns, int nds, int npen, const double *dims, int maxIters, int iters, const void *tape,
+                              const float *gout, float *gY, double *glam, void *stream);
 int proxtv_PD_TV_f32(const float *y, double *lambdas, double *dims, float *x, double *info, int *ns, int nds, int npen,
                      int maxIters);                                          /* host pointers, float32 */
 

@@ -9,7 +9,8 @@ device the calls raise.
 Extensions the reference lacks (SURVEY.md section 8b): a leading batch dimension (``tv1_1d_batched``,
 ``tv1w_1d_batched``, ``tv1_2d_batched``), float32, and torch CUDA tensors as inputs (device-resident path: no PCIe
 traffic, no host transposes -- a C-ordered tensor is handled by swapping the kernels' stride roles).  The batched 1D functions,
-``tv1_2d`` / ``tv1_2d_batched``, ``tv1w_2d`` and the N-D ``tvgen_pdr`` are differentiable on torch tensors (exact backward kernels).
+``tv1_2d`` (both methods) / ``tv1_2d_batched``, ``tv1w_2d`` and the N-D ``tvgen`` / ``tvgen_pdr`` are differentiable on torch
+tensors (exact backward kernels).
 """
 import ctypes as C
 
@@ -311,13 +312,19 @@ def tv1_2d(x, w, n_threads=1, max_iters=0, method="dr"):
     grad, the forward records a segmentation tape of every prox pass (2 bits per element per pass, kept on the device until the
     backward) and the backward is the exact vector-Jacobian product of the fixed 35-iteration splitting that is computed
     (proxtv_DR2_TV_vjp_dev_*, DESIGN.md section 11), run on the current CUDA stream; double backward is not supported.
+    ``method='pd'`` on a tensor is ``tvgen(x, [w, w], [1, 2], [1, 1], max_iters=max_iters)`` on it (PD2_TV, same code, same
+    gradients; the gradient of ``w`` is the sum of both terms' penalty gradients, in float64).
     """
     assert w >= 0
     assert method in _TV1_2D_METHODS
     if method not in ("dr", "pd"):
         raise NotImplementedError("proxtv_b200 implements the 'dr' and 'pd' 2D solvers (the GPU hot path); got %r" % method)
     if _is_torch(x):
-        assert method == "dr", "torch path implements the DR solver"
+        if method == "pd":
+            assert x.dim() == 2
+            assert not _is_torch(w) or w.dim() == 0, "w must be a number or a 0-dim tensor"
+            wf = float(w.detach()) if _is_torch(w) else float(w)
+            return _nd_torch_entry("PD2_TV", x, [wf, wf], w if _is_torch(w) else None, [1, 2], max_iters)
         return _dr2_torch_entry(x, w, max_iters, batched=False)
     x = np.asfortranarray(x, dtype="float64")
     assert x.ndim == 2
@@ -604,11 +611,33 @@ def tvgen(x, ws, ds, ps, n_threads=1, max_iters=0):
     PD_TV.  PD_TV scales the caller's ``ws`` by ``len(ws)`` IN PLACE when ``ws`` is a float64 ndarray (:576 does not
     copy in that case; src/TVNDopt.cpp:100-101).  Only p = 1 norms are implemented on the GPU path.
     Extension: a float32 ``x`` is solved in float32 (the reference would upcast) when ``len(ws) != 2``.
+    ``tvgen.last_info`` = [iterations, mean|x - x_last|, RC].  Both solvers stop when mean|x - x_last| <= 1e-6 or after
+    ``max_iters`` iterations (0: 35).
+
+    torch: ``x`` a CUDA tensor (float32 or float64, any ndim >= 1) is solved on its device and current stream with the same
+    dispatch (two terms: PD2_TV, whatever ``ds`` is; else PD_TV), and the result is a tensor of x's shape and dtype, in x's memory
+    order when x is C- or Fortran-contiguous (no copy is made: a C-ordered tensor is the column-major array of the reversed shape),
+    else C order.  ``ds`` are 1-based axes of ``x``; an axis without a term is a batch axis, but the stop test is global, so the
+    slices are solved independently only when the ``max_iters`` cap ends the solve (otherwise all stop together).  ``ws`` may be a
+    list, an ndarray or a 1-D tensor of any float dtype and device, and is never modified on this path.
+    Differentiable with respect to ``x`` and a ``ws`` tensor: with grad mode on and one of them requiring grad, the forward
+    records the segmentation tape of every prox pass (2 bits per element per pass, kept on the device until the backward) and the
+    backward is the exact vector-Jacobian product of the K iterations the forward ran (proxtv_PD_TV_vjp_dev_* /
+    proxtv_PD2_TV_vjp_dev_*, DESIGN.md section 14), run on the current CUDA stream.  K is picked by the stop test and has no
+    derivative of its own: where a perturbation changes K the computed map jumps.  The tape is allocated for ``max_iters``
+    iterations, not for the ones that turn out to run, so a large ``max_iters`` costs its memory up front: PD_TV on a
+    512 x 512 x 256 volume with 3 terms at 35 iterations is 105 passes x 16 MiB, about 1.64 GiB.  Double backward is not
+    supported.  The forward result is the same either way.
     """
     assert len(ws) == len(ds)
     assert len(ws) == len(ps)
     assert n_threads >= 1
     assert max_iters >= 0
+    if _is_torch(x):
+        if np.any(force_float_matrix(ps) != 1):
+            raise NotImplementedError("proxtv_b200 implements TV-L1 (p = 1) penalty terms only")
+        lam, ws_t = _ws_floats(ws)
+        return _nd_torch_entry("PD2_TV" if len(lam) == 2 else "PD_TV", x, lam, ws_t, ds, max_iters)
     info = np.zeros(_N_INFO)
     f32 = isinstance(x, np.ndarray) and x.dtype == np.float32 and len(ws) != 2
     x = np.asfortranarray(x, dtype="float32" if f32 else "float64")
@@ -669,58 +698,80 @@ def _pdr_args(ns, dims, lam):
     return np.array(ns, dtype=np.int32), np.array(dims, dtype=np.float64), np.array(lam, dtype=np.float64)
 
 
-def _pdr_torch(xin, ns, dims, lam, max_iters):
-    """proxtv_PDR_TV_dev_* on the current stream; lam is a float64 copy of the penalties (scaled in place by the call)."""
+def _ws_floats(ws):
+    """(the penalties as a list of floats, ws when it is a tensor else None) of a list, ndarray or 1-D tensor; ws is not written."""
+    import torch
+    if _is_torch(ws):
+        assert ws.dim() == 1, "ws must be a 1-D tensor of one penalty per term"
+        return [float(v) for v in ws.detach().to(device="cpu", dtype=torch.float64).numpy()], ws
+    return [float(v) for v in np.asarray(ws, dtype=np.float64).ravel()], None
+
+
+def _nd_fns(lib, solver, dtype):
+    """(no-grad solve, tape_bytes, record, vjp) entry points of solver ("PDR_TV", "PD_TV" or "PD2_TV") for a torch dtype."""
+    import torch
+    sfx = "f32" if dtype == torch.float32 else "f64"
+    return tuple(getattr(lib, "proxtv_%s_%s" % (solver, k)) for k in ("dev_" + sfx, "tape_bytes", "record_dev_" + sfx, "vjp_dev_" + sfx))
+
+
+def _nd_owner(solver):
+    """The public function whose ``last_info`` a solve of this solver sets."""
+    return tvgen_pdr if solver == "PDR_TV" else tvgen
+
+
+def _nd_torch(solver, xin, ns, dims, lam, max_iters):
+    """proxtv_<solver>_dev_* on the current stream; lam: the penalties as floats (the call gets a float64 copy, which PDR_TV and
+    PD_TV scale in place)."""
     import torch
     nsa, dsa, lama = _pdr_args(ns, dims, lam)
     out = torch.empty_strided(xin.shape, xin.stride(), dtype=xin.dtype, device=xin.device)
     info = np.zeros(_N_INFO)
-    lib = require_device()
+    fn = _nd_fns(require_device(), solver, xin.dtype)[0]
     st = C.c_void_p(torch.cuda.current_stream(xin.device).cuda_stream)
-    fn = lib.proxtv_PDR_TV_dev_f32 if xin.dtype == torch.float32 else lib.proxtv_PDR_TV_dev_f64
     with torch.cuda.device(xin.device):
         ok = fn(C.c_void_p(xin.data_ptr()), _ptr(lama), _ptr(dsa), C.c_void_p(out.data_ptr()), _ptr(info), _ptr(nsa), len(ns), len(lam),
                 int(max_iters), st)
-    _check(ok and info[2] != 3, "PDR_TV (device)")
-    tvgen_pdr.last_info = info
+    _check(ok and info[2] != 3, "%s (device)" % solver)
+    _nd_owner(solver).last_info = info
     return out
 
 
-_PDR_FN = None
+_ND_FN = None
 
 
-def _pdr_fn():
-    """torch.autograd.Function around PDR_TV on the device (made on first use, so that numpy users never import torch).
+def _nd_fn():
+    """torch.autograd.Function around the N-D solvers PDR_TV, PD_TV and PD2_TV on the device (made on first use, so that numpy users
+    never import torch).
 
-    forward(xin, ws_t, ns, dims, lam, max_iters): xin column-major over ns (see _pdr_layout), lam the unscaled penalties as floats,
-    ws_t the 1-D tensor they came from (or None; only receives the gradient).  proxtv_PDR_TV_record_dev_* -- the solve of _pdr_torch,
-    keeping the segmentation tape of every pass that reaches the result (a uint8 CUDA tensor, proxtv_PDR_TV_tape_bytes() long) on ctx.
-    backward: proxtv_PDR_TV_vjp_dev_* on the current stream; the gradient of ws_t is npen * glam (glam: the gradients of the scaled
-    penalties, float64)."""
-    global _PDR_FN
-    if _PDR_FN is not None:
-        return _PDR_FN
+    forward(xin, ws_t, solver, ns, dims, lam, max_iters): xin column-major over ns (see _pdr_layout), lam the unscaled penalties as
+    floats, ws_t the tensor they came from (or None; only receives the gradient; a 0-dim ws_t is one penalty shared by every term).
+    proxtv_<solver>_record_dev_* -- the solve of _nd_torch, keeping on ctx the segmentation tape (a uint8 CUDA tensor,
+    proxtv_<solver>_tape_bytes() long) and the iteration count the solve ran (the Dykstra solvers' stop rule picks it).
+    backward: proxtv_<solver>_vjp_dev_* on the current stream; the gradient of ws_t is npen * glam for PDR_TV and PD_TV (glam: the
+    gradients of the scaled penalties), glam for PD2_TV, in float64, summed over the terms for a 0-dim ws_t."""
+    global _ND_FN
+    if _ND_FN is not None:
+        return _ND_FN
     import torch
     from torch.autograd.function import once_differentiable
 
-    class PDR(torch.autograd.Function):
+    class ND(torch.autograd.Function):
         @staticmethod
-        def forward(ctx, xin, ws_t, ns, dims, lam, max_iters):
+        def forward(ctx, xin, ws_t, solver, ns, dims, lam, max_iters):
             nsa, dsa, lama = _pdr_args(ns, dims, lam)
-            lib = require_device()
+            _, tape_bytes, record, _ = _nd_fns(require_device(), solver, xin.dtype)
             out = torch.empty_strided(xin.shape, xin.stride(), dtype=xin.dtype, device=xin.device)
-            nb = int(lib.proxtv_PDR_TV_tape_bytes(_ptr(nsa), len(ns), len(lam), int(max_iters)))
+            nb = int(tape_bytes(_ptr(nsa), len(ns), len(lam), int(max_iters)))     # 0: too large; the record call refuses it
             tape = torch.empty(max(nb, 256), dtype=torch.uint8, device=xin.device)
             info = np.zeros(_N_INFO)
             st = C.c_void_p(torch.cuda.current_stream(xin.device).cuda_stream)
-            fn = lib.proxtv_PDR_TV_record_dev_f32 if xin.dtype == torch.float32 else lib.proxtv_PDR_TV_record_dev_f64
             with torch.cuda.device(xin.device):
-                ok = fn(C.c_void_p(xin.data_ptr()), _ptr(lama), _ptr(dsa), C.c_void_p(out.data_ptr()), _ptr(info), _ptr(nsa), len(ns),
-                        len(lam), int(max_iters), C.c_void_p(tape.data_ptr()), tape.numel(), st)
-            _check(ok and info[2] != 3, "PDR_TV (recorded, device)")
-            tvgen_pdr.last_info = info
+                ok = record(C.c_void_p(xin.data_ptr()), _ptr(lama), _ptr(dsa), C.c_void_p(out.data_ptr()), _ptr(info), _ptr(nsa),
+                            len(ns), len(lam), int(max_iters), C.c_void_p(tape.data_ptr()), tape.numel(), st)
+            _check(ok and info[2] != 3, "%s (recorded, device)" % solver)
+            _nd_owner(solver).last_info = info
             ctx.save_for_backward(tape)
-            ctx.geom = (nsa, dsa, int(max_iters), tuple(out.shape), out.stride(), out.dtype)
+            ctx.geom = (solver, nsa, dsa, int(max_iters), int(info[0]), tuple(out.shape), out.stride(), out.dtype)
             ctx.ws_meta = (ws_t.dtype, ws_t.device, ws_t.shape) if ws_t is not None else None
             return out
 
@@ -728,7 +779,7 @@ def _pdr_fn():
         @once_differentiable
         def backward(ctx, gout):
             (tape,) = ctx.saved_tensors
-            nsa, dsa, max_iters, shape, stride, dt = ctx.geom
+            solver, nsa, dsa, max_iters, iters, shape, stride, dt = ctx.geom
             need_x, need_ws = ctx.needs_input_grad[:2]
             npen = len(dsa)
             dev = tape.device
@@ -736,37 +787,37 @@ def _pdr_fn():
             g.copy_(gout)
             gY = torch.empty_strided(shape, stride, dtype=dt, device=dev)
             glam = torch.empty(npen, dtype=torch.float64, device=dev) if need_ws else None
-            lib = require_device()
+            vjp = _nd_fns(require_device(), solver, dt)[3]
+            it = () if solver == "PDR_TV" else (iters,)                          # PDR_TV runs exactly max_iters iterations
             st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            fn = lib.proxtv_PDR_TV_vjp_dev_f32 if dt == torch.float32 else lib.proxtv_PDR_TV_vjp_dev_f64
             with torch.cuda.device(dev):
-                _check(fn(_ptr(nsa), len(nsa), npen, _ptr(dsa), max_iters, C.c_void_p(tape.data_ptr()), C.c_void_p(g.data_ptr()),
-                          C.c_void_p(gY.data_ptr()), C.c_void_p(glam.data_ptr()) if glam is not None else None, st),
-                       "PDR_TV backward (device)")
+                _check(vjp(_ptr(nsa), len(nsa), npen, _ptr(dsa), max_iters, *it, C.c_void_p(tape.data_ptr()), C.c_void_p(g.data_ptr()),
+                           C.c_void_p(gY.data_ptr()), C.c_void_p(glam.data_ptr()) if glam is not None else None, st),
+                       "%s backward (device)" % solver)
             g_ws = None
             if need_ws:
                 dtw, devw, shw = ctx.ws_meta
-                g_ws = (glam * float(npen)).to(dtype=dtw, device=devw).reshape(shw)
-            return (gY if need_x else None), g_ws, None, None, None, None
+                gl = glam if solver == "PD2_TV" else glam * float(npen)
+                if len(shw) == 0:
+                    gl = gl.sum(dtype=torch.float64)
+                g_ws = gl.to(dtype=dtw, device=devw).reshape(shw)
+            return (gY if need_x else None), g_ws, None, None, None, None, None
 
-    _PDR_FN = PDR
-    return PDR
+    _ND_FN = ND
+    return ND
 
 
-def _pdr_torch_entry(x, ws, ds, max_iters):
-    """The torch path of tvgen_pdr: differentiable when grad mode is on and x, or ws given as a tensor, requires grad; otherwise
-    exactly _pdr_torch.  ws (list, ndarray or 1-D tensor) is read, never written."""
+def _nd_torch_entry(solver, x, lam, ws_t, ds, max_iters):
+    """The torch path of tvgen_pdr, tvgen and tv1_2d(method='pd'): differentiable when grad mode is on and x, or the penalty tensor
+    ws_t, requires grad; otherwise exactly _nd_torch.  lam: the penalties as floats; ws_t: None, a 1-D tensor of them, or a 0-dim
+    tensor shared by every term.  Nothing the caller passed is written."""
     import torch
-    ws_t = ws if _is_torch(ws) else None
-    if ws_t is not None:
-        assert ws_t.dim() == 1, "ws must be a 1-D tensor of one penalty per term"
-        lam = [float(v) for v in ws_t.detach().to(device="cpu", dtype=torch.float64).numpy()]
-    else:
-        lam = [float(v) for v in np.asarray(ws, dtype=np.float64).ravel()]
+    assert len(lam) == len(ds)
+    assert ws_t is None or tuple(ws_t.shape) in ((), (len(lam),)), "ws must be one penalty per term, or one 0-dim penalty for all"
     ns, dims, xin = _pdr_layout(x, ds)
     if torch.is_grad_enabled() and (x.requires_grad or (ws_t is not None and ws_t.requires_grad)):
-        return _pdr_fn().apply(xin, ws_t, ns, dims, lam, int(max_iters))
-    return _pdr_torch(xin, ns, dims, lam, max_iters)
+        return _nd_fn().apply(xin, ws_t, solver, ns, dims, lam, int(max_iters))
+    return _nd_torch(solver, xin, ns, dims, lam, max_iters)
 
 
 def tvgen_pdr(x, ws, ds, ps, n_threads=1, max_iters=0):
@@ -794,7 +845,8 @@ def tvgen_pdr(x, ws, ds, ps, n_threads=1, max_iters=0):
     if _is_torch(x):
         if np.any(force_float_matrix(ps) != 1):
             raise NotImplementedError("proxtv_b200 implements TV-L1 (p = 1) penalty terms only")
-        return _pdr_torch_entry(x, ws, ds, max_iters)
+        lam, ws_t = _ws_floats(ws)
+        return _nd_torch_entry("PDR_TV", x, lam, ws_t, ds, max_iters)
     info = np.zeros(_N_INFO)
     x = np.asfortranarray(x, dtype="float64")
     ws = force_float_matrix(ws)

@@ -79,6 +79,16 @@ SIGNATURES = {
     "proxtv_PDR_TV_record_dev_f32": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, _vp, C.c_size_t, _vp]),
     "proxtv_PDR_TV_vjp_dev_f64": (C.c_int, [_vp, C.c_int, C.c_int, _vp, C.c_int, _vp, _vp, _vp, _vp, _vp]),
     "proxtv_PDR_TV_vjp_dev_f32": (C.c_int, [_vp, C.c_int, C.c_int, _vp, C.c_int, _vp, _vp, _vp, _vp, _vp]),
+    "proxtv_PD_TV_tape_bytes": (C.c_size_t, [_vp, C.c_int, C.c_int, C.c_int]),
+    "proxtv_PD2_TV_tape_bytes": (C.c_size_t, [_vp, C.c_int, C.c_int, C.c_int]),
+    "proxtv_PD_TV_record_dev_f64": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, _vp, C.c_size_t, _vp]),
+    "proxtv_PD_TV_record_dev_f32": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, _vp, C.c_size_t, _vp]),
+    "proxtv_PD2_TV_record_dev_f64": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, _vp, C.c_size_t, _vp]),
+    "proxtv_PD2_TV_record_dev_f32": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, _vp, C.c_size_t, _vp]),
+    "proxtv_PD_TV_vjp_dev_f64": (C.c_int, [_vp, C.c_int, C.c_int, _vp, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp]),
+    "proxtv_PD_TV_vjp_dev_f32": (C.c_int, [_vp, C.c_int, C.c_int, _vp, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp]),
+    "proxtv_PD2_TV_vjp_dev_f64": (C.c_int, [_vp, C.c_int, C.c_int, _vp, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp]),
+    "proxtv_PD2_TV_vjp_dev_f32": (C.c_int, [_vp, C.c_int, C.c_int, _vp, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp]),
     "proxtv_PD_TV_f32": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int]),
     "proxtv_PDR_TV_dev_f64": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, _vp]),
     "proxtv_PDR_TV_dev_f32": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, _vp]),

@@ -322,7 +322,9 @@ static int dev_pdr_record(const char* fn, const T* y, double* lambdas, const dou
     if (!y || !x || !lambdas || !dims || !ns || !tape) { fail(fn, "NULL array", info); return 0; }
     if (const char* why = pdr_args_check(ns, nds, npen, dims)) { fail(fn, why, info); return 0; }
     for (int i = 0; i < npen; i++) if (!(lambdas[i] >= 0)) { fail(fn, "negative penalty", info); return 0; }
-    if (tape_bytes < pdr_tape_bytes(ns, nds, npen, maxIters)) { fail(fn, "tape_bytes smaller than proxtv_PDR_TV_tape_bytes()", info); return 0; }
+    const size_t need = pdr_tape_bytes(ns, nds, npen, maxIters);
+    if (need == 0) { fail(fn, "tape size does not fit in size_t (maxIters too large)", info); return 0; }
+    if (tape_bytes < need) { fail(fn, "tape_bytes smaller than proxtv_PDR_TV_tape_bytes()", info); return 0; }
     if (!have_device(fn, info)) return 0;
     WsGuard guard((cudaStream_t)stream);
     long long n = 1; for (int i = 0; i < nds; i++) n *= ns[i];
@@ -346,6 +348,51 @@ static int dev_pdr_vjp(const char* fn, const int* ns, int nds, int npen, const d
     void* ws = g_ws.get(ws_bytes_pdr_vjp<T>(ns, nds, npen, dims, glam != nullptr));
     if (!ws) { fail(fn, "out of memory", nullptr); return 0; }
     return cuda_ok(fn, pdr_vjp_device<T>(ns, nds, npen, dims, maxIters, tape, gout, gY, glam, ws, (cudaStream_t)stream), nullptr);
+}
+
+// PD_TV (pd2 false) or PD2_TV as proxtv_PD_TV_dev_* / proxtv_PD2_TV_dev_* compute it (the same pd_device / pd2_device call), writing
+// the tape and, after the solve, its header with the iterations run; every refusal comes before anything is written, lambdas included.
+template <typename T>
+static int dev_pd_record(const char* fn, bool pd2, const T* y, double* lambdas, const double* dims, T* x, double* info, const int* ns,
+                         int nds, int npen, int maxIters, void* tape, size_t tape_bytes, void* stream) {
+    if (!y || !x || !lambdas || !dims || !ns || !tape) { fail(fn, "NULL array", info); return 0; }
+    if (pd2 && (npen < 1 || npen > 2)) { fail(fn, "PD2_TV takes 1 or 2 penalty terms", info); return 0; }
+    if (const char* why = pdr_args_check(ns, nds, npen, dims)) { fail(fn, why, info); return 0; }
+    for (int i = 0; i < npen; i++) if (!(lambdas[i] >= 0)) { fail(fn, "negative penalty", info); return 0; }
+    const size_t need = pd_tape_bytes(pd2, ns, nds, npen, maxIters);
+    if (need == 0) { fail(fn, "tape size does not fit in size_t (maxIters too large)", info); return 0; }
+    if (tape_bytes < need) {
+        fail(fn, pd2 ? "tape_bytes smaller than proxtv_PD2_TV_tape_bytes()" : "tape_bytes smaller than proxtv_PD_TV_tape_bytes()", info);
+        return 0;
+    }
+    if (!have_device(fn, info)) return 0;
+    WsGuard guard((cudaStream_t)stream);
+    long long n = 1; for (int i = 0; i < nds; i++) n *= ns[i];
+    void* ws = g_ws.get(ws_bytes_pd<T>(n, npen > 2 ? npen : 2));
+    if (!ws) { fail(fn, "out of memory", info); return 0; }
+    double linfo[3] = {0, 0, RC_OK};                   // the header needs the iteration count even when the caller passes no info
+    double* pinfo = info ? info : linfo;
+    if (!pd2) for (int i = 0; i < npen; i++) lambdas[i] *= npen;                        // as run_pd
+    const int ok = pd2 ? pd2_device<T>(y, lambdas, dims, x, pinfo, ns, nds, npen, maxIters, ws, (Engine)g_engine, (cudaStream_t)stream, tape)
+                       : pd_device<T>(y, lambdas, dims, x, pinfo, ns, nds, npen, maxIters, ws, (Engine)g_engine, (cudaStream_t)stream, tape);
+    if (!ok) { fail(fn, "device solver failed", info); return 0; }
+    return cuda_ok(fn, pd_tape_header(pd2, tape, sizeof(T), ns, nds, npen, dims, maxIters, (int)pinfo[INFO_ITERS], (cudaStream_t)stream),
+                   info) ? 1 : 0;
+}
+
+template <typename T>
+static int dev_pd_vjp(const char* fn, bool pd2, const int* ns, int nds, int npen, const double* dims, int maxIters, int iters,
+                      const void* tape, const T* gout, T* gY, double* glam, void* stream) {
+    if (!ns || !dims || !tape || !gout || !gY) { fail(fn, "NULL array", nullptr); return 0; }
+    if (pd2 && (npen < 1 || npen > 2)) { fail(fn, "PD2_TV takes 1 or 2 penalty terms", nullptr); return 0; }
+    if (const char* why = pdr_args_check(ns, nds, npen, dims)) { fail(fn, why, nullptr); return 0; }
+    if (!have_device(fn, nullptr)) return 0;
+    WsGuard guard((cudaStream_t)stream);
+    if (const char* why = pd_tape_check(pd2, tape, sizeof(T), ns, nds, npen, dims, maxIters, iters, (cudaStream_t)stream)) {
+        fail(fn, why, nullptr); return 0; }
+    void* ws = g_ws.get(ws_bytes_pdr_vjp<T>(ns, nds, npen, dims, glam != nullptr));
+    if (!ws) { fail(fn, "out of memory", nullptr); return 0; }
+    return cuda_ok(fn, pd_vjp_device<T>(pd2, ns, nds, npen, dims, iters, tape, gout, gY, glam, ws, (cudaStream_t)stream), nullptr);
 }
 
 }  // namespace
@@ -590,6 +637,37 @@ int proxtv_PDR_TV_vjp_dev_f64(const int* ns, int nds, int npen, const double* di
 int proxtv_PDR_TV_vjp_dev_f32(const int* ns, int nds, int npen, const double* dims, int maxIters, const void* tape, const float* gout,
                               float* gY, double* glam, void* stream) {
     return dev_pdr_vjp<float>("proxtv_PDR_TV_vjp_dev_f32", ns, nds, npen, dims, maxIters, tape, gout, gY, glam, stream); }
+static size_t pd_tape_bytes_checked(bool pd2, const int* ns, int nds, int npen, int maxIters) {
+    if (!ns || nds < 1 || nds > PDR_TAPE_MAX_DIMS || npen < 1 || npen > (pd2 ? 2 : 64)) return 0;
+    for (int i = 0; i < nds; i++) if (ns[i] < 0) return 0;
+    return pd_tape_bytes(pd2, ns, nds, npen, maxIters);
+}
+size_t proxtv_PD_TV_tape_bytes(const int* ns, int nds, int npen, int maxIters) { return pd_tape_bytes_checked(false, ns, nds, npen, maxIters); }
+size_t proxtv_PD2_TV_tape_bytes(const int* ns, int nds, int npen, int maxIters) { return pd_tape_bytes_checked(true, ns, nds, npen, maxIters); }
+int proxtv_PD_TV_record_dev_f64(const double* y, double* lambdas, double* dims, double* x, double* info, int* ns, int nds, int npen,
+                                int maxIters, void* tape, size_t tape_bytes, void* stream) {
+    return dev_pd_record<double>("proxtv_PD_TV_record_dev_f64", false, y, lambdas, dims, x, info, ns, nds, npen, maxIters, tape, tape_bytes, stream); }
+int proxtv_PD_TV_record_dev_f32(const float* y, double* lambdas, double* dims, float* x, double* info, int* ns, int nds, int npen,
+                                int maxIters, void* tape, size_t tape_bytes, void* stream) {
+    return dev_pd_record<float>("proxtv_PD_TV_record_dev_f32", false, y, lambdas, dims, x, info, ns, nds, npen, maxIters, tape, tape_bytes, stream); }
+int proxtv_PD2_TV_record_dev_f64(const double* y, double* lambdas, double* dims, double* x, double* info, int* ns, int nds, int npen,
+                                 int maxIters, void* tape, size_t tape_bytes, void* stream) {
+    return dev_pd_record<double>("proxtv_PD2_TV_record_dev_f64", true, y, lambdas, dims, x, info, ns, nds, npen, maxIters, tape, tape_bytes, stream); }
+int proxtv_PD2_TV_record_dev_f32(const float* y, double* lambdas, double* dims, float* x, double* info, int* ns, int nds, int npen,
+                                 int maxIters, void* tape, size_t tape_bytes, void* stream) {
+    return dev_pd_record<float>("proxtv_PD2_TV_record_dev_f32", true, y, lambdas, dims, x, info, ns, nds, npen, maxIters, tape, tape_bytes, stream); }
+int proxtv_PD_TV_vjp_dev_f64(const int* ns, int nds, int npen, const double* dims, int maxIters, int iters, const void* tape,
+                             const double* gout, double* gY, double* glam, void* stream) {
+    return dev_pd_vjp<double>("proxtv_PD_TV_vjp_dev_f64", false, ns, nds, npen, dims, maxIters, iters, tape, gout, gY, glam, stream); }
+int proxtv_PD_TV_vjp_dev_f32(const int* ns, int nds, int npen, const double* dims, int maxIters, int iters, const void* tape,
+                             const float* gout, float* gY, double* glam, void* stream) {
+    return dev_pd_vjp<float>("proxtv_PD_TV_vjp_dev_f32", false, ns, nds, npen, dims, maxIters, iters, tape, gout, gY, glam, stream); }
+int proxtv_PD2_TV_vjp_dev_f64(const int* ns, int nds, int npen, const double* dims, int maxIters, int iters, const void* tape,
+                              const double* gout, double* gY, double* glam, void* stream) {
+    return dev_pd_vjp<double>("proxtv_PD2_TV_vjp_dev_f64", true, ns, nds, npen, dims, maxIters, iters, tape, gout, gY, glam, stream); }
+int proxtv_PD2_TV_vjp_dev_f32(const int* ns, int nds, int npen, const double* dims, int maxIters, int iters, const void* tape,
+                              const float* gout, float* gY, double* glam, void* stream) {
+    return dev_pd_vjp<float>("proxtv_PD2_TV_vjp_dev_f32", true, ns, nds, npen, dims, maxIters, iters, tape, gout, gY, glam, stream); }
 int proxtv_PD_TV_f32(const float* y, double* lambdas, double* dims, float* x, double* info, int* ns, int nds, int npen, int maxIters) {
     return run_pd<float>("proxtv_PD_TV_f32", 1, true, y, lambdas, nullptr, dims, x, info, ns, nds, npen, maxIters, 0); }
 

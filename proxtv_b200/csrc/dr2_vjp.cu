@@ -1,6 +1,6 @@
-// dr2_vjp.cu -- the exact backward passes of DR2_TV (DESIGN.md section 11), of the weighted DR2L1W_TV (section 12) and of the N-D
-// PDR_TV (section 13, at the end): a recorded forward that writes the segmentation tape of every prox pass, and the unrolled
-// vector-Jacobian product driven by that tape.
+// dr2_vjp.cu -- the exact backward passes of DR2_TV (DESIGN.md section 11), of the weighted DR2L1W_TV (section 12), of the N-D
+// PDR_TV (section 13) and of the proximal Dykstra PD_TV / PD2_TV (section 14, at the end): a recorded forward that writes the
+// segmentation tape of every prox pass, and the unrolled vector-Jacobian product driven by that tape.
 //
 // DR2_TV is a fixed, unconverged splitting (35 iterations and a final projection), so the gradient is the one of the function actually
 // computed: the lane engine's schedule (solver.cu: dr2_lane_body), per image, storage type T, column prox P_c (axis 0, penalty w1) and
@@ -536,51 +536,68 @@ struct PdrTapeHeader {
     int32_t elem, K, npen, nds;
     int32_t ns[PDR_TAPE_MAX_DIMS];
     uint8_t axis[64];                                                       // 0-based axis of each term
-    uint8_t pad[256 - 8 - 16 - 4 * PDR_TAPE_MAX_DIMS - 64];
+    int32_t cap;                                                            // PD_TV / PD2_TV: the capacity in iterations; PDR_TV: 0
+    uint8_t pad[256 - 8 - 16 - 4 * PDR_TAPE_MAX_DIMS - 64 - 4];
 };
 static_assert(sizeof(PdrTapeHeader) == 256, "tape header is 256 bytes");
 static constexpr uint64_t PDR_TAPE_MAGIC = 0x3150415452524450ull;          // "PDRRTAP1"
+static constexpr uint64_t PD_TAPE_MAGIC = 0x3150415456544450ull;           // "PDTVTAP1"
+static constexpr uint64_t PD2_TAPE_MAGIC = 0x3150415454324450ull;          // "PD2TTAP1"
 
 static long long pdr_elems(const int* ns, int nds) { long long n = 1; for (int i = 0; i < nds; i++) n *= ns[i]; return n; }
 
-size_t pdr_tape_bytes(const int* ns, int nds, int npen, int maxIters) {
-    const int K = maxIters <= 0 ? MAX_ITERS_DR : maxIters;
-    return 256 + (size_t)(K - 1) * (size_t)npen * 2 * ptvv::vjp_tape_set_bytes(pdr_elems(ns, nds));
+// 256 + passes x two bitsets of n-element passes, in 64-bit arithmetic; 0 when that does not fit in size_t
+static size_t nd_tape_bytes(unsigned long long passes, long long n) {
+    const unsigned long long set2 = 2ull * (unsigned long long)ptvv::vjp_tape_set_bytes(n);
+    if (set2 && passes > (SIZE_MAX - 256) / set2) return 0;
+    return 256 + (size_t)(passes * set2);
 }
 
-template <typename T> cudaError_t pdr_tape_pass(void* tape, long long n, int p, const T* y, FiberGeom g, T lam, cudaStream_t st) {
+size_t pdr_tape_bytes(const int* ns, int nds, int npen, int maxIters) {
+    const int K = maxIters <= 0 ? MAX_ITERS_DR : maxIters;
+    return nd_tape_bytes((unsigned long long)(K - 1) * (unsigned long long)npen, pdr_elems(ns, nds));
+}
+
+template <typename T> cudaError_t pdr_tape_pass(void* tape, long long n, long long p, const T* y, FiberGeom g, T lam, cudaStream_t st) {
     const size_t sb = ptvv::vjp_tape_set_bytes(n);
     uint32_t* F = (uint32_t*)((char*)tape + 256 + (size_t)p * 2 * sb);
     return ptvv::fiber_tape<T>(y, g.nf, g.len, g.inc, lam, nullptr, F, F + sb / 4, st);
 }
 
-static PdrTapeHeader pdr_header(size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters) {
+static PdrTapeHeader nd_header(uint64_t magic, size_t elem, const int* ns, int nds, int npen, const double* dims, int K, int cap) {
     PdrTapeHeader h;
     memset(&h, 0, sizeof(h));
-    h.magic = PDR_TAPE_MAGIC; h.elem = (int32_t)elem; h.K = maxIters <= 0 ? MAX_ITERS_DR : maxIters; h.npen = npen; h.nds = nds;
+    h.magic = magic; h.elem = (int32_t)elem; h.K = K; h.npen = npen; h.nds = nds; h.cap = cap;
     for (int i = 0; i < nds; i++) h.ns[i] = ns[i];
     for (int i = 0; i < npen; i++) h.axis[i] = (uint8_t)(int)(dims[i] - 1);
     return h;
 }
 
 cudaError_t pdr_tape_header(void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters, cudaStream_t st) {
-    const PdrTapeHeader h = pdr_header(elem, ns, nds, npen, dims, maxIters);
+    const PdrTapeHeader h = nd_header(PDR_TAPE_MAGIC, elem, ns, nds, npen, dims, maxIters <= 0 ? MAX_ITERS_DR : maxIters, 0);
     return cudaMemcpyAsync(tape, &h, sizeof(h), cudaMemcpyHostToDevice, st);
 }
 
-const char* pdr_tape_check(const void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters,
-                           cudaStream_t st) {
+// the header check of the three N-D tapes: magic (not_ours when it is not this solver's), dtype, shape, terms, capacity, K
+static const char* nd_tape_check(uint64_t magic, const char* not_ours, const void* tape, size_t elem, const int* ns, int nds, int npen,
+                                 const double* dims, int K, int cap, cudaStream_t st) {
     PdrTapeHeader h;
     if (cudaMemcpyAsync(&h, tape, sizeof(h), cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) {
         cudaGetLastError(); return "cannot read the tape header";
     }
-    const PdrTapeHeader w = pdr_header(elem, ns, nds, npen, dims, maxIters);
-    if (h.magic != w.magic) return "not a PDR_TV tape";
+    const PdrTapeHeader w = nd_header(magic, elem, ns, nds, npen, dims, K, cap);
+    if (h.magic != w.magic) return not_ours;
     if (h.elem != w.elem) return "tape recorded with another dtype";
     if (h.nds != w.nds || memcmp(h.ns, w.ns, sizeof(h.ns)) != 0) return "tape recorded for another shape";
     if (h.npen != w.npen || memcmp(h.axis, w.axis, sizeof(h.axis)) != 0) return "tape recorded with other penalty terms";
+    if (h.cap != w.cap) return "tape recorded with another maxIters";
     if (h.K != w.K) return "tape recorded with another iteration count";
     return nullptr;
+}
+
+const char* pdr_tape_check(const void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters,
+                           cudaStream_t st) {
+    return nd_tape_check(PDR_TAPE_MAGIC, "not a PDR_TV tape", tape, elem, ns, nds, npen, dims, maxIters <= 0 ? MAX_ITERS_DR : maxIters, 0, st);
 }
 
 template <typename T> size_t ws_bytes_pdr_vjp(const int* ns, int nds, int npen, const double* dims, bool want_glam) {
@@ -664,7 +681,7 @@ cudaError_t pdr_vjp_device(const int* ns, int nds, int npen, const double* dims,
     RTRY(step(true, npen - 1, K >= 2));
     for (int j = K - 2; j >= 0; j--) {
         for (int i = 0; i < npen; i++) {
-            const uint32_t* F = (const uint32_t*)(tb + (size_t)(j * npen + i) * 2 * sb);
+            const uint32_t* F = (const uint32_t*)(tb + ((size_t)j * npen + i) * 2 * sb);
             RTRY(ptvv::vjp_fibers_tape<T>(F, F + sb / 4, h, sc, gw, g[i].nf, g[i].len, g[i].inc, vscr, st));
             // one "image" of all edges: img_sums adds its sum to glam[2 * 0 + i]
             if (glam) RTRY(img_sums<T>(gw, g[i].nf * (long long)(g[i].len - 1), 1, scratch, nullptr, glam, i, 1.0, st));
@@ -675,10 +692,170 @@ cudaError_t pdr_vjp_device(const int* ns, int nds, int npen, const double* dims,
 #undef RTRY
 }
 
+// ================================================================ PD_TV and PD2_TV (DESIGN.md section 14)
+// Both are the solvers of solver.cu themselves; the function differentiated is K iterations, K = the count the forward ran (info[0],
+// the header's K): the stop test only picks K.  P_i is the 1D prox along axis dims[i], S_{j,i} its segment-mean Jacobian.
+// PD_TV (pd_device, k = npen terms, kk = (T)k, lam_i scaled by k), all K npen passes reach out (pass p = j npen + i):
+//     z_i = Y ;  j = 0..K-1:  p_i = P_i(z_i) ; x = ((0 + p_0 / kk) + p_1 / kk) + ... ; z_i = z_i + (x - p_i)       out = x (j = K-1)
+//   backward, in T (sums term by term, i in order):
+//     a_i = 0 ; gk = G / kk ; h = gk - a_0                                                                  (k_pdv, start)
+//     j = K-1..0:  i = 0..k-1:  a_i = a_i + S_{j,i}(h) ; h = gk - a_{i+1}     (one VJP pass, then k_pdv; after the last term:
+//                  s = (a_0 + a_1) + ... ; j > 0: gk = s / kk, h = gk - a_0 ; j = 0: gY = s)
+// PD2_TV (pd2_device, npen <= 2, penalties as given), passes 2j (z = P_0(x + p)) and 2j + 1 (x' = P_1(z + q)); npen = 1: one
+// iteration, x' = z, pass 0.  Backward with the adjoints (gx, gp, gq) of (x', p', q') = (G, 0, 0); after the first step gx == gp, so
+// one array gp holds both:
+//     gp = 0 ; gq = 0 ; h = G - 0                                                                           (k_pd2v, mode 0)
+//     j = K-1..0:  [npen = 2: gv = S_1(h) ; gq = gq + gv ; h = gq - gp                                      (mode 1)]
+//                  gu = S_0(h) ; gp = gp + gu ; j > 0: h = gp - gq ; j = 0: gY = gp                           (mode 2)
+// Penalty gradients: glam_i = 0.0 ; glam_i = glam_i + sum(gw) per pass of term i in backward order, gw the pass's edge gradients for
+// its upstream gradient h, each sum img_sums' fixed two-stage double sum.  No atomics.
+static int pd_cap(int maxIters) { return maxIters <= 0 ? MAX_ITERS_PD : maxIters; }
+static unsigned long long pd_passes(bool pd2, int npen, int K) {
+    const unsigned long long k = (unsigned long long)K;
+    return pd2 ? (npen == 1 ? (K > 0 ? 1 : 0) : 2 * k) : k * (unsigned long long)npen;
+}
+
+size_t pd_tape_bytes(bool pd2, const int* ns, int nds, int npen, int maxIters) {
+    return nd_tape_bytes(pd_passes(pd2, npen, pd_cap(maxIters)), pdr_elems(ns, nds));
+}
+
+cudaError_t pd_tape_header(bool pd2, void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters, int iters,
+                           cudaStream_t st) {
+    const PdrTapeHeader h = nd_header(pd2 ? PD2_TAPE_MAGIC : PD_TAPE_MAGIC, elem, ns, nds, npen, dims, iters, pd_cap(maxIters));
+    return cudaMemcpyAsync(tape, &h, sizeof(h), cudaMemcpyHostToDevice, st);
+}
+
+const char* pd_tape_check(bool pd2, const void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters,
+                          int iters, cudaStream_t st) {
+    return nd_tape_check(pd2 ? PD2_TAPE_MAGIC : PD_TAPE_MAGIC, pd2 ? "not a PD2_TV tape" : "not a PD_TV tape", tape, elem, ns, nds, npen,
+                         dims, iters, pd_cap(maxIters), st);
+}
+
+// start: every a_l = 0, gk = G / kk, h = gk - a_0.  Else the step after term i's VJP pass (result sc): a_i = a_i + sc, then h = gk - a_{i+1}
+// for the next term; after the last term s = (a_0 + a_1) + ... ; more: gk = s / kk, h = gk - a_0 ; else gY = s.
+template <typename T>
+__global__ void k_pdv(PdrvPtrs<T> a, int npen, int i, bool start, bool more, const T* __restrict__ G, const T* __restrict__ sc,
+                      T* __restrict__ Gk, T* __restrict__ h, T* __restrict__ gY, long long n) {
+    const T kk = (T)npen;
+    GRID_STRIDE(q, n) {
+        if (start) {
+            for (int l = 0; l < npen; l++) a.gz[l][q] = T(0);
+            const T gk = G[q] / kk;
+            Gk[q] = gk;
+            h[q] = gk - T(0);
+            continue;
+        }
+        const T v = a.gz[i][q] + sc[q];
+        a.gz[i][q] = v;
+        if (i + 1 < npen) { h[q] = Gk[q] - a.gz[i + 1][q]; continue; }
+        T s = npen == 1 ? v : a.gz[0][q];
+        for (int l = 1; l < npen; l++) s = s + (l == npen - 1 ? v : a.gz[l][q]);
+        if (more) {
+            const T gk = s / kk;
+            Gk[q] = gk;
+            h[q] = gk - (npen == 1 ? v : a.gz[0][q]);
+        } else {
+            gY[q] = s;
+        }
+    }
+}
+
+// mode 0: gp = 0, gq = 0, h = G - 0.  1 (after P_1's VJP, sc = gv): gq = gq + gv, h = gq - gp.  2 (after P_0's VJP, sc = gu): gp = gp + gu;
+// more: h = gp - gq ; else gY = gp.
+template <typename T>
+__global__ void k_pd2v(int mode, bool more, const T* __restrict__ G, const T* __restrict__ sc, T* __restrict__ gp, T* __restrict__ gq,
+                       T* __restrict__ h, T* __restrict__ gY, long long n) {
+    GRID_STRIDE(q, n) {
+        if (mode == 0) {
+            gp[q] = T(0); gq[q] = T(0);
+            h[q] = G[q] - T(0);
+        } else if (mode == 1) {
+            const T v = gq[q] + sc[q];
+            gq[q] = v;
+            h[q] = v - gp[q];
+        } else {
+            const T v = gp[q] + sc[q];
+            if (more) { gp[q] = v; h[q] = v - gq[q]; }
+            else gY[q] = v;
+        }
+    }
+}
+
+template <typename T>
+cudaError_t pd_vjp_device(bool pd2, const int* ns, int nds, int npen, const double* dims, int iters, const void* tape, const T* gout, T* gY,
+                          double* glam, void* ws, cudaStream_t st) {
+#define RTRY(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) return e__; } while (0)
+    const long long n = pdr_elems(ns, nds);
+    const int K = iters;
+    if (glam) RTRY(cudaMemsetAsync(glam, 0, (size_t)npen * sizeof(double), st));
+    if (n == 0 || K <= 0) return cudaSuccess;
+    const size_t ab = al256((size_t)n * sizeof(T)), sb = ptvv::vjp_tape_set_bytes(n);
+    FiberGeom g[64];
+    size_t vs = 0;
+    for (int i = 0; i < npen; i++) {
+        geom_of(ns, nds, dims[i], n, &g[i]);
+        const size_t b = ptvv::vjp_scratch_bytes(g[i].nf, g[i].len);
+        if (b > vs) vs = b;
+    }
+    char* w = (char*)ws;                       // the layout of ws_bytes_pdr_vjp: npen + 3 arrays (PD2_TV uses 4), gw, VJP scratch, sums
+    PdrvPtrs<T> a;
+    for (int i = 0; i < npen; i++) { a.gz[i] = (T*)w; w += ab; }
+    T* Gk = (T*)w; w += ab;
+    T* h = (T*)w; w += ab;
+    T* sc = (T*)w; w += ab;
+    T* gw = nullptr;
+    if (glam) { gw = (T*)w; w += ab; }
+    void* vscr = w; w += al256(vs);
+    double* scratch = (double*)w;
+    const char* tb = (const char*)tape + 256;
+    const unsigned ge = ew_grid(n);
+    // the VJP of pass p (term i) for the upstream h into sc, and its edge gradients into glam[i]
+    auto pass = [&](long long p, int i) -> cudaError_t {
+        const uint32_t* F = (const uint32_t*)(tb + (size_t)p * 2 * sb);
+        RTRY(ptvv::vjp_fibers_tape<T>(F, F + sb / 4, h, sc, gw, g[i].nf, g[i].len, g[i].inc, vscr, st));
+        if (glam) RTRY(img_sums<T>(gw, g[i].nf * (long long)(g[i].len - 1), 1, scratch, nullptr, glam, i, 1.0, st));
+        return cudaSuccess;
+    };
+    if (!pd2) {
+        auto step = [&](bool start, int i, bool more) -> cudaError_t {
+            KernelSpan sp(KC_ELEMENTWISE, 1, st);
+            k_pdv<T><<<ge, 256, 0, st>>>(a, npen, i, start, more, gout, sc, Gk, h, gY, n);
+            return cudaGetLastError();
+        };
+        RTRY(step(true, 0, true));
+        for (int j = K - 1; j >= 0; j--)
+            for (int i = 0; i < npen; i++) {
+                RTRY(pass((long long)j * npen + i, i));
+                RTRY(step(false, i, j > 0));
+            }
+    } else {
+        T* gp = a.gz[0];                       // npen + 3 >= 4 arrays: gp, gq (= Gk's slot when npen = 1), h, sc
+        T* gq = npen >= 2 ? a.gz[1] : Gk;
+        auto step = [&](int mode, bool more) -> cudaError_t {
+            KernelSpan sp(KC_ELEMENTWISE, 1, st);
+            k_pd2v<T><<<ge, 256, 0, st>>>(mode, more, gout, sc, gp, gq, h, gY, n);
+            return cudaGetLastError();
+        };
+        RTRY(step(0, true));
+        for (int j = K - 1; j >= 0; j--) {
+            if (npen >= 2) {
+                RTRY(pass(2LL * j + 1, 1));
+                RTRY(step(1, true));
+            }
+            RTRY(pass(npen >= 2 ? 2LL * j : 0, 0));
+            RTRY(step(2, j > 0));
+        }
+    }
+    return cudaSuccess;
+#undef RTRY
+}
+
 #define INST(T) \
-    template cudaError_t pdr_tape_pass<T>(void*, long long, int, const T*, FiberGeom, T, cudaStream_t); \
+    template cudaError_t pdr_tape_pass<T>(void*, long long, long long, const T*, FiberGeom, T, cudaStream_t); \
     template size_t ws_bytes_pdr_vjp<T>(const int*, int, int, const double*, bool); \
     template cudaError_t pdr_vjp_device<T>(const int*, int, int, const double*, int, const void*, const T*, T*, double*, void*, cudaStream_t); \
+    template cudaError_t pd_vjp_device<T>(bool, const int*, int, int, const double*, int, const void*, const T*, T*, double*, void*, \
+                                          cudaStream_t); \
     template size_t ws_bytes_dr2_record<T>(size_t, size_t, int); \
     template size_t ws_bytes_dr2_vjp<T>(size_t, size_t, int); \
     template cudaError_t dr2_record_device<T>(size_t, size_t, int, int, const T*, T, T, T*, int, void*, void*, Engine, cudaStream_t); \

@@ -96,10 +96,13 @@ template <typename T> int dr2_device(size_t M, size_t N, int batch, int row_majo
 template <typename T> int drw_device(size_t M, size_t N, const T* Y, const T* W1, const T* W2, T* out, int maxit, double* info, void* ws,
                                      Engine eng, cudaStream_t st);
 template <typename T> size_t ws_bytes_pd(long long n, int npen);
+// PD2_TV / PD_TV (proximal Dykstra, stop rule mean|x - x_old| <= STOP_PD).  tape: nullptr, or the recorded forward's buffer (header
+// written by the caller after the call, from info[0]): the segmentation tape of every pass
 template <typename T> int pd2_device(const T* y, const double* lambdas, const double* dims, T* x, double* info, const int* ns,
-                                     int nds, int npen, int maxIters, void* ws, Engine eng, cudaStream_t st);
+                                     int nds, int npen, int maxIters, void* ws, Engine eng, cudaStream_t st, void* tape = nullptr);
 template <typename T> int pd_device(const T* y, const double* lambdas_scaled, const double* dims, T* x, double* info,
-                                    const int* ns, int nds, int npen, int maxIters, void* ws, Engine eng, cudaStream_t st);
+                                    const int* ns, int nds, int npen, int maxIters, void* ws, Engine eng, cudaStream_t st,
+                                    void* tape = nullptr);
 // Engine choice under ENGINE_AUTO for data y (device pointer, n elements) and penalty lam: the lane engine keeps every open segment of
 // a fiber inside a 64-row (float64) / 128-row (float32) shared-memory window and sends fibers whose segments outgrow it through a
 // slow exact repair path, so it only pays while segments are short -- lam not larger than about the mean step |y[i+1] - y[i]| of the
@@ -147,9 +150,9 @@ template <typename T> int pdr_device(const T* y, const double* lambdas_scaled, c
 bool geom_of(const int* ns, int nds, double dim, long long n, FiberGeom* g);
 // ---- exact backward pass of PDR_TV (dr2_vjp.cu, DESIGN.md section 13) ----
 constexpr int PDR_TAPE_MAX_DIMS = 16;                                    // axes the tape header holds
-size_t pdr_tape_bytes(const int* ns, int nds, int npen, int maxIters);    // header + (K - 1) npen passes x two bitsets
+size_t pdr_tape_bytes(const int* ns, int nds, int npen, int maxIters);    // header + (K - 1) npen passes x two bitsets; 0: too large
 // the tape of pass p (output y over the fibers g, penalty lam) into a tape of n-element passes
-template <typename T> cudaError_t pdr_tape_pass(void* tape, long long n, int p, const T* y, FiberGeom g, T lam, cudaStream_t st);
+template <typename T> cudaError_t pdr_tape_pass(void* tape, long long n, long long p, const T* y, FiberGeom g, T lam, cudaStream_t st);
 // writes the 256-byte header (arguments checked by the caller; axes = dims - 1)
 cudaError_t pdr_tape_header(void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters, cudaStream_t st);
 // validates a tape's header against the arguments (one stream synchronisation): nullptr ok, else the reason
@@ -159,6 +162,19 @@ template <typename T> size_t ws_bytes_pdr_vjp(const int* ns, int nds, int npen, 
 // gY, and glam[npen] (d/d of the scaled penalties) unless nullptr, from the tape alone; arguments checked by the caller
 template <typename T> cudaError_t pdr_vjp_device(const int* ns, int nds, int npen, const double* dims, int maxIters, const void* tape,
                                                  const T* gout, T* gY, double* glam, void* ws, cudaStream_t st);
+// ---- exact backward passes of PD_TV and PD2_TV (dr2_vjp.cu, DESIGN.md section 14); pd2 selects PD2_TV ----
+// header + the capacity of maxIters (0: 35) iterations: maxIters npen passes (PD_TV), 2 maxIters (PD2_TV; 1 when npen = 1); 0 when
+// the byte count does not fit in size_t
+size_t pd_tape_bytes(bool pd2, const int* ns, int nds, int npen, int maxIters);
+// writes the 256-byte header after the solve: capacity maxIters, iters = the iterations run (info[0])
+cudaError_t pd_tape_header(bool pd2, void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters, int iters,
+                           cudaStream_t st);
+const char* pd_tape_check(bool pd2, const void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters,
+                          int iters, cudaStream_t st);
+// gY, and glam[npen] unless nullptr (PD_TV: d/d of the scaled penalties; PD2_TV: of the penalties as given), from the tape of a solve
+// that ran `iters` iterations; arguments checked by the caller; workspace ws_bytes_pdr_vjp
+template <typename T> cudaError_t pd_vjp_device(bool pd2, const int* ns, int nds, int npen, const double* dims, int iters, const void* tape,
+                                                const T* gout, T* gY, double* glam, void* ws, cudaStream_t st);
 
 }  // namespace ptv
 

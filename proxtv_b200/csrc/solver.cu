@@ -482,9 +482,11 @@ static int read_stop(const double* dres, double* stop, cudaStream_t st) {
     return e == cudaSuccess;
 }
 
+// tape != nullptr (the recorded forward, dr2_vjp.cu): after each pass the segmentation tape of its output is written -- z as pass
+// 2 iters, x as pass 2 iters + 1 (npen = 1: z as pass 0); nothing else changes.
 template <typename T>
 int pd2_device(const T* y, const double* lambdas, const double* dims, T* x, double* info, const int* ns, int nds, int npen,
-               int maxIters, void* ws, Engine eng, cudaStream_t st) {
+               int maxIters, void* ws, Engine eng, cudaStream_t st, void* tape) {
     if (npen > 2) { printf("PD2_TV: this algorithm can not work with more than 2 penalties\n");      // :95-96
                     if (info) info[INFO_RC] = RC_ERROR; return 0; }
     long long n = 1; for (int i = 0; i < nds; i++) n *= ns[i];
@@ -505,9 +507,11 @@ int pd2_device(const T* y, const double* lambdas, const double* dims, T* x, doub
         while (stop > STOP_PD && (npen > 1 || !iters) && iters < maxIters) {                           // :157
             PTV_TRY(cudaMemcpyAsync(xl, x, (size_t)n * sizeof(T), cudaMemcpyDeviceToDevice, st));
             PTV_TRY(prox_fibers<T>(x, p, IN_A_PLUS_B, z, 0, g0, (T)lambdas[0], nullptr, eng, scr, st, 3 * n));       // :171-208
+            if (tape) PTV_TRY(pdr_tape_pass<T>(tape, n, 2LL * iters, z, g0, (T)lambdas[0], st));
             PTV_TRY(ew_dual_update<T>(p, x, z, n, st));                                               // :211-213
             if (npen >= 2) {
                 PTV_TRY(prox_fibers<T>(z, q, IN_A_PLUS_B, x, 0, g1, (T)lambdas[1], nullptr, eng, scr, st, 3 * n));   // :216-258
+                if (tape) PTV_TRY(pdr_tape_pass<T>(tape, n, 2LL * iters + 1, x, g1, (T)lambdas[1], st));
                 PTV_TRY(ew_dual_update<T>(q, z, x, n, st));                                           // :261-263
             } else {
                 PTV_TRY(cudaMemcpyAsync(x, z, (size_t)n * sizeof(T), cudaMemcpyDeviceToDevice, st));  // :266-269
@@ -522,9 +526,11 @@ int pd2_device(const T* y, const double* lambdas, const double* dims, T* x, doub
     return 1;
 }
 
+// tape != nullptr (the recorded forward, dr2_vjp.cu): after each pass the segmentation tape of its output p_i is written as pass
+// iters * npen + i; nothing else changes.
 template <typename T>
 int pd_device(const T* y, const double* lam, const double* dims, T* x, double* info, const int* ns, int nds, int npen,
-              int maxIters, void* ws, Engine eng, cudaStream_t st) {
+              int maxIters, void* ws, Engine eng, cudaStream_t st, void* tape) {
     long long n = 1; for (int i = 0; i < nds; i++) n *= ns[i];
     if (maxIters <= 0) maxIters = MAX_ITERS_PD;
     if (npen > 64) { printf("PD_TV: more than 64 penalty terms are not supported\n"); if (info) info[INFO_RC] = RC_ERROR; return 0; }
@@ -548,8 +554,10 @@ int pd_device(const T* y, const double* lam, const double* dims, T* x, double* i
         PTV_TRY(cudaMemsetAsync(x, 0, (size_t)n * sizeof(T), st));                                    // :125-130
         for (int i = 0; i < npen; i++) PTV_TRY(cudaMemcpyAsync(hz[i], y, (size_t)n * sizeof(T), cudaMemcpyDeviceToDevice, st));
         while (stop > STOP_PD && iters < maxIters) {                                                  // :151
-            for (int i = 0; i < npen; i++)
+            for (int i = 0; i < npen; i++) {
                 PTV_TRY(prox_fibers<T>(hz[i], nullptr, IN_A, hp[i], 0, g[i], (T)lam[i], nullptr, eng, scr, st, 3 * n));  // :171-208
+                if (tape) PTV_TRY(pdr_tape_pass<T>(tape, n, (long long)iters * npen + i, hp[i], g[i], (T)lam[i], st));
+            }
             PTV_TRY(ew_pd_combine<T>(dp, dz, hp, hz, npen, x, n, scratch, dres, st));                         // :212-227
             if (!read_stop(dres, &stop, st)) { PTV_TRY(cudaGetLastError()); PTV_TRY(cudaErrorUnknown); }
             iters++;
@@ -598,7 +606,7 @@ int pdr_device(const T* y, const double* lam, const double* dims, T* x, double* 
         while (iters < maxIters) {                                                                    // :394
             for (int i = 0; i < npen; i++) {
                 PTV_TRY(prox_fibers<T>(hz[i], nullptr, IN_A, hp[i], 0, g[i], (T)lam[i], nullptr, eng, scr, st, 3 * n));  // :409-449
-                if (tape && iters < maxIters - 1) PTV_TRY(pdr_tape_pass<T>(tape, n, iters * npen + i, hp[i], g[i], (T)lam[i], st));
+                if (tape && iters < maxIters - 1) PTV_TRY(pdr_tape_pass<T>(tape, n, (long long)iters * npen + i, hp[i], g[i], (T)lam[i], st));
             }
             PTV_TRY(ew_pdr_combine<T>(dp, dz, hp, hz, npen, x, n, scratch, dres, st));                        // :456-475
             iters++;
@@ -619,8 +627,10 @@ int pdr_device(const T* y, const double* lam, const double* dims, T* x, double* 
     template int dr2_lane_pick<T>(size_t, size_t, int, int, const T*, const T*, const void*, T, T, Engine, void**); \
     template int drw_device<T>(size_t, size_t, const T*, const T*, const T*, T*, int, double*, void*, Engine, cudaStream_t); \
     template size_t ws_bytes_pd<T>(long long, int); \
-    template int pd2_device<T>(const T*, const double*, const double*, T*, double*, const int*, int, int, int, void*, Engine, cudaStream_t); \
-    template int pd_device<T>(const T*, const double*, const double*, T*, double*, const int*, int, int, int, void*, Engine, cudaStream_t); \
+    template int pd2_device<T>(const T*, const double*, const double*, T*, double*, const int*, int, int, int, void*, Engine, cudaStream_t, \
+                               void*); \
+    template int pd_device<T>(const T*, const double*, const double*, T*, double*, const int*, int, int, int, void*, Engine, cudaStream_t, \
+                              void*); \
     template int pdr_device<T>(const T*, const double*, const double*, T*, double*, const int*, int, int, int, void*, Engine, cudaStream_t, \
                                void*);
 INST(double)
