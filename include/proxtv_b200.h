@@ -149,7 +149,8 @@ int proxtv_prox_fibers_vjp_tape_dev_f64(const unsigned *F, const unsigned *U, co
                                         int len, long long inc, void *stream);
 int proxtv_prox_fibers_vjp_tape_dev_f32(const unsigned *F, const unsigned *U, const float *g, float *gx, float *gw, long long nf,
                                         int len, long long inc, void *stream);
-/* host-pointer form of the above (pageable or pinned memory); synchronous. */
+/* host-pointer form of the above (pageable or pinned memory); synchronous.  in and out hold nf * len elements, so nf must be a
+ * multiple of inc; other geometries are refused (returns 0) without writing anything. */
 int proxtv_prox_fibers_f64(const double *in, double *out, long long nf, int len, long long inc, double lam,
                            const double *lamv);
 int proxtv_prox_fibers_f32(const float *in, float *out, long long nf, int len, long long inc, float lam,
@@ -321,6 +322,10 @@ unsigned long long proxtv_lane_stats(int reset);
  * mean step |y[i+1] - y[i]| of (a sample of) the input, measured with one small kernel and one stream synchronisation per call --
  * and the chunked engine otherwise.  Last decision on the current device: 1 lane, 0 chunked, -1 none taken. */
 int proxtv_lane_guard_last(void);
+/* tests: contiguous unweighted fibers longer than shared memory go through overlapping tiles whose stitching is verified on the device,
+ * and the whole call falls back to the sequential kernel when a check fails.  What the latest proxtv_prox_fibers_* call (or 1D entry
+ * point of Part 1) on the current device did: 1 used the tiles, 0 tried them and fell back, -1 did not try them. */
+int proxtv_long_fiber_last(void);
 /* tools: device buffer of 4 x cap_tasks uint64 that receives, per warp task of the next launches, {start ns, scan end ns, end ns, SM id}
  * (globaltimer); NULL switches the log off. */
 void proxtv_lane_tasklog(unsigned long long *dev, long long cap_tasks);

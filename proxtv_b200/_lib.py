@@ -98,6 +98,7 @@ SIGNATURES = {
     "proxtv_lane_tuning": (None, [C.c_int, C.c_int, C.c_int]),
     "proxtv_lane_stats": (C.c_ulonglong, [C.c_int]),
     "proxtv_lane_guard_last": (C.c_int, []),
+    "proxtv_long_fiber_last": (C.c_int, []),
     "proxtv_lane_tasklog": (None, [_vp, C.c_longlong]),
     "proxtv_profile_enable": (None, [C.c_int]),
     "proxtv_profile_reset": (None, []),

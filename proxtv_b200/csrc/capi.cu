@@ -86,6 +86,9 @@ inline size_t al(size_t b) { return (b + 255) & ~(size_t)255; }
 template <typename T>
 int host_prox_fibers(const char* fn, const T* in, T* out, long long nf, int len, long long inc, T lam, const T* lamv) {
     if (nf <= 0 || len <= 0) return 1;
+    // the host arrays are staged as nf * len elements: with inc > 1 that is the whole slicing only when nf is a multiple of inc (the
+    // last fibers of a partial slab would lie beyond it)
+    if (inc < 1 || (inc > 1 && nf % inc != 0)) return fail(fn, "invalid fiber geometry (need inc >= 1 and nf a multiple of inc)", nullptr) ? 1 : 0;
     if (!have_device(fn, nullptr)) return 0;
     WsGuard guard(0);
     const size_t n = (size_t)nf * len, nw = lamv ? (size_t)nf * (len - 1) : 0;
@@ -99,6 +102,7 @@ int host_prox_fibers(const char* fn, const T* in, T* out, long long nf, int len,
     if (!cuda_ok(fn, cudaMemcpyAsync(din, in, n * sizeof(T), cudaMemcpyHostToDevice, st), nullptr)) return 0;
     if (nw && !cuda_ok(fn, cudaMemcpyAsync(dw, lamv, nw * sizeof(T), cudaMemcpyHostToDevice, st), nullptr)) return 0;
     FiberGeom g{nf, len, inc};
+    long_fiber_note(-1);
     const Engine eng = (!lamv && nf >= 1024 && len >= 64) ? lane_guard<T>((Engine)g_engine, din, (long long)n, (double)lam, st) : (Engine)g_engine;
     if (!cuda_ok(fn, prox_fibers<T>(din, nullptr, IN_A, dout, 0, g, lam, lamv ? dw : nullptr, eng, scr, st,
                                      (inc == 1 && scr) ? lf_scratch_elems(nf, len) : (inc != 1 ? strided_scratch_elems(nf, len) : 0)), nullptr)) return 0;
@@ -441,6 +445,7 @@ int proxtv_lane_prox_dev_f32(int op, const float* A, const float* B, const float
 void proxtv_lane_tuning(int clen, int halo, int variant) { ptvl::lane_set_tuning(clen, halo, variant); }
 void proxtv_lane_tasklog(unsigned long long* dev, long long cap_tasks) { ptvl::lane_set_tasklog(dev, cap_tasks); }
 int proxtv_lane_guard_last(void) { return lane_guard_last(); }
+int proxtv_long_fiber_last(void) { return long_fiber_last(); }
 unsigned long long proxtv_lane_stats(int reset) { return ptvl::lane_read_stats(reset); }
 
 // ---- Part 1: drop-in symbols ----
@@ -525,6 +530,7 @@ int PDR_TV(double* y, double* lambdas, double* norms, double* dims, double* x, d
 int proxtv_prox_fibers_dev_f64(const double* in, double* out, long long nf, int len, long long inc, double lam, const double* lamv, void* stream) {
     if (!have_device("proxtv_prox_fibers_dev_f64", nullptr)) return 0;
     WsGuard guard((cudaStream_t)stream);
+    long_fiber_note(-1);
     const Engine eng = (!lamv && nf >= 1024 && len >= 64) ? lane_guard<double>((Engine)g_engine, in, nf * (long long)len, lam, (cudaStream_t)stream) : (Engine)g_engine;
     return cuda_ok("proxtv_prox_fibers_dev_f64", prox_fibers<double>(in, nullptr, IN_A, out, 0, FiberGeom{nf, len, inc}, lam, lamv, eng, dev_scratch<double>(nf, len, inc), (cudaStream_t)stream,
                                                                  (inc == 1 && len > 16384) ? lf_scratch_elems(nf, len) : (inc != 1 ? strided_scratch_elems(nf, len) : 0)), nullptr);
@@ -532,6 +538,7 @@ int proxtv_prox_fibers_dev_f64(const double* in, double* out, long long nf, int 
 int proxtv_prox_fibers_dev_f32(const float* in, float* out, long long nf, int len, long long inc, float lam, const float* lamv, void* stream) {
     if (!have_device("proxtv_prox_fibers_dev_f32", nullptr)) return 0;
     WsGuard guard((cudaStream_t)stream);
+    long_fiber_note(-1);
     const Engine eng = (!lamv && nf >= 1024 && len >= 64) ? lane_guard<float>((Engine)g_engine, in, nf * (long long)len, (double)lam, (cudaStream_t)stream) : (Engine)g_engine;
     return cuda_ok("proxtv_prox_fibers_dev_f32", prox_fibers<float>(in, nullptr, IN_A, out, 0, FiberGeom{nf, len, inc}, lam, lamv, eng, dev_scratch<float>(nf, len, inc), (cudaStream_t)stream,
                                                                  (inc == 1 && len > 16384) ? lf_scratch_elems(nf, len) : (inc != 1 ? strided_scratch_elems(nf, len) : 0)), nullptr);

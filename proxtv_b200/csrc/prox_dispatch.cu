@@ -34,6 +34,12 @@ cudaError_t scatter_fibers_sparse(const T* in, const uint32_t* Mk, const T* Cv, 
 // elements of scratch the strided route needs for its sparse form: two staging arrays + per-chunk masks and entering values
 long long strided_scratch_elems(long long nf, long long len) { return 2 * nf * len + 2 * nf * ((len + 31) / 32) + 64; }
 
+// outcome of the long-fiber tiles per device, for tests (long_fiber_last in ptv_internal.h); stored + 2, so a slot never written reads -1
+static int g_lf_last_d[64] = {};
+static int lf_slot() { int d = 0; if (cudaGetDevice(&d) != cudaSuccess) { cudaGetLastError(); d = 0; } return (d < 0 || d >= 64) ? 63 : d; }
+void long_fiber_note(int v) { g_lf_last_d[lf_slot()] = v + 2; }
+int long_fiber_last() { const int v = g_lf_last_d[lf_slot()]; return v ? v - 2 : -1; }
+
 template <typename T>
 cudaError_t prox_fibers_ex(const T* A, const T* B, const T* C, InOp op, T* X, int out_op, FiberGeom g, T lam, const T* lamv,
                            Engine eng, T* scratch, cudaStream_t st, long long scratch_elems) {
@@ -64,6 +70,7 @@ cudaError_t prox_fibers_ex(const T* A, const T* B, const T* C, InOp op, T* X, in
             // (plain results only: the agreement test of the stitching compares prox values, which the fused output forms would hide)
             if (!lamv && out_op == OUT_X && scratch && scratch_elems >= lf_scratch_elems(g.nf, g.len)) {
                 e = prox_long_fibers<T>(A, B, op, X, out_op, g, lam, scratch, lf_scratch_elems(g.nf, g.len), st);
+                if (e == cudaSuccess || e == cudaErrorNotReady) long_fiber_note(e == cudaSuccess ? 1 : 0);
                 if (e == cudaSuccess) return e;
                 if (e != cudaErrorInvalidConfiguration && e != cudaErrorNotReady) return e;
                 cudaGetLastError();

@@ -49,6 +49,10 @@ cudaError_t prox_fibers_ex(const T* A, const T* B, const T* C, InOp op, T* X, in
 
 long long strided_scratch_elems(long long nf, long long len);   // scratch elements that enable the sparse strided route (else 2n: dense route)
 long long lf_scratch_elems(long long nf, long long len);     // scratch elements prox_fibers needs for contiguous fibers longer than shared memory
+// tests: what the long-fiber tiles (long_fiber.cu) did in the latest batched 1D prox entry call on this device -- 1 used, 0 tried and
+// fell back to the sequential kernel, -1 not tried.  The entry points note -1 before they dispatch; prox_fibers_ex notes 1 or 0.
+void long_fiber_note(int v);
+int long_fiber_last();
 
 // ---- launch accounting / event timing (profile.cu) ----
 enum KernelClass { KC_PROX_CONTIG = 0, KC_PROX_STRIDED = 1, KC_ELEMENTWISE = 2, KC_COUNT = 3 };
