@@ -13,6 +13,8 @@ traffic, no host transposes -- a C-ordered tensor is handled by swapping the ker
 tensors (exact backward kernels).
 """
 import ctypes as C
+import functools
+import types
 
 import numpy as np
 
@@ -60,6 +62,42 @@ def _is_torch(x):
 def _check(ok, what):
     if not ok:
         raise ProxTVError("%s failed: %s" % (what, _lib.last_error()))
+
+
+# ---- torch CUDA tensors: device calls and autograd ----
+def _dev_call(entry, ref, *args, rc=True, info=None):
+    """Call proxtv_<entry>_f32 / _f64 (by ref's dtype) on ref's device, with ref's current CUDA stream appended to args; torch
+    tensors in args go as device pointers, numpy arrays as host pointers, None as NULL.  Raises ProxTVError naming the entry point
+    when the call fails: on a zero return (unless not rc) or, given the info array the call fills, on info[2] == 3."""
+    import torch
+    name = "proxtv_%s_%s" % (entry, "f32" if ref.dtype == torch.float32 else "f64")
+    fn = getattr(require_device(), name)
+    args = [C.c_void_p(a.data_ptr()) if isinstance(a, torch.Tensor) else _ptr(a) if isinstance(a, np.ndarray) else a for a in args]
+    with torch.cuda.device(ref.device):
+        ok = fn(*args, C.c_void_p(torch.cuda.current_stream(ref.device).cuda_stream))
+    _check((ok or not rc) and (info is None or info[2] != 3), name)
+
+
+def _needs_grad(*objs):
+    """Grad mode is on and one of objs is a torch tensor that requires grad: the solve must be recorded for a backward."""
+    import torch
+    return torch.is_grad_enabled() and any(_is_torch(t) and t.requires_grad for t in objs)
+
+
+def _w_float(w):
+    """(the penalty w as a float, w when it is a tensor else None); the solve takes the float, the tensor only receives the gradient."""
+    w_t = w if _is_torch(w) else None
+    return (float(w_t.detach()) if w_t is not None else float(w)), w_t
+
+
+def _penalty_grad(g, like):
+    """The gradient of a penalty tensor, like = its (dtype, device, shape), from g, the gradients of the penalties the solve used:
+    summed in float64 for a 0-dim tensor (one penalty for all of them), then cast to the tensor's dtype and device."""
+    import torch
+    dtype, device, shape = like
+    if len(shape) == 0:
+        g = g.sum(dtype=torch.float64)
+    return g.to(dtype=dtype, device=device).reshape(shape)
 
 
 # ---- result arrays in pooled page-locked memory ----
@@ -170,68 +208,12 @@ def tv1w_1d(x, w, method="tautstring", sigma=0.05):
     return y
 
 
-def _prox_rows_torch(xt, w, wt):
-    """The device prox of every row of the contiguous float32/float64 CUDA tensor xt (B, L); penalty w, or weights wt (B, L-1)."""
+def _prox_rows(x, w, wt):
+    """The device prox of every row of the contiguous float32/float64 CUDA tensor x (B, L); penalty w, or weights wt (B, L-1)."""
     import torch
-    out = torch.empty_like(xt)
-    B, L = xt.shape
-    lib = require_device()
-    st = C.c_void_p(torch.cuda.current_stream(xt.device).cuda_stream)
-    fn = lib.proxtv_prox_fibers_dev_f32 if xt.dtype == torch.float32 else lib.proxtv_prox_fibers_dev_f64
-    with torch.cuda.device(xt.device):
-        _check(fn(C.c_void_p(xt.data_ptr()), C.c_void_p(out.data_ptr()), B, L, 1, float(w),
-                  C.c_void_p(wt.data_ptr()) if wt is not None else None, st), "batched 1D prox")
+    out = torch.empty_like(x)
+    _dev_call("prox_fibers_dev", x, x, out, x.shape[0], x.shape[1], 1, w, wt)
     return out
-
-
-_PROX_ROWS_FN = None
-
-
-def _prox_rows_fn():
-    """torch.autograd.Function around _prox_rows_torch (made on first use, so that numpy users never import torch).
-
-    forward(x, w, w_t, wt): x (B, L) contiguous, w the penalty as a float, w_t the 0-dim tensor it came from (or None; only receives
-    the gradient), wt (B, L-1) weights or None.  backward: proxtv_prox_fibers_vjp_dev_* on the current stream -- gx = segment means of
-    the upstream gradient, gw per edge; the gradient of w_t is gw summed in float64."""
-    global _PROX_ROWS_FN
-    if _PROX_ROWS_FN is not None:
-        return _PROX_ROWS_FN
-    import torch
-    from torch.autograd.function import once_differentiable
-
-    class ProxRows(torch.autograd.Function):
-        @staticmethod
-        def forward(ctx, x, w, w_t, wt):
-            y = _prox_rows_torch(x, w, wt)
-            ctx.save_for_backward(y, wt)
-            ctx.w = w
-            ctx.w_t_meta = (w_t.dtype, w_t.device) if w_t is not None else None
-            return y
-
-        @staticmethod
-        @once_differentiable
-        def backward(ctx, gy):
-            y, wt = ctx.saved_tensors
-            need_x, _, need_wt_scalar, need_wt = ctx.needs_input_grad
-            B, L = y.shape
-            g = gy.to(dtype=y.dtype).contiguous()
-            gx = torch.empty_like(y)
-            gw = torch.empty((B, max(L - 1, 0)), dtype=y.dtype, device=y.device) if (need_wt_scalar or need_wt) else None
-            lib = require_device()
-            st = C.c_void_p(torch.cuda.current_stream(y.device).cuda_stream)
-            fn = lib.proxtv_prox_fibers_vjp_dev_f32 if y.dtype == torch.float32 else lib.proxtv_prox_fibers_vjp_dev_f64
-            with torch.cuda.device(y.device):
-                _check(fn(C.c_void_p(y.data_ptr()), C.c_void_p(g.data_ptr()), C.c_void_p(gx.data_ptr()),
-                          C.c_void_p(gw.data_ptr()) if gw is not None else None, B, L, 1, ctx.w,
-                          C.c_void_p(wt.data_ptr()) if wt is not None else None, st), "batched 1D prox backward")
-            g_scalar = None
-            if need_wt_scalar:
-                w_t = ctx.w_t_meta
-                g_scalar = gw.sum(dtype=torch.float64).to(dtype=w_t[0], device=w_t[1]).reshape(())
-            return (gx if need_x else None), None, g_scalar, (gw if need_wt else None)
-
-    _PROX_ROWS_FN = ProxRows
-    return ProxRows
 
 
 def _batched_1d(x, w, weights):
@@ -248,12 +230,10 @@ def _batched_1d(x, w, weights):
         if weights is not None:
             wt = weights.to(dtype=xt.dtype, device=xt.device).contiguous()
             assert tuple(wt.shape) == (B, L - 1)
-        w_t = w if _is_torch(w) else None
-        wf = float(w_t.detach()) if w_t is not None else float(w)
-        if torch.is_grad_enabled() and (xt.requires_grad or (wt is not None and wt.requires_grad)
-                                        or (w_t is not None and w_t.requires_grad)):
-            return _prox_rows_fn().apply(xt, wf, w_t, wt)
-        return _prox_rows_torch(xt, wf, wt)
+        wf, w_t = _w_float(w)
+        if _needs_grad(xt, wt, w_t):
+            return _autograd().ProxRows.apply(xt, wf, w_t, wt)
+        return _prox_rows(xt, wf, wt)
     x = np.asarray(x)
     assert x.ndim == 2
     f32 = x.dtype == np.float32
@@ -323,9 +303,9 @@ def tv1_2d(x, w, n_threads=1, max_iters=0, method="dr"):
         if method == "pd":
             assert x.dim() == 2
             assert not _is_torch(w) or w.dim() == 0, "w must be a number or a 0-dim tensor"
-            wf = float(w.detach()) if _is_torch(w) else float(w)
-            return _nd_torch_entry("PD2_TV", x, [wf, wf], w if _is_torch(w) else None, [1, 2], max_iters)
-        return _dr2_torch_entry(x, w, max_iters, batched=False)
+            wf, w_t = _w_float(w)
+            return _nd_torch("PD2_TV", x, [wf, wf], w_t, [1, 2], max_iters)
+        return _dr2_torch(x, w, max_iters, batched=False)
     x = np.asfortranarray(x, dtype="float64")
     assert x.ndim == 2
     w = force_float_scalar(w)
@@ -360,7 +340,7 @@ def tv1w_2d(x, w_col, w_row, max_iters=0, n_threads=1):
     either way; double backward is not supported.
     """
     if _is_torch(x):
-        return _drw_torch_entry(x, w_col, w_row, max_iters)
+        return _drw_torch(x, w_col, w_row, max_iters)
     assert np.all(np.asarray(w_col) >= 0)
     assert np.all(np.asarray(w_row) >= 0)
     M, N = np.shape(x)
@@ -378,96 +358,33 @@ def tv1w_2d(x, w_col, w_row, max_iters=0, n_threads=1):
 
 
 def _drw_torch(x, w_col, w_row, max_iters):
+    """The torch path of tv1w_2d; recorded by the Function when grad mode is on and x, w_col or w_row requires grad.  The solver works
+    on column-major arrays, the row-major storage of the transposes: the transposes and casts to them are ordinary autograd ops."""
     import torch
     assert x.is_cuda and x.dtype in (torch.float64, torch.float32) and x.dim() == 2
     M, N = int(x.shape[0]), int(x.shape[1])
     assert tuple(w_col.shape) == (M - 1, N) and tuple(w_row.shape) == (M, N - 1)
-    # the solver works on column-major arrays == the row-major storage of the transposes
     xt = x.t().contiguous()
     w1 = w_col.to(device=x.device, dtype=x.dtype).t().contiguous()
     w2 = w_row.to(device=x.device, dtype=x.dtype).t().contiguous()
-    out = torch.empty_like(xt)
+    if _needs_grad(x, w_col, w_row):
+        return _autograd().DRW.apply(xt, w1, w2, int(max_iters)).t()
+    return _drw_solve(xt, w1, w2, int(max_iters)).t()
+
+
+def _drw_solve(Y, W1, W2, max_iters, tape=None):
+    """DR2L1W_TV on the solver's buffers Y (N, M), W1 (N, M-1), W2 (N-1, M): proxtv_DR2L1W_TV_dev_*, or given a tape (a uint8 CUDA
+    tensor, proxtv_DR2L1W_TV_tape_bytes() long) proxtv_DR2L1W_TV_record_dev_*, the same solve recording every prox pass's segmentation."""
+    import torch
+    N, M = Y.shape
+    out = torch.empty_like(Y)
     info = np.zeros(_N_INFO)
-    lib = require_device()
-    st = C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)
-    fn = lib.proxtv_DR2L1W_TV_dev_f32 if x.dtype == torch.float32 else lib.proxtv_DR2L1W_TV_dev_f64
-    with torch.cuda.device(x.device):
-        fn(M, N, C.c_void_p(xt.data_ptr()), C.c_void_p(w1.data_ptr()), C.c_void_p(w2.data_ptr()), C.c_void_p(out.data_ptr()),
-           int(max_iters), _ptr(info), st)
-    _check(info[2] != 3, "DR2L1W_TV (device)")
-    return out.t()
-
-
-_DRW_FN = None
-
-
-def _drw_fn():
-    """torch.autograd.Function around DR2L1W_TV on the device (made on first use, so that numpy users never import torch).
-
-    forward(Y, W1, W2, max_iters): Y (N, M), W1 (N, M-1), W2 (N-1, M) contiguous, x's dtype and device -- the column-major buffers
-    of the solver.  proxtv_DR2L1W_TV_record_dev_* -- the solve of _drw_torch, keeping the segmentation tape of every prox pass (a
-    uint8 CUDA tensor, proxtv_DR2L1W_TV_tape_bytes() long) on ctx.  backward: proxtv_DR2L1W_TV_vjp_dev_* on the current stream, with
-    NULL for a weight map whose input does not need its gradient."""
-    global _DRW_FN
-    if _DRW_FN is not None:
-        return _DRW_FN
-    import torch
-    from torch.autograd.function import once_differentiable
-
-    class DRW(torch.autograd.Function):
-        @staticmethod
-        def forward(ctx, Y, W1, W2, max_iters):
-            N, M = int(Y.shape[0]), int(Y.shape[1])
-            lib = require_device()
-            out = torch.empty_like(Y)
-            tape = torch.empty(int(lib.proxtv_DR2L1W_TV_tape_bytes(M, N, int(max_iters))), dtype=torch.uint8, device=Y.device)
-            info = np.zeros(_N_INFO)
-            st = C.c_void_p(torch.cuda.current_stream(Y.device).cuda_stream)
-            fn = lib.proxtv_DR2L1W_TV_record_dev_f32 if Y.dtype == torch.float32 else lib.proxtv_DR2L1W_TV_record_dev_f64
-            with torch.cuda.device(Y.device):
-                ok = fn(M, N, C.c_void_p(Y.data_ptr()), C.c_void_p(W1.data_ptr()), C.c_void_p(W2.data_ptr()), C.c_void_p(out.data_ptr()),
-                        int(max_iters), C.c_void_p(tape.data_ptr()), tape.numel(), _ptr(info), st)
-            _check(ok, "DR2L1W_TV (recorded, device)")
-            ctx.save_for_backward(tape)
-            ctx.geom = (M, N, int(max_iters))
-            return out
-
-        @staticmethod
-        @once_differentiable
-        def backward(ctx, gout):
-            (tape,) = ctx.saved_tensors
-            M, N, max_iters = ctx.geom
-            need_y, need_w1, need_w2, _ = ctx.needs_input_grad
-            dev, dt = tape.device, gout.dtype
-            g = gout.contiguous()
-            gY = torch.empty((N, M), dtype=dt, device=dev)
-            gW1 = torch.empty((N, M - 1), dtype=dt, device=dev) if need_w1 else None
-            gW2 = torch.empty((N - 1, M), dtype=dt, device=dev) if need_w2 else None
-            lib = require_device()
-            st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            fn = lib.proxtv_DR2L1W_TV_vjp_dev_f32 if dt == torch.float32 else lib.proxtv_DR2L1W_TV_vjp_dev_f64
-            p = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None          # noqa: E731
-            with torch.cuda.device(dev):
-                _check(fn(M, N, max_iters, p(tape), p(g), p(gY), p(gW1), p(gW2), st), "DR2L1W_TV backward (device)")
-            return (gY if need_y else None), gW1, gW2, None
-
-    _DRW_FN = DRW
-    return DRW
-
-
-def _drw_torch_entry(x, w_col, w_row, max_iters):
-    """The torch path of tv1w_2d: differentiable when grad mode is on and x, w_col or w_row requires grad; otherwise exactly
-    _drw_torch.  The transposes and casts to the solver's column-major buffers are ordinary autograd ops outside the Function."""
-    import torch
-    if not (torch.is_grad_enabled() and any(_is_torch(t) and t.requires_grad for t in (x, w_col, w_row))):
-        return _drw_torch(x, w_col, w_row, max_iters)
-    assert x.is_cuda and x.dtype in (torch.float64, torch.float32) and x.dim() == 2
-    M, N = int(x.shape[0]), int(x.shape[1])
-    assert tuple(w_col.shape) == (M - 1, N) and tuple(w_row.shape) == (M, N - 1)
-    xt = x.t().contiguous()
-    w1 = w_col.to(device=x.device, dtype=x.dtype).t().contiguous()
-    w2 = w_row.to(device=x.device, dtype=x.dtype).t().contiguous()
-    return _drw_fn().apply(xt, w1, w2, int(max_iters)).t()
+    args = (M, N, Y, W1, W2, out, max_iters)
+    if tape is None:       # returns 0 on success, like the reference's DR2L1W_TV: only info[2] == 3 signals a failure
+        _dev_call("DR2L1W_TV_dev", Y, *args, info, rc=False, info=info)
+    else:
+        _dev_call("DR2L1W_TV_record_dev", Y, *args, tape, tape.numel(), info)
+    return out
 
 
 def _dr2_layout(x, batched):
@@ -489,91 +406,30 @@ def _dr2_layout(x, batched):
 
 
 def _dr2_torch(x, w, max_iters, batched):
-    import torch
+    """The torch path of tv1_2d / tv1_2d_batched; recorded by the Function when grad mode is on and x, or w given as a 0-dim tensor,
+    requires grad."""
+    wf, w_t = _w_float(w)
     M, N, batch, row_major, xin = _dr2_layout(x, batched)
+    geom = (M, N, batch, row_major, int(max_iters))
+    if _needs_grad(x, w_t):
+        return _autograd().DR2.apply(xin, wf, w_t, geom)
+    return _dr2_solve(xin, wf, geom)
+
+
+def _dr2_solve(xin, w, geom, tape=None):
+    """DR2_TV on xin, geom = (M, N, batch, row_major, max_iters) of _dr2_layout: proxtv_DR2_TV_dev_*, or given a tape (a uint8 CUDA
+    tensor, proxtv_DR2_TV_tape_bytes() long) proxtv_DR2_TV_record_dev_*, the lane engine's schedule in plain passes recording every
+    prox pass's segmentation.  The result has xin's layout."""
+    import torch
     out = torch.empty_strided(xin.shape, xin.stride(), dtype=xin.dtype, device=xin.device)
     info = np.zeros(_N_INFO)
-    lib = require_device()
-    st = C.c_void_p(torch.cuda.current_stream(xin.device).cuda_stream)
-    fn = lib.proxtv_DR2_TV_dev_f32 if xin.dtype == torch.float32 else lib.proxtv_DR2_TV_dev_f64
-    with torch.cuda.device(xin.device):
-        fn(M, N, batch, row_major, C.c_void_p(xin.data_ptr()), w, w, C.c_void_p(out.data_ptr()), int(max_iters),
-           _ptr(info), st)
-    _check(info[2] != 3, "DR2_TV (device)")
+    M, N, batch, row_major, max_iters = geom
+    args = (M, N, batch, row_major, xin, w, w, out, max_iters)
+    if tape is None:       # returns 0 on success, like the reference's DR2_TV: only info[2] == 3 signals a failure
+        _dev_call("DR2_TV_dev", xin, *args, info, rc=False, info=info)
+    else:
+        _dev_call("DR2_TV_record_dev", xin, *args, tape, tape.numel(), info)
     return out
-
-
-_DR2_FN = None
-
-
-def _dr2_fn():
-    """torch.autograd.Function around DR2_TV on the device (made on first use, so that numpy users never import torch).
-
-    forward(x, w, w_t, max_iters, batched): proxtv_DR2_TV_record_dev_* -- the solve of _dr2_torch with the lane engine's schedule in
-    plain passes, keeping the segmentation tape of every prox pass (a uint8 CUDA tensor, proxtv_DR2_TV_tape_bytes() long) on ctx.
-    backward: proxtv_DR2_TV_vjp_dev_* on the current stream -- the exact vector-Jacobian product of the unrolled iteration; the
-    gradient of w_t is glam (per image and axis) summed in float64."""
-    global _DR2_FN
-    if _DR2_FN is not None:
-        return _DR2_FN
-    import torch
-    from torch.autograd.function import once_differentiable
-
-    class DR2(torch.autograd.Function):
-        @staticmethod
-        def forward(ctx, x, w, w_t, max_iters, batched):
-            M, N, batch, row_major, xin = _dr2_layout(x, batched)
-            lib = require_device()
-            out = torch.empty_strided(xin.shape, xin.stride(), dtype=xin.dtype, device=xin.device)
-            tape = torch.empty(int(lib.proxtv_DR2_TV_tape_bytes(M, N, batch, int(max_iters))), dtype=torch.uint8, device=xin.device)
-            info = np.zeros(_N_INFO)
-            st = C.c_void_p(torch.cuda.current_stream(xin.device).cuda_stream)
-            fn = lib.proxtv_DR2_TV_record_dev_f32 if xin.dtype == torch.float32 else lib.proxtv_DR2_TV_record_dev_f64
-            with torch.cuda.device(xin.device):
-                ok = fn(M, N, batch, row_major, C.c_void_p(xin.data_ptr()), w, w, C.c_void_p(out.data_ptr()), int(max_iters),
-                        C.c_void_p(tape.data_ptr()), tape.numel(), _ptr(info), st)
-            _check(ok, "DR2_TV (recorded, device)")
-            ctx.save_for_backward(tape)
-            ctx.geom = (M, N, batch, row_major, int(max_iters), tuple(out.shape), out.stride(), out.dtype)
-            ctx.w_t_meta = (w_t.dtype, w_t.device) if w_t is not None else None
-            return out
-
-        @staticmethod
-        @once_differentiable
-        def backward(ctx, gout):
-            (tape,) = ctx.saved_tensors
-            M, N, batch, row_major, max_iters, shape, stride, dt = ctx.geom
-            need_x, _, need_w_t, _, _ = ctx.needs_input_grad
-            dev = tape.device
-            g = torch.empty_strided(shape, stride, dtype=dt, device=dev)      # the upstream gradient in the output's layout
-            g.copy_(gout)
-            gY = torch.empty_strided(shape, stride, dtype=dt, device=dev)
-            glam = torch.empty(2 * batch, dtype=torch.float64, device=dev) if need_w_t else None
-            lib = require_device()
-            st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            fn = lib.proxtv_DR2_TV_vjp_dev_f32 if dt == torch.float32 else lib.proxtv_DR2_TV_vjp_dev_f64
-            with torch.cuda.device(dev):
-                _check(fn(M, N, batch, row_major, max_iters, C.c_void_p(tape.data_ptr()), C.c_void_p(g.data_ptr()),
-                          C.c_void_p(gY.data_ptr()), C.c_void_p(glam.data_ptr()) if glam is not None else None, st),
-                       "DR2_TV backward (device)")
-            g_w = None
-            if need_w_t:
-                g_w = glam.sum(dtype=torch.float64).to(dtype=ctx.w_t_meta[0], device=ctx.w_t_meta[1]).reshape(())
-            return (gY if need_x else None), None, g_w, None, None
-
-    _DR2_FN = DR2
-    return DR2
-
-
-def _dr2_torch_entry(x, w, max_iters, batched):
-    """The torch path of tv1_2d / tv1_2d_batched: differentiable when grad mode is on and x, or w given as a 0-dim tensor, requires
-    grad; otherwise exactly _dr2_torch."""
-    import torch
-    w_t = w if _is_torch(w) else None
-    wf = float(w_t.detach()) if w_t is not None else float(w)
-    if torch.is_grad_enabled() and (x.requires_grad or (w_t is not None and w_t.requires_grad)):
-        return _dr2_fn().apply(x, wf, w_t, max_iters, batched)
-    return _dr2_torch(x, wf, max_iters, batched)
 
 
 def tv1_2d_batched(x, w, max_iters=0):
@@ -584,7 +440,7 @@ def tv1_2d_batched(x, w, max_iters=0):
     """
     assert w >= 0
     if _is_torch(x):
-        return _dr2_torch_entry(x, w, max_iters, batched=True)
+        return _dr2_torch(x, w, max_iters, batched=True)
     x = np.asarray(x)
     assert x.ndim == 3
     f32 = x.dtype == np.float32
@@ -637,7 +493,7 @@ def tvgen(x, ws, ds, ps, n_threads=1, max_iters=0):
         if np.any(force_float_matrix(ps) != 1):
             raise NotImplementedError("proxtv_b200 implements TV-L1 (p = 1) penalty terms only")
         lam, ws_t = _ws_floats(ws)
-        return _nd_torch_entry("PD2_TV" if len(lam) == 2 else "PD_TV", x, lam, ws_t, ds, max_iters)
+        return _nd_torch("PD2_TV" if len(lam) == 2 else "PD_TV", x, lam, ws_t, ds, max_iters)
     info = np.zeros(_N_INFO)
     f32 = isinstance(x, np.ndarray) and x.dtype == np.float32 and len(ws) != 2
     x = np.asfortranarray(x, dtype="float32" if f32 else "float64")
@@ -694,10 +550,6 @@ def _pdr_c_order(shape, ds):
     return [int(n) for n in shape][::-1], [float(nd + 1 - d) for d in ds]
 
 
-def _pdr_args(ns, dims, lam):
-    return np.array(ns, dtype=np.int32), np.array(dims, dtype=np.float64), np.array(lam, dtype=np.float64)
-
-
 def _ws_floats(ws):
     """(the penalties as a list of floats, ws when it is a tensor else None) of a list, ndarray or 1-D tensor; ws is not written."""
     import torch
@@ -707,117 +559,33 @@ def _ws_floats(ws):
     return [float(v) for v in np.asarray(ws, dtype=np.float64).ravel()], None
 
 
-def _nd_fns(lib, solver, dtype):
-    """(no-grad solve, tape_bytes, record, vjp) entry points of solver ("PDR_TV", "PD_TV" or "PD2_TV") for a torch dtype."""
-    import torch
-    sfx = "f32" if dtype == torch.float32 else "f64"
-    return tuple(getattr(lib, "proxtv_%s_%s" % (solver, k)) for k in ("dev_" + sfx, "tape_bytes", "record_dev_" + sfx, "vjp_dev_" + sfx))
-
-
-def _nd_owner(solver):
-    """The public function whose ``last_info`` a solve of this solver sets."""
-    return tvgen_pdr if solver == "PDR_TV" else tvgen
-
-
-def _nd_torch(solver, xin, ns, dims, lam, max_iters):
-    """proxtv_<solver>_dev_* on the current stream; lam: the penalties as floats (the call gets a float64 copy, which PDR_TV and
-    PD_TV scale in place)."""
-    import torch
-    nsa, dsa, lama = _pdr_args(ns, dims, lam)
-    out = torch.empty_strided(xin.shape, xin.stride(), dtype=xin.dtype, device=xin.device)
-    info = np.zeros(_N_INFO)
-    fn = _nd_fns(require_device(), solver, xin.dtype)[0]
-    st = C.c_void_p(torch.cuda.current_stream(xin.device).cuda_stream)
-    with torch.cuda.device(xin.device):
-        ok = fn(C.c_void_p(xin.data_ptr()), _ptr(lama), _ptr(dsa), C.c_void_p(out.data_ptr()), _ptr(info), _ptr(nsa), len(ns), len(lam),
-                int(max_iters), st)
-    _check(ok and info[2] != 3, "%s (device)" % solver)
-    _nd_owner(solver).last_info = info
-    return out
-
-
-_ND_FN = None
-
-
-def _nd_fn():
-    """torch.autograd.Function around the N-D solvers PDR_TV, PD_TV and PD2_TV on the device (made on first use, so that numpy users
-    never import torch).
-
-    forward(xin, ws_t, solver, ns, dims, lam, max_iters): xin column-major over ns (see _pdr_layout), lam the unscaled penalties as
-    floats, ws_t the tensor they came from (or None; only receives the gradient; a 0-dim ws_t is one penalty shared by every term).
-    proxtv_<solver>_record_dev_* -- the solve of _nd_torch, keeping on ctx the segmentation tape (a uint8 CUDA tensor,
-    proxtv_<solver>_tape_bytes() long) and the iteration count the solve ran (the Dykstra solvers' stop rule picks it).
-    backward: proxtv_<solver>_vjp_dev_* on the current stream; the gradient of ws_t is npen * glam for PDR_TV and PD_TV (glam: the
-    gradients of the scaled penalties), glam for PD2_TV, in float64, summed over the terms for a 0-dim ws_t."""
-    global _ND_FN
-    if _ND_FN is not None:
-        return _ND_FN
-    import torch
-    from torch.autograd.function import once_differentiable
-
-    class ND(torch.autograd.Function):
-        @staticmethod
-        def forward(ctx, xin, ws_t, solver, ns, dims, lam, max_iters):
-            nsa, dsa, lama = _pdr_args(ns, dims, lam)
-            _, tape_bytes, record, _ = _nd_fns(require_device(), solver, xin.dtype)
-            out = torch.empty_strided(xin.shape, xin.stride(), dtype=xin.dtype, device=xin.device)
-            nb = int(tape_bytes(_ptr(nsa), len(ns), len(lam), int(max_iters)))     # 0: too large; the record call refuses it
-            tape = torch.empty(max(nb, 256), dtype=torch.uint8, device=xin.device)
-            info = np.zeros(_N_INFO)
-            st = C.c_void_p(torch.cuda.current_stream(xin.device).cuda_stream)
-            with torch.cuda.device(xin.device):
-                ok = record(C.c_void_p(xin.data_ptr()), _ptr(lama), _ptr(dsa), C.c_void_p(out.data_ptr()), _ptr(info), _ptr(nsa),
-                            len(ns), len(lam), int(max_iters), C.c_void_p(tape.data_ptr()), tape.numel(), st)
-            _check(ok and info[2] != 3, "%s (recorded, device)" % solver)
-            _nd_owner(solver).last_info = info
-            ctx.save_for_backward(tape)
-            ctx.geom = (solver, nsa, dsa, int(max_iters), int(info[0]), tuple(out.shape), out.stride(), out.dtype)
-            ctx.ws_meta = (ws_t.dtype, ws_t.device, ws_t.shape) if ws_t is not None else None
-            return out
-
-        @staticmethod
-        @once_differentiable
-        def backward(ctx, gout):
-            (tape,) = ctx.saved_tensors
-            solver, nsa, dsa, max_iters, iters, shape, stride, dt = ctx.geom
-            need_x, need_ws = ctx.needs_input_grad[:2]
-            npen = len(dsa)
-            dev = tape.device
-            g = torch.empty_strided(shape, stride, dtype=dt, device=dev)      # the upstream gradient in the output's layout
-            g.copy_(gout)
-            gY = torch.empty_strided(shape, stride, dtype=dt, device=dev)
-            glam = torch.empty(npen, dtype=torch.float64, device=dev) if need_ws else None
-            vjp = _nd_fns(require_device(), solver, dt)[3]
-            it = () if solver == "PDR_TV" else (iters,)                          # PDR_TV runs exactly max_iters iterations
-            st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            with torch.cuda.device(dev):
-                _check(vjp(_ptr(nsa), len(nsa), npen, _ptr(dsa), max_iters, *it, C.c_void_p(tape.data_ptr()), C.c_void_p(g.data_ptr()),
-                           C.c_void_p(gY.data_ptr()), C.c_void_p(glam.data_ptr()) if glam is not None else None, st),
-                       "%s backward (device)" % solver)
-            g_ws = None
-            if need_ws:
-                dtw, devw, shw = ctx.ws_meta
-                gl = glam if solver == "PD2_TV" else glam * float(npen)
-                if len(shw) == 0:
-                    gl = gl.sum(dtype=torch.float64)
-                g_ws = gl.to(dtype=dtw, device=devw).reshape(shw)
-            return (gY if need_x else None), g_ws, None, None, None, None, None
-
-    _ND_FN = ND
-    return ND
-
-
-def _nd_torch_entry(solver, x, lam, ws_t, ds, max_iters):
-    """The torch path of tvgen_pdr, tvgen and tv1_2d(method='pd'): differentiable when grad mode is on and x, or the penalty tensor
-    ws_t, requires grad; otherwise exactly _nd_torch.  lam: the penalties as floats; ws_t: None, a 1-D tensor of them, or a 0-dim
-    tensor shared by every term.  Nothing the caller passed is written."""
-    import torch
+def _nd_torch(solver, x, lam, ws_t, ds, max_iters):
+    """The torch path of tvgen_pdr, tvgen and tv1_2d(method='pd'); recorded by the Function when grad mode is on and x, or the
+    penalty tensor ws_t, requires grad.  lam: the penalties as floats; ws_t: None, a 1-D tensor of them, or a 0-dim tensor shared by
+    every term.  Nothing the caller passed is written: the solve gets a float64 copy of lam, which PDR_TV and PD_TV scale in place."""
     assert len(lam) == len(ds)
     assert ws_t is None or tuple(ws_t.shape) in ((), (len(lam),)), "ws must be one penalty per term, or one 0-dim penalty for all"
     ns, dims, xin = _pdr_layout(x, ds)
-    if torch.is_grad_enabled() and (x.requires_grad or (ws_t is not None and ws_t.requires_grad)):
-        return _nd_fn().apply(xin, ws_t, solver, ns, dims, lam, int(max_iters))
-    return _nd_torch(solver, xin, ns, dims, lam, max_iters)
+    args = (solver, np.array(ns, dtype=np.int32), np.array(dims, dtype=np.float64), np.array(lam, dtype=np.float64), int(max_iters))
+    if _needs_grad(x, ws_t):
+        return _autograd().ND.apply(xin, ws_t, *args)
+    return _nd_solve(xin, *args)[0]
+
+
+def _nd_solve(xin, solver, nsa, dsa, lama, max_iters, tape=None):
+    """proxtv_<solver>_dev_* (solver: "PDR_TV", "PD_TV" or "PD2_TV") on xin, column-major over nsa (see _pdr_layout), or given a tape
+    (a uint8 CUDA tensor, proxtv_<solver>_tape_bytes() long) proxtv_<solver>_record_dev_*, the same solve recording every prox pass's
+    segmentation.  Sets the last_info of the public function that runs the solver; returns (result in xin's layout, info)."""
+    import torch
+    out = torch.empty_strided(xin.shape, xin.stride(), dtype=xin.dtype, device=xin.device)
+    info = np.zeros(_N_INFO)
+    args = (xin, lama, dsa, out, info, nsa, len(nsa), len(lama), max_iters)
+    if tape is None:
+        _dev_call(solver + "_dev", xin, *args, info=info)
+    else:
+        _dev_call(solver + "_record_dev", xin, *args, tape, tape.numel(), info=info)
+    (tvgen_pdr if solver == "PDR_TV" else tvgen).last_info = info
+    return out, info
 
 
 def tvgen_pdr(x, ws, ds, ps, n_threads=1, max_iters=0):
@@ -846,7 +614,7 @@ def tvgen_pdr(x, ws, ds, ps, n_threads=1, max_iters=0):
         if np.any(force_float_matrix(ps) != 1):
             raise NotImplementedError("proxtv_b200 implements TV-L1 (p = 1) penalty terms only")
         lam, ws_t = _ws_floats(ws)
-        return _nd_torch_entry("PDR_TV", x, lam, ws_t, ds, max_iters)
+        return _nd_torch("PDR_TV", x, lam, ws_t, ds, max_iters)
     info = np.zeros(_N_INFO)
     x = np.asfortranarray(x, dtype="float64")
     ws = force_float_matrix(ws)
@@ -864,3 +632,129 @@ def tvgen_pdr(x, ws, ds, ps, n_threads=1, max_iters=0):
 
 
 tvgen_pdr.last_info = None
+
+
+# ======================================================================================================================
+# torch autograd
+# ======================================================================================================================
+@functools.cache
+def _autograd():
+    """The torch.autograd.Function of each differentiable solver, made on first use so that numpy users never import torch.
+
+    Each forward is the solver's no-grad solve, given a tape by the iterative solvers; each backward runs the solver's vector-Jacobian
+    product entry point on the current stream and returns None for an input that needs no gradient.  A penalty given as a float
+    comes with the tensor it was read from (w_t / ws_t, or None), which only receives the gradient.  Double backward is not
+    supported."""
+    import torch
+    from torch.autograd.function import once_differentiable
+
+    class ProxRows(torch.autograd.Function):
+        """apply(x, w, w_t, wt) of _prox_rows.  backward: proxtv_prox_fibers_vjp_dev_* -- gx = segment means of the upstream
+        gradient, gw per edge."""
+        @staticmethod
+        def forward(ctx, x, w, w_t, wt):
+            y = _prox_rows(x, w, wt)
+            ctx.save_for_backward(y, wt)
+            ctx.w = w
+            ctx.w_like = (w_t.dtype, w_t.device, ()) if w_t is not None else None
+            return y
+
+        @staticmethod
+        @once_differentiable
+        def backward(ctx, gy):
+            y, wt = ctx.saved_tensors
+            need_x, _, need_w_t, need_wt = ctx.needs_input_grad
+            B, L = y.shape
+            g = gy.to(dtype=y.dtype).contiguous()
+            gx = torch.empty_like(y)
+            gw = torch.empty((B, max(L - 1, 0)), dtype=y.dtype, device=y.device) if (need_w_t or need_wt) else None
+            _dev_call("prox_fibers_vjp_dev", y, y, g, gx, gw, B, L, 1, ctx.w, wt)
+            g_w = _penalty_grad(gw, ctx.w_like) if need_w_t else None
+            return (gx if need_x else None), None, g_w, (gw if need_wt else None)
+
+    class DRW(torch.autograd.Function):
+        """apply(Y, W1, W2, max_iters) of _drw_solve.  backward: proxtv_DR2L1W_TV_vjp_dev_*, with NULL for a weight map whose input
+        does not need its gradient."""
+        @staticmethod
+        def forward(ctx, Y, W1, W2, max_iters):
+            N, M = Y.shape
+            tape = torch.empty(int(require_device().proxtv_DR2L1W_TV_tape_bytes(M, N, max_iters)), dtype=torch.uint8, device=Y.device)
+            out = _drw_solve(Y, W1, W2, max_iters, tape)
+            ctx.save_for_backward(tape)
+            ctx.geom = (M, N, max_iters)
+            return out
+
+        @staticmethod
+        @once_differentiable
+        def backward(ctx, gout):
+            (tape,) = ctx.saved_tensors
+            M, N, max_iters = ctx.geom
+            need_y, need_w1, need_w2, _ = ctx.needs_input_grad
+            g = gout.contiguous()
+            gY = torch.empty((N, M), dtype=g.dtype, device=g.device)
+            gW1 = torch.empty((N, M - 1), dtype=g.dtype, device=g.device) if need_w1 else None
+            gW2 = torch.empty((N - 1, M), dtype=g.dtype, device=g.device) if need_w2 else None
+            _dev_call("DR2L1W_TV_vjp_dev", g, M, N, max_iters, tape, g, gY, gW1, gW2)
+            return (gY if need_y else None), gW1, gW2, None
+
+    class DR2(torch.autograd.Function):
+        """apply(xin, w, w_t, geom) of _dr2_solve.  backward: proxtv_DR2_TV_vjp_dev_*, the exact vector-Jacobian product of the
+        unrolled iteration; glam per image and axis."""
+        @staticmethod
+        def forward(ctx, xin, w, w_t, geom):
+            M, N, batch, _, max_iters = geom
+            tape = torch.empty(int(require_device().proxtv_DR2_TV_tape_bytes(M, N, batch, max_iters)), dtype=torch.uint8, device=xin.device)
+            out = _dr2_solve(xin, w, geom, tape)
+            ctx.save_for_backward(tape)
+            ctx.geom, ctx.layout = geom, (out.shape, out.stride(), out.dtype)
+            ctx.w_like = (w_t.dtype, w_t.device, ()) if w_t is not None else None
+            return out
+
+        @staticmethod
+        @once_differentiable
+        def backward(ctx, gout):
+            (tape,) = ctx.saved_tensors
+            M, N, batch, row_major, max_iters = ctx.geom
+            shape, stride, dt = ctx.layout
+            need_x, _, need_w_t, _ = ctx.needs_input_grad
+            g = torch.empty_strided(shape, stride, dtype=dt, device=tape.device)      # the upstream gradient in the output's layout
+            g.copy_(gout)
+            gY = torch.empty_strided(shape, stride, dtype=dt, device=tape.device)
+            glam = torch.empty(2 * batch, dtype=torch.float64, device=tape.device) if need_w_t else None
+            _dev_call("DR2_TV_vjp_dev", g, M, N, batch, row_major, max_iters, tape, g, gY, glam)
+            g_w = _penalty_grad(glam, ctx.w_like) if need_w_t else None
+            return (gY if need_x else None), None, g_w, None
+
+    class ND(torch.autograd.Function):
+        """apply(xin, ws_t, solver, nsa, dsa, lama, max_iters) of _nd_solve; ctx also keeps the iteration count the solve ran (the
+        Dykstra solvers' stop rule picks it).  backward: proxtv_<solver>_vjp_dev_*; the gradient of ws_t is npen * glam for PDR_TV
+        and PD_TV (glam: the gradients of the scaled penalties), glam for PD2_TV."""
+        @staticmethod
+        def forward(ctx, xin, ws_t, solver, nsa, dsa, lama, max_iters):
+            tape_bytes = getattr(require_device(), "proxtv_%s_tape_bytes" % solver)
+            nb = int(tape_bytes(_ptr(nsa), len(nsa), len(lama), max_iters))      # 0: too large; the record call refuses it
+            tape = torch.empty(max(nb, 256), dtype=torch.uint8, device=xin.device)
+            out, info = _nd_solve(xin, solver, nsa, dsa, lama, max_iters, tape)
+            ctx.save_for_backward(tape)
+            ctx.geom, ctx.layout = (solver, nsa, dsa, max_iters, int(info[0])), (out.shape, out.stride(), out.dtype)
+            ctx.ws_like = (ws_t.dtype, ws_t.device, ws_t.shape) if ws_t is not None else None
+            return out
+
+        @staticmethod
+        @once_differentiable
+        def backward(ctx, gout):
+            (tape,) = ctx.saved_tensors
+            solver, nsa, dsa, max_iters, iters = ctx.geom
+            shape, stride, dt = ctx.layout
+            need_x, need_ws = ctx.needs_input_grad[:2]
+            npen = len(dsa)
+            g = torch.empty_strided(shape, stride, dtype=dt, device=tape.device)      # the upstream gradient in the output's layout
+            g.copy_(gout)
+            gY = torch.empty_strided(shape, stride, dtype=dt, device=tape.device)
+            glam = torch.empty(npen, dtype=torch.float64, device=tape.device) if need_ws else None
+            it = () if solver == "PDR_TV" else (iters,)                               # PDR_TV runs exactly max_iters iterations
+            _dev_call(solver + "_vjp_dev", g, nsa, len(nsa), npen, dsa, max_iters, *it, tape, g, gY, glam)
+            g_ws = _penalty_grad(glam if solver == "PD2_TV" else glam * float(npen), ctx.ws_like) if need_ws else None
+            return (gY if need_x else None), g_ws, None, None, None, None, None
+
+    return types.SimpleNamespace(ProxRows=ProxRows, DRW=DRW, DR2=DR2, ND=ND)

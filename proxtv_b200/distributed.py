@@ -185,33 +185,21 @@ def _sharded_pipelined(x, w, max_iters, src, group, solver, device, pieces, timi
 # ======================================================================================================================
 # ONE image over several GPUs (SURVEY.md 8f N3)
 # ======================================================================================================================
-def _lane_passes(device, dtype):
+def _lane_passes():
     """The two passes of a Douglas-Rachford iteration on this rank's slabs, as launches of the lane engine through the C ABI
     (proxtv_lane_prox_dev_*: device pointers, current stream).  Slabs are column-major, held as row-major tensors [columns][rows]."""
-    import ctypes as C
     import torch
-    from . import require_device
-    lib = require_device()
-    f32 = dtype == torch.float32
-    fn = lib.proxtv_lane_prox_dev_f32 if f32 else lib.proxtv_lane_prox_dev_f64
-    vp = C.c_void_p
-
-    def st():
-        return vp(torch.cuda.current_stream(device).cuda_stream)
+    from . import _dev_call, require_device
+    require_device()                               # refuse here, before the first exchange, rather than inside the iteration
 
     def cols(t_c, w):                              # t_c [n_cols][M]: every column is a contiguous fiber
         out = torch.empty_like(t_c)
-        ok = fn(0, vp(t_c.data_ptr()), None, None, vp(out.data_ptr()), t_c.shape[0], t_c.shape[1], 1, float(w), st())
-        if not ok:
-            raise RuntimeError("lane engine refused the column slab %s: %s" % (tuple(t_c.shape), lib.proxtv_last_error()))
+        _dev_call("lane_prox_dev", t_c, 0, t_c, None, None, out, t_c.shape[0], t_c.shape[1], 1, float(w))
         return out
 
     def rows(final, y_r, x1_r, t_r, w):            # slabs [N][m]: row fibers have stride m, adjacent rows are adjacent in memory
         out = torch.empty_like(t_r)
-        ok = fn(2 if final else 1, vp(y_r.data_ptr()), vp(x1_r.data_ptr()), vp(t_r.data_ptr()), vp(out.data_ptr()),
-                t_r.shape[1], t_r.shape[0], t_r.shape[1], float(w), st())
-        if not ok:
-            raise RuntimeError("lane engine refused the row slab %s: %s" % (tuple(t_r.shape), lib.proxtv_last_error()))
+        _dev_call("lane_prox_dev", t_r, 2 if final else 1, y_r, x1_r, t_r, out, t_r.shape[1], t_r.shape[0], t_r.shape[1], float(w))
         return out
 
     return cols, rows
@@ -257,7 +245,7 @@ def tv1_2d_single_sharded(x, w, max_iters=0, src=0, group=None, passes=None, dev
     m, n = M // G, N // G
     maxit = int(max_iters) if max_iters and max_iters > 0 else 35              # src/TV2Dopt.cpp:387
     if passes is None:
-        passes = _lane_passes(device, dtype)
+        passes = _lane_passes()
     prox_cols, row_pass = passes
 
     def all_to_all(send):                          # [G][n][m] -> [G][n][m], chunk g goes to / comes from rank g
