@@ -65,14 +65,17 @@ cudaError_t prox_fibers_ex(const T* A, const T* B, const T* C, InOp op, T* X, in
             cudaError_t e = prox_fibers_chunked_contig<T>(A, B, C, op, X, out_op, g, lam, lamv, st);
             if (e != cudaErrorInvalidConfiguration) return e;
             cudaGetLastError();
+            span.cancel();                  // refused before launching: the launch counters count kernels that ran
             // too long for shared memory: overlapping tiles, verified stitching (long_fiber.cu); the scratch convention for
             // this case is lf_scratch_elems() elements, which the 1D host entry points provide
             // (plain results only: the agreement test of the stitching compares prox values, which the fused output forms would hide)
             if (!lamv && out_op == OUT_X && scratch && scratch_elems >= lf_scratch_elems(g.nf, g.len)) {
+                KernelSpan lspan(KC_PROX_CONTIG, 1, st);
                 e = prox_long_fibers<T>(A, B, op, X, out_op, g, lam, scratch, lf_scratch_elems(g.nf, g.len), st);
                 if (e == cudaSuccess || e == cudaErrorNotReady) long_fiber_note(e == cudaSuccess ? 1 : 0);
                 if (e == cudaSuccess) return e;
                 if (e != cudaErrorInvalidConfiguration && e != cudaErrorNotReady) return e;
+                if (e == cudaErrorInvalidConfiguration) lspan.cancel();      // NotReady: the tiles ran, their check failed
                 cudaGetLastError();
             }
         } else if (!lamv) {
@@ -102,7 +105,8 @@ cudaError_t prox_fibers_ex(const T* A, const T* B, const T* C, InOp op, T* X, in
                 T* Cv = scratch + 2 * n; uint32_t* Mk = reinterpret_cast<uint32_t*>(Cv + g.nf * lpf);
                 { KernelSpan span(KC_PROX_STRIDED, 1, st);
                   e = sparse ? prox_fibers_chunked_contig_sparse<T>(t1, t2, gc, lam, nullptr, Mk, Cv, st)
-                             : prox_fibers_chunked_contig<T>(t1, nullptr, nullptr, IN_A, t2, OUT_X, gc, lam, nullptr, st); }
+                             : prox_fibers_chunked_contig<T>(t1, nullptr, nullptr, IN_A, t2, OUT_X, gc, lam, nullptr, st);
+                  if (e == cudaErrorInvalidConfiguration) span.cancel(); }
                 if (e == cudaSuccess) {
                     KernelSpan span(KC_ELEMENTWISE, 1, st);
                     if (sparse) return out_op == OUT_X ? scatter_fibers_sparse<T>(t2, Mk, Cv, nullptr, nullptr, nullptr, IN_A, OUT_X, X, g, st)
