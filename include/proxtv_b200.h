@@ -326,8 +326,15 @@ int proxtv_lane_guard_last(void);
  * and the whole call falls back to the sequential kernel when a check fails.  What the latest proxtv_prox_fibers_* call (or 1D entry
  * point of Part 1) on the current device did: 1 used the tiles, 0 tried them and fell back, -1 did not try them. */
 int proxtv_long_fiber_last(void);
-/* tools: device buffer of 4 x cap_tasks uint64 that receives, per warp task of the next launches, {start ns, scan end ns, end ns, SM id}
- * (globaltimer); NULL switches the log off. */
+/* tools: device buffer of 16 x cap_tasks uint64 that receives, per warp task of the next lane launches (a launch with more tasks than
+ * cap_tasks is not logged):
+ *   [0] start ns  [1] scan end ns  [2] end ns (globaltimer)  [3] SM id
+ *   [4] epochs  [5] scan steps  [6] epochs of fewer than 8 steps (every lane near the landed rows)  [7] waits for a tile
+ *   [8] SM cycles (clock64) in the epoch loop, of which  [9] blocked on a tile  [10] other epochs where no lane could move (tail,
+ *   retirement)  [11] sweep and drain (including the drain's operand loads)  [12] feed (tile requests, landing)  [13] scan
+ *   (the remainder is the epochs' warp reductions)
+ *   [14] rows the task scans (owned + halo)  [15] 0
+ * NULL switches the log off. */
 void proxtv_lane_tasklog(unsigned long long *dev, long long cap_tasks);
 
 #ifdef __cplusplus

@@ -91,9 +91,10 @@ template <typename T> struct LaneArgs {
     int* rec;                       // [5][plan.nmax][slabs*gps*32] chunk records (in, out, overflow, in2, in3)
     int* group_count;               // [slabs*gps] finished-task counters (self-resetting)
     unsigned long long* stats;      // [0] repair scans, [1] retired lanes
-    unsigned long long* tlog;       // optional (tools): per task {start ns, scan end ns, end ns, SM id}
+    unsigned long long* tlog;       // optional (tools): per task TLOG_WORDS words, see k_lane
     long long ntasks;
 };
+constexpr int TLOG_WORDS = 16;
 
 // fused arithmetic of a pass: what a lane scans (in) and what it writes for prox value x (out)
 template <typename T, int OP> struct PassOp {
@@ -493,7 +494,7 @@ __device__ __noinline__ int repair_fiber(const LaneArgs<T>* a, const ChunkPlan p
 __device__ __forceinline__ unsigned long long gtimer() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 __device__ __forceinline__ unsigned smid() { unsigned r; asm volatile("mov.u32 %0, %%smid;" : "=r"(r)); return r; }
 
-template <typename T, int W, int RT, int TITER, int OP, int NW, int LAY>
+template <typename T, int W, int RT, int TITER, int OP, int NW, int LAY, bool LOG>
 __global__ void __launch_bounds__(NW * 32, (12 + NW - 1) / NW) k_lane(const __grid_constant__ LaneArgs<T> a) {
     using SM = LaneSmem<T, W, RT, OP, LAY, NW>;
     extern __shared__ __align__(1024) unsigned char smem[];
@@ -515,8 +516,14 @@ __global__ void __launch_bounds__(NW * 32, (12 + NW - 1) / NW) k_lane(const __gr
     }
     __syncthreads();                                    // the only CTA barrier: reciprocal table ready
     if (!has_task) return;
-    if (a.tlog && lane == 0) { a.tlog[task * 4 + 0] = gtimer(); a.tlog[task * 4 + 3] = smid(); }
-    struct TLogEnd { unsigned long long* p; __device__ ~TLogEnd() { if (p) *p = gtimer(); } } tlog_end{a.tlog && lane == 0 ? a.tlog + task * 4 + 2 : nullptr};
+    // task log (tools: the LOG instantiation, launched only when a.tlog is set), TLOG_WORDS words per task:
+    //   [0] start ns  [1] scan end ns  [2] end ns (globaltimer)  [3] SM id  [4] epochs  [5] scan steps  [6] starved epochs (< DMIN steps)
+    //   [7] tile waits  [8] cycles in the epoch loop (clock64), of which  [9] blocked on a tile  [10] rest of nobody-can-move (tail,
+    //   retirement)  [11] sweep + drain  [12] feed (requests, landing)  [13] scan  (the remainder: the epoch's warp reductions)
+    //   [14] rows the task scans (owned + halo)  [15] 0
+    unsigned long long* const tl = LOG ? a.tlog + task * TLOG_WORDS : nullptr;
+    if (tl && lane == 0) { tl[0] = gtimer(); tl[3] = smid(); }
+    struct TLogEnd { unsigned long long* p; __device__ ~TLogEnd() { if (p) *p = gtimer(); } } tlog_end{tl && lane == 0 ? tl + 2 : nullptr};
 
     long long group; int chunk, nc;
     a.plan.locate(task, &group, &chunk, &nc);
@@ -536,17 +543,24 @@ __global__ void __launch_bounds__(NW * 32, (12 + NW - 1) / NW) k_lane(const __gr
     env.dw.wbase = s32(win); env.dw.lane8 = lane * (uint32_t)sizeof(T); env.dw.flg = s32(flg) + lane * (uint32_t)Window<T, W>::FP; env.dw.rcp = s32(rcp);
     Window<T, W> w{win, flg};
     env.L.init(w, lane, g, a.lam, valid);
+    TaskStats ts{};
+    TaskStats* const sp = LOG ? &ts : nullptr;
+    const long long tc0 = LOG ? clock64() : 0;
     if constexpr (LAY == LAY_CONTIG) {
         FeedContig<T, W> feed{&a, win, bar, x0, g.p0 / FeedContig<T, W>::R, lane};
         DrainContig<T, W> drain{&a, stB, x0, lane, g.ce};
-        warp_task<T, W, TITER>(env, feed, drain, w, rcp, g, a.lam, TITER + TITER / 2 + FeedContig<T, W>::R, (TaskStats*)nullptr);
+        warp_task<T, W, TITER>(env, feed, drain, w, rcp, g, a.lam, TITER + TITER / 2 + FeedContig<T, W>::R, sp);
     } else {
         FeedStrided<T, W, RT, OP> feed{&a, win, stB, stC, bar, x0, z, g.p0 / RT, lane};
         DrainStrided<T, W, OP> drain; drain.B = a.B; drain.C = a.C; drain.X = a.X; drain.X2 = a.X2; drain.gbase = gbase; drain.stride = a.inc;
         drain.pf_row = -1; drain.pol = policy_evict_first(); drain.ce = g.ce; drain.tbase = tgroup; drain.n = pl.n; drain.nvalid = (int)(a.per_slab - x0 < LANES ? a.per_slab - x0 : LANES);
-        warp_task<T, W, TITER>(env, feed, drain, w, rcp, g, a.lam, TITER + TITER / 2 + RT, (TaskStats*)nullptr);
+        warp_task<T, W, TITER>(env, feed, drain, w, rcp, g, a.lam, TITER + TITER / 2 + RT, sp);
     }
-    if (a.tlog && lane == 0) a.tlog[task * 4 + 1] = gtimer();
+    if (tl && lane == 0) {
+        tl[1] = gtimer();
+        tl[4] = ts.epochs; tl[5] = ts.iters; tl[6] = ts.starved; tl[7] = ts.waits; tl[8] = clock64() - tc0;
+        tl[9] = ts.c_wait; tl[10] = ts.c_stuck; tl[11] = ts.c_sweep; tl[12] = ts.c_feed; tl[13] = ts.c_scan; tl[14] = g.ce - g.p0; tl[15] = 0;
+    }
 
     // ---- chunk records; the last warp of the fiber group to finish verifies (and repairs) its 32 fibers ----
     int* rec = a.rec;
@@ -640,7 +654,7 @@ static long long lane_scratch_bytes(long long groups_cap, long long nf, int len)
 template <typename T, int W, int RT, int TITER, int OP, int NW, int LAY>
 static cudaError_t launch_v(LaneArgs<T>& a, cudaStream_t st, int* slots) {
     using SM = LaneSmem<T, W, RT, OP, LAY, NW>;
-    auto kern = k_lane<T, W, RT, TITER, OP, NW, LAY>;
+    auto kern = k_lane<T, W, RT, TITER, OP, NW, LAY, false>;
     const size_t smem = SM::total;
     static int s_slots = 0;                      // per instantiation: resident warps on the current device
     if (!s_slots) {
@@ -655,7 +669,13 @@ static cudaError_t launch_v(LaneArgs<T>& a, cudaStream_t st, int* slots) {
     }
     if (slots) { *slots = s_slots; return cudaSuccess; }
     const unsigned blocks = (unsigned)((a.ntasks + NW - 1) / NW);
-    kern<<<blocks, NW * 32, smem, st>>>(a);
+    if (a.tlog) {                                // tools: the instrumented copy (same shared memory, same residency)
+        auto klog = k_lane<T, W, RT, TITER, OP, NW, LAY, true>;
+        cudaError_t e = cudaFuncSetAttribute(klog, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        cudaFuncSetAttribute(klog, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        klog<<<blocks, NW * 32, smem, st>>>(a);
+    } else kern<<<blocks, NW * 32, smem, st>>>(a);
     return cudaGetLastError();
 }
 

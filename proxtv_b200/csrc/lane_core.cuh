@@ -245,13 +245,24 @@ template <typename T> struct Lane {
 //   Feed:  R rows per tile (8) ; MAXQ tiles that may be outstanding ; request(env, row0) ; bool landed(env, row0, block)
 //   Drain: prefetch(r0, ce, valid) ; rows8(w, r0, cnt, lane, xs, valid) inside each() for every aligned group of 8 owned rows, in order ; flush(env, w,
 //          upto, final) ; hold(): first row the window still has to keep for it
-struct TaskStats { int epochs, retired, tail, iters; };
+// stats (optional; nullptr in production): counters, and on the device where the warp's cycles go (clock64; 0 on the host)
+//   starved: scan epochs shorter than DMIN steps (every lane close to the landed frontier)
+//   c_wait: blocked on the next tile (nobody can move) ; c_stuck: the rest of the nobody-can-move branch (tail, retirement)
+//   c_sweep: sweep + drain, including the drain's operand prefetch ; c_feed: requests + landing ; c_scan: scan steps + settle
+struct TaskStats { int epochs, retired, tail, iters; int starved, waits; long long c_wait, c_stuck, c_sweep, c_feed, c_scan; };
+PTV_HD long long task_clock() {
+#ifdef __CUDA_ARCH__
+    return clock64();
+#else
+    return 0;
+#endif
+}
 
 template <typename T, int W, int TITER, class Env, class Feed, class Drain>
 PTV_HD void warp_task(Env& env, Feed& feed, Drain& drain, const Window<T, W>& w, const acc_t* __restrict__ rcp, const TaskGeom g, T lam,
                       int ahead, TaskStats* stats) {
     constexpr int R = Feed::R;
-    constexpr int DMIN = 8;           // lanes closer than this to the frontier sit an epoch out rather than shorten it for everybody
+    constexpr int DMIN = 8;           // rows kept in front of a lane that overruns its chunk; epochs shorter than this count as starved
     const acc_t lam2 = 2.0 * (acc_t)lam;
     int row_lo = g.p0;                // first row still held by the window
     int row_req = g.p0;               // rows below have been requested
@@ -266,6 +277,7 @@ PTV_HD void warp_task(Env& env, Feed& feed, Drain& drain, const Window<T, W>& w,
         const int maxi = env.rmax([&](Lane<T>& L, int) { return L.done ? -1 : L.i; });
         const int low = env.rmin([&](Lane<T>& L, int) { return L.done ? BIG : L.last + 1; });
         const bool all_done = (low == BIG);
+        long long tc = stats ? task_clock() : 0;
         // ---- sweep finished rows (aligned groups of 8), slide the window ----
         {
             int upto = low < g.ce ? low : g.ce;
@@ -321,6 +333,7 @@ PTV_HD void warp_task(Env& env, Feed& feed, Drain& drain, const Window<T, W>& w,
         if (all_done) break;
         if (stats) stats->epochs = epoch + 1;
         env.each([&](Lane<T>& L, int) { drain.prefetch(fill_pos, g.ce, L.valid); });     // operands of the next group to be swept
+        if (stats) { const long long t = task_clock(); stats->c_sweep += t - tc; tc = t; }
         // ---- feed: keep `ahead` rows in front of the fastest lane, never more than the window holds ----
         {
             int want = maxi + ahead;
@@ -333,19 +346,24 @@ PTV_HD void warp_task(Env& env, Feed& feed, Drain& drain, const Window<T, W>& w,
             if (Feed::MAXQ < 2)
                 while (row_req < want && row_req + R <= row_lo + W && row_req - row_hi < Feed::MAXQ * R) { feed.request(env, row_req); row_req += R; }
         }
-        // ---- how many steps can every participating lane take? ----
+        if (stats) { const long long t = task_clock(); stats->c_feed += t - tc; tc = t; }
+        // ---- how many steps can the lanes take?  Each lane runs up to TITER steps, as far as the landed rows reach (its own bound:
+        //      a lane never passes lim), so the epoch lasts as long as the lane with the most room needs ----
         const int lim = row_hi < g.n - 1 ? row_hi : g.n - 1;
-        int niter = env.rmin([&](Lane<T>& L, int) { const int d = lim - L.i; return (L.done || d < DMIN) ? BIG : d; });
-        if (niter == BIG) {              // nobody has DMIN rows in front of it: take what there is
-            niter = env.rmin([&](Lane<T>& L, int) { const int d = lim - L.i; return (L.done || d < 1) ? BIG : d; });
-            if (niter == BIG) {          // nobody can move
-                if (row_hi < row_req) { feed.landed(env, row_hi, true); row_hi += R; continue; }        // wait for the next tile
+        int niter = env.rmax([&](Lane<T>& L, int) { const int d = lim - L.i; return L.done ? 0 : d; });
+        {
+            if (niter < 1) {             // nobody can move
+                if (row_hi < row_req) {                                                                  // wait for the next tile
+                    feed.landed(env, row_hi, true); row_hi += R;
+                    if (stats) { stats->waits++; stats->c_wait += task_clock() - tc; }
+                    continue;
+                }
                 // lanes that wait in front of the fiber's last sample: finish them once it is in the window
                 const bool movable = env.any([&](Lane<T>& L, int) { return !L.done && L.i < g.n - 1; });
                 if (!movable && row_hi >= g.n) {
                     env.each([&](Lane<T>& L, int lane) { L.template finish_tail<W>(w, lane, g, lam); });
                     env.sync();
-                    if (stats) stats->tail++;
+                    if (stats) { stats->tail++; stats->c_stuck += task_clock() - tc; }
                     continue;
                 }
                 // stuck: nothing pending, nothing more fits -> retire the lanes that pin the window
@@ -356,22 +374,25 @@ PTV_HD void warp_task(Env& env, Feed& feed, Drain& drain, const Window<T, W>& w,
                     });
                     if (stats) stats->retired++;
                 }
+                if (stats) stats->c_stuck += task_clock() - tc;
                 continue;
             }
         }
         if (niter > TITER) niter = TITER;
+        if (stats) { if (niter < DMIN) stats->starved++; tc = task_clock(); }
         // ---- scan ----
         {
-            const int lim_ = lim, niter_ = niter; const bool ph1_ = ph1;
+            const int lim_ = lim; const bool ph1_ = ph1;
             env.each([&](Lane<T>& L, int lane) {
-                if (!L.done && lim_ - L.i >= niter_) {
-                    env.scan(L, w, lane, g, rcp, lam2, ph1_, niter_);      // Lane::run, or the kernel's equivalent device form
+                const int d = lim_ - L.i;
+                if (!L.done && d >= 1) {
+                    env.scan(L, w, lane, g, rcp, lam2, ph1_, d < TITER ? d : TITER);      // Lane::run, or the kernel's equivalent device form
                     L.template settle<W>(w, lane, g);
                 }
             });
             env.sync();
             if (ph1) ph1 = env.any([&](Lane<T>& L, int) { return !L.done && L.in_rec == REC_NONE; });
-            if (stats) stats->iters += niter;
+            if (stats) { stats->iters += niter; stats->c_scan += task_clock() - tc; }
         }
     }
     drain.flush(env, w, fill_pos, true);

@@ -15,14 +15,14 @@ y = torch.tensor(np.ascontiguousarray(Y.T), device="cuda").t()      # column-maj
 ptv.set_engine(eng)
 out = ptv.tv1_2d(y, 0.2, max_iters=maxit); torch.cuda.synchronize()
 CAP = 1 << 16
-log = torch.zeros(CAP * 4, dtype=torch.int64, device="cuda")
+log = torch.zeros(CAP * 16, dtype=torch.int64, device="cuda")      # 16 words per task (proxtv_lane_tasklog)
 lib.proxtv_profile_enable(1)                     # plain launches (no graph replay), so that the log pointer is seen
 lib.proxtv_lane_stats(1)
 lib.proxtv_lane_tasklog(vp(log.data_ptr()), CAP)
 out = ptv.tv1_2d(y, 0.2, max_iters=maxit); torch.cuda.synchronize()
 lib.proxtv_lane_tasklog(None, 0)
 print("repairs in this solve:", lib.proxtv_lane_stats(1))
-L = log.cpu().numpy().reshape(-1, 4); L = L[L[:, 0] > 0]
+L = log.cpu().numpy().reshape(-1, 16); L = L[L[:, 0] > 0]
 t0 = L[:, 0].min()
 start = (L[:, 0] - t0) / 1e3; scan_end = (L[:, 1] - t0) / 1e3; end = (L[:, 2] - t0) / 1e3
 print("%d tasks in the log (last launches of the solve overwrite earlier ones; tasks of the final pass: those with the latest start)" % len(L))
