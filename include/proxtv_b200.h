@@ -212,6 +212,38 @@ int proxtv_DR2L1W_TV_vjp_dev_f64(size_t M, size_t N, int maxit, const void *tape
                                  double *gW2, void *stream);
 int proxtv_DR2L1W_TV_vjp_dev_f32(size_t M, size_t N, int maxit, const void *tape, const float *gout, float *gY, float *gW1,
                                  float *gW2, void *stream);
+/* DR2L1W_TV on `batch` independent M x N images stored back to back (image b starts at b M N), each solved with exactly the
+ * single-image iteration (its own 2 * mean start value, columns first).  row_major = 0: column-major images, 1: C-ordered images; the
+ * weight maps are back to back per image and laid out in the same order:
+ *     row_major = 0:  Y[b M N + j M + i]   W1[b (M-1) N + j (M-1) + i]   W2[b M (N-1) + j M + i]
+ *     row_major = 1:  Y[b M N + i N + j]   W1[b (M-1) N + i N + j]       W2[b M (N-1) + i (N-1) + j]
+ * W1 weights the edge (i, j)-(i+1, j), W2 the edge (i, j)-(i, j+1).  The (1, 0) call is proxtv_DR2L1W_TV_dev_* itself.  Weights
+ * must be >= 0 (not checked on the device).
+ * dev: returns 0 like DR2L1W_TV (check info[2]); refused (info[2] = 3, nothing written): batch < 0, Y or out NULL, W1 NULL with
+ * M > 1, W2 NULL with N > 1.  record / vjp / tape_bytes: as proxtv_DR2L1W_TV_record_dev_* / _vjp_dev_* / _tape_bytes over all
+ * batch M N elements in storage order (tape_bytes: 0 for batch < 1); also refused: batch < 1, and a tape whose header does not
+ * match dtype, shape, batch, row_major or maxit (a single-image tape included when batch > 1, and a DR2_TV tape).  The gradients
+ * are laid out like Y, W1 and W2; the weight gradients are per image and edge, with no sum across images.
+ * host form (_batched_f64 / _f32): host arrays, synchronous. */
+size_t proxtv_DR2L1W_TV_batched_tape_bytes(size_t M, size_t N, int batch, int maxit);
+int proxtv_DR2L1W_TV_batched_dev_f64(size_t M, size_t N, int batch, int row_major, const double *Y, const double *W1, const double *W2,
+                                     double *out, int maxit, double *info, void *stream);
+int proxtv_DR2L1W_TV_batched_dev_f32(size_t M, size_t N, int batch, int row_major, const float *Y, const float *W1, const float *W2,
+                                     float *out, int maxit, double *info, void *stream);
+int proxtv_DR2L1W_TV_batched_record_dev_f64(size_t M, size_t N, int batch, int row_major, const double *Y, const double *W1,
+                                            const double *W2, double *out, int maxit, void *tape, size_t tape_bytes, double *info,
+                                            void *stream);
+int proxtv_DR2L1W_TV_batched_record_dev_f32(size_t M, size_t N, int batch, int row_major, const float *Y, const float *W1,
+                                            const float *W2, float *out, int maxit, void *tape, size_t tape_bytes, double *info,
+                                            void *stream);
+int proxtv_DR2L1W_TV_batched_vjp_dev_f64(size_t M, size_t N, int batch, int row_major, int maxit, const void *tape, const double *gout,
+                                         double *gY, double *gW1, double *gW2, void *stream);
+int proxtv_DR2L1W_TV_batched_vjp_dev_f32(size_t M, size_t N, int batch, int row_major, int maxit, const void *tape, const float *gout,
+                                         float *gY, float *gW1, float *gW2, void *stream);
+int proxtv_DR2L1W_TV_batched_f64(size_t M, size_t N, int batch, int row_major, const double *Y, const double *W1, const double *W2,
+                                 double *out, int maxit, double *info);
+int proxtv_DR2L1W_TV_batched_f32(size_t M, size_t N, int batch, int row_major, const float *Y, const float *W1, const float *W2,
+                                 float *out, int maxit, double *info);
 
 /* PD2_TV / PD_TV with device arrays y, x (lambdas, dims, ns, info stay on the host).  Synchronous (the stop test needs
  * one 8-byte read-back per iteration).  proxtv_PD_TV_* scale lambdas in place like PD_TV. */

@@ -7,9 +7,9 @@ behaviour and return conventions; the computation runs in hand-written sm_90a CU
 device the calls raise.
 
 Extensions the reference lacks (SURVEY.md section 8b): a leading batch dimension (``tv1_1d_batched``,
-``tv1w_1d_batched``, ``tv1_2d_batched``), float32, and torch CUDA tensors as inputs (device-resident path: no PCIe
+``tv1w_1d_batched``, ``tv1_2d_batched``, ``tv1w_2d_batched``), float32, and torch CUDA tensors as inputs (device-resident path: no PCIe
 traffic, no host transposes -- a C-ordered tensor is handled by swapping the kernels' stride roles).  The batched 1D functions,
-``tv1_2d`` (both methods) / ``tv1_2d_batched``, ``tv1w_2d`` and the N-D ``tvgen`` / ``tvgen_pdr`` are differentiable on torch
+``tv1_2d`` (both methods) / ``tv1_2d_batched``, ``tv1w_2d`` / ``tv1w_2d_batched`` and the N-D ``tvgen`` / ``tvgen_pdr`` are differentiable on torch
 tensors (exact backward kernels).
 """
 import ctypes as C
@@ -22,7 +22,7 @@ from . import _lib
 from ._lib import ProxTVError, load, require_device  # noqa: F401
 
 __all__ = ["tv1_1d", "tv1w_1d", "tv1_2d", "tv1w_2d", "tvgen", "tvgen_pdr", "tv1_1d_batched", "tv1w_1d_batched", "tv1_2d_batched",
-           "set_engine", "set_pinned_results", "ProxTVError"]
+           "tv1w_2d_batched", "set_engine", "set_pinned_results", "ProxTVError"]
 
 _N_INFO = 3                      # prox_tv/__init__.py:67
 ENGINES = {"auto": 0, "seq": 1, "chunked": 2, "chunked-strided": 3, "pipelined": 4, "tspace": 5, "tpose": 6, "lane": 7, "lane-t": 8}
@@ -367,24 +367,78 @@ def _drw_torch(x, w_col, w_row, max_iters):
     xt = x.t().contiguous()
     w1 = w_col.to(device=x.device, dtype=x.dtype).t().contiguous()
     w2 = w_row.to(device=x.device, dtype=x.dtype).t().contiguous()
+    geom = (M, N, 1, 0, int(max_iters))
     if _needs_grad(x, w_col, w_row):
-        return _autograd().DRW.apply(xt, w1, w2, int(max_iters)).t()
-    return _drw_solve(xt, w1, w2, int(max_iters)).t()
+        return _autograd().DRW.apply(xt, w1, w2, geom).t()
+    return _drw_solve(xt, w1, w2, geom).t()
 
 
-def _drw_solve(Y, W1, W2, max_iters, tape=None):
-    """DR2L1W_TV on the solver's buffers Y (N, M), W1 (N, M-1), W2 (N-1, M): proxtv_DR2L1W_TV_dev_*, or given a tape (a uint8 CUDA
-    tensor, proxtv_DR2L1W_TV_tape_bytes() long) proxtv_DR2L1W_TV_record_dev_*, the same solve recording every prox pass's segmentation."""
+def _drw_solve(Y, W1, W2, geom, tape=None):
+    """DR2L1W_TV on the solver's buffers, geom = (M, N, batch, row_major, max_iters): Y and the weight maps W1, W2 laid out as
+    proxtv_DR2L1W_TV_batched_dev_* takes them (their memory, whatever the tensors' shapes): proxtv_DR2L1W_TV_batched_dev_*, or given a
+    tape (a uint8 CUDA tensor, proxtv_DR2L1W_TV_batched_tape_bytes() long) proxtv_DR2L1W_TV_batched_record_dev_*, the same solve
+    recording every prox pass's segmentation.  The result has Y's layout."""
     import torch
-    N, M = Y.shape
-    out = torch.empty_like(Y)
+    out = torch.empty_strided(Y.shape, Y.stride(), dtype=Y.dtype, device=Y.device)
     info = np.zeros(_N_INFO)
-    args = (M, N, Y, W1, W2, out, max_iters)
+    M, N, batch, row_major, max_iters = geom
+    args = (M, N, batch, row_major, Y, W1, W2, out, max_iters)
     if tape is None:       # returns 0 on success, like the reference's DR2L1W_TV: only info[2] == 3 signals a failure
-        _dev_call("DR2L1W_TV_dev", Y, *args, info, rc=False, info=info)
+        _dev_call("DR2L1W_TV_batched_dev", Y, *args, info, rc=False, info=info)
     else:
-        _dev_call("DR2L1W_TV_record_dev", Y, *args, tape, tape.numel(), info)
+        _dev_call("DR2L1W_TV_batched_record_dev", Y, *args, tape, tape.numel(), info)
     return out
+
+
+def tv1w_2d_batched(x, w_col, w_row, max_iters=0):
+    r"""``tv1w_2d`` on every image of x (B, H, W), with per-image weight maps ``w_col`` (B, H-1, W) (edges along columns) and
+    ``w_row`` (B, H, W-1) (edges along rows).  Each image is solved independently with exactly the single-image iteration (its own
+    2 * mean start value, 35 iterations unless ``max_iters`` > 0).
+
+    numpy: float64, or float32 solved in float32; the weights are cast to x's dtype.  Returns a C-ordered (B, H, W) array of x's dtype.
+    torch: a CUDA tensor (float32 / float64).  C-ordered and per-image column-major tensors are solved in place of their layout (no
+    transposes), anything else is made contiguous; the result has the solved tensor's layout.  Weights of any floating dtype or
+    device are moved to x's device and dtype and laid out like it through ordinary autograd ops.  Differentiable with respect to
+    ``x``, ``w_col`` and ``w_row`` like ``tv1w_2d`` (proxtv_DR2L1W_TV_batched_vjp_dev_*, DESIGN.md section 12); an expanded weight
+    (``w.expand(B, H - 1, W)``) gets the sum of its per-edge gradients through autograd.
+    """
+    if _is_torch(x):
+        return _drw_batched_torch(x, w_col, w_row, max_iters)
+    x = np.asarray(x)
+    assert x.ndim == 3
+    B, H, W = x.shape
+    assert np.shape(w_col) == (B, H - 1, W)
+    assert np.shape(w_row) == (B, H, W - 1)
+    assert np.all(np.asarray(w_col) >= 0)
+    assert np.all(np.asarray(w_row) >= 0)
+    dt = np.float32 if x.dtype == np.float32 else np.float64
+    x = np.ascontiguousarray(x, dtype=dt)
+    w1 = np.ascontiguousarray(w_col, dtype=dt)
+    w2 = np.ascontiguousarray(w_row, dtype=dt)
+    out = _pool.empty(x.shape, dt, "C")
+    if x.size:
+        info = np.zeros(_N_INFO)
+        lib = require_device()
+        fn = lib.proxtv_DR2L1W_TV_batched_f32 if dt == np.float32 else lib.proxtv_DR2L1W_TV_batched_f64
+        fn(H, W, B, 1, _ptr(x), _ptr(w1), _ptr(w2), _ptr(out), int(max_iters), _ptr(info))
+        _check(info[2] != 3, "DR2L1W_TV (batched)")
+    return out
+
+
+def _drw_batched_torch(x, w_col, w_row, max_iters):
+    """The torch path of tv1w_2d_batched: the layout of _dr2_layout, the weight maps laid out to match (row_major = 1: C order;
+    0: every image's map column-major)."""
+    M, N, batch, row_major, xin = _dr2_layout(x, batched=True)
+    assert tuple(w_col.shape) == (batch, M - 1, N) and tuple(w_row.shape) == (batch, M, N - 1)
+
+    def lay(w):
+        w = w.to(device=xin.device, dtype=xin.dtype)
+        return w.contiguous() if row_major else w.transpose(1, 2).contiguous().transpose(1, 2)
+    w1, w2 = lay(w_col), lay(w_row)
+    geom = (M, N, batch, row_major, int(max_iters))
+    if _needs_grad(x, w_col, w_row):
+        return _autograd().DRW.apply(xin, w1, w2, geom)
+    return _drw_solve(xin, w1, w2, geom)
 
 
 def _dr2_layout(x, batched):
@@ -673,28 +727,35 @@ def _autograd():
             return (gx if need_x else None), None, g_w, (gw if need_wt else None)
 
     class DRW(torch.autograd.Function):
-        """apply(Y, W1, W2, max_iters) of _drw_solve.  backward: proxtv_DR2L1W_TV_vjp_dev_*, with NULL for a weight map whose input
-        does not need its gradient."""
+        """apply(Y, W1, W2, geom) of _drw_solve.  backward: proxtv_DR2L1W_TV_batched_vjp_dev_*, with NULL for a weight map whose input
+        does not need its gradient; the upstream gradient is taken in the output's layout, the gradients come in their inputs'."""
         @staticmethod
-        def forward(ctx, Y, W1, W2, max_iters):
-            N, M = Y.shape
-            tape = torch.empty(int(require_device().proxtv_DR2L1W_TV_tape_bytes(M, N, max_iters)), dtype=torch.uint8, device=Y.device)
-            out = _drw_solve(Y, W1, W2, max_iters, tape)
+        def forward(ctx, Y, W1, W2, geom):
+            M, N, batch, _, max_iters = geom
+            nb = int(require_device().proxtv_DR2L1W_TV_batched_tape_bytes(M, N, batch, max_iters))
+            tape = torch.empty(nb, dtype=torch.uint8, device=Y.device)
+            out = _drw_solve(Y, W1, W2, geom, tape)
             ctx.save_for_backward(tape)
-            ctx.geom = (M, N, max_iters)
+            ctx.geom = geom
+            ctx.layouts = [(t.shape, t.stride(), t.dtype) for t in (out, W1, W2)]
             return out
 
         @staticmethod
         @once_differentiable
         def backward(ctx, gout):
             (tape,) = ctx.saved_tensors
-            M, N, max_iters = ctx.geom
+            M, N, batch, row_major, max_iters = ctx.geom
             need_y, need_w1, need_w2, _ = ctx.needs_input_grad
-            g = gout.contiguous()
-            gY = torch.empty((N, M), dtype=g.dtype, device=g.device)
-            gW1 = torch.empty((N, M - 1), dtype=g.dtype, device=g.device) if need_w1 else None
-            gW2 = torch.empty((N - 1, M), dtype=g.dtype, device=g.device) if need_w2 else None
-            _dev_call("DR2L1W_TV_vjp_dev", g, M, N, max_iters, tape, g, gY, gW1, gW2)
+
+            def like(i):
+                shape, stride, dt = ctx.layouts[i]
+                return torch.empty_strided(shape, stride, dtype=dt, device=tape.device)
+            g = like(0)                                   # the upstream gradient in the output's layout
+            g.copy_(gout)
+            gY = like(0)
+            gW1 = like(1) if need_w1 else None
+            gW2 = like(2) if need_w2 else None
+            _dev_call("DR2L1W_TV_batched_vjp_dev", g, M, N, batch, row_major, max_iters, tape, g, gY, gW1, gW2)
             return (gY if need_y else None), gW1, gW2, None
 
     class DR2(torch.autograd.Function):

@@ -132,17 +132,20 @@ int host_dr2(const char* fn, size_t M, size_t N, int batch, const T* Y, T W1, T 
     return 0;
 }
 
-// DR2L1W_TV with host (host_io) or device arrays.  W1: (M-1) x N, W2: M x (N-1), column-major like Y.
+// DR2L1W_TV with host (host_io) or device arrays: `batch` images back to back, column-major (row_major = 0) or C order (1); W1:
+// (M-1) x N, W2: M x (N-1) per image, laid out like Y (include/proxtv_b200.h).
 template <typename T>
-int run_drw(const char* fn, bool host_io, size_t M, size_t N, const T* Y, const T* W1, const T* W2, T* out, int maxit, double* info,
-            cudaStream_t st) {
+int run_drw(const char* fn, bool host_io, size_t M, size_t N, int batch, int row_major, const T* Y, const T* W1, const T* W2, T* out, int maxit,
+            double* info, cudaStream_t st) {
+    if (batch < 0) { fail(fn, "invalid shape (need batch >= 0)", info); return 0; }
     if (!have_device(fn, info)) return 0;
     WsGuard guard(st);
-    const size_t n = M * N, n1 = M ? (M - 1) * N : 0, n2 = N ? M * (N - 1) : 0;
+    const size_t n = M * N * (size_t)batch, n1 = M ? (M - 1) * N * (size_t)batch : 0, n2 = N ? M * (N - 1) * (size_t)batch : 0;
     if (n == 0) { if (info) { info[INFO_ITERS] = maxit <= 0 ? MAX_ITERS_DR : maxit; info[INFO_RC] = RC_OK; } return 0; }
-    void* ws = g_ws.get(ws_bytes_dr2<T>(M, N, 1));
+    if (!Y || !out || (n1 && !W1) || (n2 && !W2)) { fail(fn, "NULL array", info); return 0; }
+    void* ws = g_ws.get(ws_bytes_dr2<T>(M, N, batch));
     if (!ws) { fail(fn, "out of memory", info); return 0; }                             // TV2DWopt.cpp:78-79
-    if (!host_io) return drw_device<T>(M, N, Y, W1, W2, out, maxit, info, ws, (Engine)g_engine, st);
+    if (!host_io) return drw_device<T>(M, N, batch, row_major, Y, W1, W2, out, maxit, info, ws, (Engine)g_engine, st);
     char* d = (char*)g_io.get(2 * al(n * sizeof(T)) + al(n1 * sizeof(T) + 8) + al(n2 * sizeof(T) + 8));
     if (!d) { fail(fn, "out of memory", info); return 0; }
     T* dY = (T*)d; T* dout = (T*)(d + al(n * sizeof(T))); T* d1 = (T*)(d + 2 * al(n * sizeof(T))); T* d2 = (T*)((char*)d1 + al(n1 * sizeof(T) + 8));
@@ -151,7 +154,7 @@ int run_drw(const char* fn, bool host_io, size_t M, size_t N, const T* Y, const 
     if (n2 && !cuda_ok(fn, cudaMemcpyAsync(d2, W2, n2 * sizeof(T), cudaMemcpyHostToDevice, st), info)) return 0;
     double linfo[3] = {0, 0, RC_OK};
     double* pinfo = info ? info : linfo;
-    drw_device<T>(M, N, dY, d1, d2, dout, maxit, pinfo, ws, (Engine)g_engine, st);
+    drw_device<T>(M, N, batch, row_major, dY, d1, d2, dout, maxit, pinfo, ws, (Engine)g_engine, st);
     if (pinfo[INFO_RC] == RC_ERROR) { fail(fn, "device solver failed", info); return 0; }
     if (!cuda_ok(fn, cudaMemcpyAsync(out, dout, n * sizeof(T), cudaMemcpyDeviceToHost, st), info)) return 0;
     if (!cuda_ok(fn, cudaStreamSynchronize(st), info)) return 0;
@@ -281,30 +284,32 @@ static int dev_dr2_vjp(const char* fn, size_t M, size_t N, int batch, int row_ma
 }
 
 template <typename T>
-static int dev_drw_record(const char* fn, size_t M, size_t N, const T* Y, const T* W1, const T* W2, T* out, int maxit, void* tape,
-                          size_t tape_bytes, double* info, void* stream) {
-    if (M < 1 || N < 1) { fail(fn, "invalid shape (need M, N >= 1)", info); return 0; }
+static int dev_drw_record(const char* fn, size_t M, size_t N, int batch, int row_major, const T* Y, const T* W1, const T* W2, T* out, int maxit,
+                          void* tape, size_t tape_bytes, double* info, void* stream) {
+    if (M < 1 || N < 1 || batch < 1) { fail(fn, "invalid shape (need M, N, batch >= 1)", info); return 0; }
     if (!Y || !out || !tape || (M > 1 && !W1) || (N > 1 && !W2)) { fail(fn, "NULL array", info); return 0; }
-    if (tape_bytes < drw_tape_bytes(M, N, maxit)) { fail(fn, "tape_bytes smaller than proxtv_DR2L1W_TV_tape_bytes()", info); return 0; }
+    if (tape_bytes < drw_tape_bytes(M, N, batch, maxit)) { fail(fn, "tape_bytes smaller than proxtv_DR2L1W_TV_batched_tape_bytes()", info); return 0; }
     if (!have_device(fn, info)) return 0;
     WsGuard guard((cudaStream_t)stream);
-    void* ws = g_ws.get(ws_bytes_drw_record<T>(M, N));
+    void* ws = g_ws.get(ws_bytes_drw_record<T>(M, N, batch));
     if (!ws) { fail(fn, "out of memory", info); return 0; }
-    if (!cuda_ok(fn, drw_record_device<T>(M, N, Y, W1, W2, out, maxit, tape, ws, (Engine)g_engine, (cudaStream_t)stream), info)) return 0;
+    if (!cuda_ok(fn, drw_record_device<T>(M, N, batch, row_major, Y, W1, W2, out, maxit, tape, ws, (Engine)g_engine, (cudaStream_t)stream), info))
+        return 0;
     if (info) { info[INFO_ITERS] = maxit <= 0 ? MAX_ITERS_DR : maxit; info[INFO_RC] = RC_OK; }
     return 1;
 }
 
 template <typename T>
-static int dev_drw_vjp(const char* fn, size_t M, size_t N, int maxit, const void* tape, const T* gout, T* gY, T* gW1, T* gW2, void* stream) {
-    if (M < 1 || N < 1) { fail(fn, "invalid shape (need M, N >= 1)", nullptr); return 0; }
+static int dev_drw_vjp(const char* fn, size_t M, size_t N, int batch, int row_major, int maxit, const void* tape, const T* gout, T* gY, T* gW1,
+                       T* gW2, void* stream) {
+    if (M < 1 || N < 1 || batch < 1) { fail(fn, "invalid shape (need M, N, batch >= 1)", nullptr); return 0; }
     if (!tape || !gout || !gY) { fail(fn, "NULL array", nullptr); return 0; }
     if (!have_device(fn, nullptr)) return 0;
     WsGuard guard((cudaStream_t)stream);
-    if (const char* why = drw_tape_check(tape, sizeof(T), M, N, maxit, (cudaStream_t)stream)) { fail(fn, why, nullptr); return 0; }
-    void* ws = g_ws.get(ws_bytes_drw_vjp<T>(M, N));
+    if (const char* why = drw_tape_check(tape, sizeof(T), M, N, batch, row_major, maxit, (cudaStream_t)stream)) { fail(fn, why, nullptr); return 0; }
+    void* ws = g_ws.get(ws_bytes_drw_vjp<T>(M, N, batch));
     if (!ws) { fail(fn, "out of memory", nullptr); return 0; }
-    return cuda_ok(fn, drw_vjp_device<T>(M, N, maxit, tape, gout, gY, gW1, gW2, ws, (cudaStream_t)stream), nullptr);
+    return cuda_ok(fn, drw_vjp_device<T>(M, N, batch, row_major, maxit, tape, gout, gY, gW1, gW2, ws, (cudaStream_t)stream), nullptr);
 }
 
 // Arguments of the PDR_TV tape entry points: nullptr when valid, else the reason.
@@ -511,7 +516,7 @@ int DR2_TV(size_t M, size_t N, double* unary, double W1, double W2, double norm1
     return host_dr2<double>("DR2_TV", M, N, 1, unary, W1, W2, s, maxit, info);
 }
 int DR2L1W_TV(size_t M, size_t N, double* unary, double* W1, double* W2, double* s, int, int maxit, double* info) {
-    return run_drw<double>("DR2L1W_TV", true, M, N, unary, W1, W2, s, maxit, info, 0);
+    return run_drw<double>("DR2L1W_TV", true, M, N, 1, 0, unary, W1, W2, s, maxit, info, 0);
 }
 int PD2_TV(double* y, double* lambdas, double* norms, double* dims, double* x, double* info, int* ns, int nds, int npen, int,
            int maxIters) {
@@ -598,22 +603,49 @@ int proxtv_DR2_TV_batched_f32(size_t M, size_t N, int batch, const float* Y, flo
     return host_dr2<float>("proxtv_DR2_TV_batched_f32", M, N, batch, Y, W1, W2, out, maxit, info); }
 
 int proxtv_DR2L1W_TV_dev_f64(size_t M, size_t N, const double* Y, const double* W1, const double* W2, double* out, int maxit, double* info, void* stream) {
-    return run_drw<double>("proxtv_DR2L1W_TV_dev_f64", false, M, N, Y, W1, W2, out, maxit, info, (cudaStream_t)stream); }
+    return run_drw<double>("proxtv_DR2L1W_TV_dev_f64", false, M, N, 1, 0, Y, W1, W2, out, maxit, info, (cudaStream_t)stream); }
 int proxtv_DR2L1W_TV_dev_f32(size_t M, size_t N, const float* Y, const float* W1, const float* W2, float* out, int maxit, double* info, void* stream) {
-    return run_drw<float>("proxtv_DR2L1W_TV_dev_f32", false, M, N, Y, W1, W2, out, maxit, info, (cudaStream_t)stream); }
-size_t proxtv_DR2L1W_TV_tape_bytes(size_t M, size_t N, int maxit) { return drw_tape_bytes(M, N, maxit); }
+    return run_drw<float>("proxtv_DR2L1W_TV_dev_f32", false, M, N, 1, 0, Y, W1, W2, out, maxit, info, (cudaStream_t)stream); }
+size_t proxtv_DR2L1W_TV_tape_bytes(size_t M, size_t N, int maxit) { return drw_tape_bytes(M, N, 1, maxit); }
 int proxtv_DR2L1W_TV_record_dev_f64(size_t M, size_t N, const double* Y, const double* W1, const double* W2, double* out, int maxit, void* tape,
                                     size_t tape_bytes, double* info, void* stream) {
-    return dev_drw_record<double>("proxtv_DR2L1W_TV_record_dev_f64", M, N, Y, W1, W2, out, maxit, tape, tape_bytes, info, stream); }
+    return dev_drw_record<double>("proxtv_DR2L1W_TV_record_dev_f64", M, N, 1, 0, Y, W1, W2, out, maxit, tape, tape_bytes, info, stream); }
 int proxtv_DR2L1W_TV_record_dev_f32(size_t M, size_t N, const float* Y, const float* W1, const float* W2, float* out, int maxit, void* tape,
                                     size_t tape_bytes, double* info, void* stream) {
-    return dev_drw_record<float>("proxtv_DR2L1W_TV_record_dev_f32", M, N, Y, W1, W2, out, maxit, tape, tape_bytes, info, stream); }
+    return dev_drw_record<float>("proxtv_DR2L1W_TV_record_dev_f32", M, N, 1, 0, Y, W1, W2, out, maxit, tape, tape_bytes, info, stream); }
 int proxtv_DR2L1W_TV_vjp_dev_f64(size_t M, size_t N, int maxit, const void* tape, const double* gout, double* gY, double* gW1, double* gW2,
                                  void* stream) {
-    return dev_drw_vjp<double>("proxtv_DR2L1W_TV_vjp_dev_f64", M, N, maxit, tape, gout, gY, gW1, gW2, stream); }
+    return dev_drw_vjp<double>("proxtv_DR2L1W_TV_vjp_dev_f64", M, N, 1, 0, maxit, tape, gout, gY, gW1, gW2, stream); }
 int proxtv_DR2L1W_TV_vjp_dev_f32(size_t M, size_t N, int maxit, const void* tape, const float* gout, float* gY, float* gW1, float* gW2,
                                  void* stream) {
-    return dev_drw_vjp<float>("proxtv_DR2L1W_TV_vjp_dev_f32", M, N, maxit, tape, gout, gY, gW1, gW2, stream); }
+    return dev_drw_vjp<float>("proxtv_DR2L1W_TV_vjp_dev_f32", M, N, 1, 0, maxit, tape, gout, gY, gW1, gW2, stream); }
+size_t proxtv_DR2L1W_TV_batched_tape_bytes(size_t M, size_t N, int batch, int maxit) { return batch < 1 ? 0 : drw_tape_bytes(M, N, batch, maxit); }
+int proxtv_DR2L1W_TV_batched_dev_f64(size_t M, size_t N, int batch, int row_major, const double* Y, const double* W1, const double* W2, double* out,
+                                     int maxit, double* info, void* stream) {
+    return run_drw<double>("proxtv_DR2L1W_TV_batched_dev_f64", false, M, N, batch, row_major, Y, W1, W2, out, maxit, info, (cudaStream_t)stream); }
+int proxtv_DR2L1W_TV_batched_dev_f32(size_t M, size_t N, int batch, int row_major, const float* Y, const float* W1, const float* W2, float* out,
+                                     int maxit, double* info, void* stream) {
+    return run_drw<float>("proxtv_DR2L1W_TV_batched_dev_f32", false, M, N, batch, row_major, Y, W1, W2, out, maxit, info, (cudaStream_t)stream); }
+int proxtv_DR2L1W_TV_batched_record_dev_f64(size_t M, size_t N, int batch, int row_major, const double* Y, const double* W1, const double* W2,
+                                            double* out, int maxit, void* tape, size_t tape_bytes, double* info, void* stream) {
+    return dev_drw_record<double>("proxtv_DR2L1W_TV_batched_record_dev_f64", M, N, batch, row_major, Y, W1, W2, out, maxit, tape, tape_bytes, info,
+                                  stream); }
+int proxtv_DR2L1W_TV_batched_record_dev_f32(size_t M, size_t N, int batch, int row_major, const float* Y, const float* W1, const float* W2,
+                                            float* out, int maxit, void* tape, size_t tape_bytes, double* info, void* stream) {
+    return dev_drw_record<float>("proxtv_DR2L1W_TV_batched_record_dev_f32", M, N, batch, row_major, Y, W1, W2, out, maxit, tape, tape_bytes, info,
+                                 stream); }
+int proxtv_DR2L1W_TV_batched_vjp_dev_f64(size_t M, size_t N, int batch, int row_major, int maxit, const void* tape, const double* gout, double* gY,
+                                         double* gW1, double* gW2, void* stream) {
+    return dev_drw_vjp<double>("proxtv_DR2L1W_TV_batched_vjp_dev_f64", M, N, batch, row_major, maxit, tape, gout, gY, gW1, gW2, stream); }
+int proxtv_DR2L1W_TV_batched_vjp_dev_f32(size_t M, size_t N, int batch, int row_major, int maxit, const void* tape, const float* gout, float* gY,
+                                         float* gW1, float* gW2, void* stream) {
+    return dev_drw_vjp<float>("proxtv_DR2L1W_TV_batched_vjp_dev_f32", M, N, batch, row_major, maxit, tape, gout, gY, gW1, gW2, stream); }
+int proxtv_DR2L1W_TV_batched_f64(size_t M, size_t N, int batch, int row_major, const double* Y, const double* W1, const double* W2, double* out,
+                                 int maxit, double* info) {
+    return run_drw<double>("proxtv_DR2L1W_TV_batched_f64", true, M, N, batch, row_major, Y, W1, W2, out, maxit, info, 0); }
+int proxtv_DR2L1W_TV_batched_f32(size_t M, size_t N, int batch, int row_major, const float* Y, const float* W1, const float* W2, float* out,
+                                 int maxit, double* info) {
+    return run_drw<float>("proxtv_DR2L1W_TV_batched_f32", true, M, N, batch, row_major, Y, W1, W2, out, maxit, info, 0); }
 
 int proxtv_PD2_TV_dev_f64(const double* y, double* lambdas, double* dims, double* x, double* info, int* ns, int nds, int npen, int maxIters, void* stream) {
     return run_pd<double>("proxtv_PD2_TV_dev_f64", 0, false, y, lambdas, nullptr, dims, x, info, ns, nds, npen, maxIters, (cudaStream_t)stream); }

@@ -307,52 +307,48 @@ cudaError_t dr2_vjp_device(size_t M, size_t N, int batch, int row_major, int max
 }
 
 // ================================================================ DR2L1W_TV (DESIGN.md section 12)
-// drw_device's iteration (solver.cu) on one column-major M x N image, column prox P_c (fibers (N, M, 1), weights W1 (M-1) x N),
-// row prox P_r (fibers (M, N, M), weights W2 M x (N-1)), in its own association (chunk_core.cuh: apply_out, apply_out_any):
+// drw_device's iteration (solver.cu) on `batch` M x N images in either storage order, column prox P_c (fibers of length M, weights W1
+// (M-1) x N per image), row prox P_r (length N, weights W2 M x (N-1)), per image, in its own association (chunk_core.cuh: apply_out,
+// apply_out_any):
 //     t = 2 mean(Y)
 //     k = 0..K-1: x1 = P_c(t) ; s = 2 (t - x1) - t ; u = Y - s ; x2 = P_r(u) ; tw = (u - x2) - Y ; t = 0.5 (t + (-2 tw - s))
 //     final:      x1 = P_c(t) ; s = t - x1 ; u = Y - s ; x2 = P_r(u) ; tw = (u - x2) - Y ; out = -s - tw
 // In real arithmetic t' = t - x1 + x2 and out = x2: section 11's recurrence, so the backward is dr2_vjp_device's with every pass
 // recorded.  Tape: the 256-byte header (own magic) and 2K + 2 passes -- p = 2k / 2k + 1: column / row pass of iteration k (k = K: the
-// final pair) -- the column pass of k = 0 included (the prox of a constant image, whose Jacobian depends on which weights are zero).
-// Row tapes are taken from x2 itself: out is x2 only in real arithmetic.
+// final pair) -- the column pass of k = 0 included (the prox of a constant image, whose Jacobian depends on which weights are zero) --
+// each a pair of bitsets over all batch M N elements in storage order.  Row tapes are taken from x2 itself: out is x2 only in real
+// arithmetic.  The start value term sums g per image (img_sums); the weight gradients need no sum across images.
 // Weight gradients: per edge, acc = 0.0 ; acc = acc + sign * (double)gw_p over the passes in backward order (p = 2K + 1 .. 0), gW = (T)acc,
 // gw_p the pass's VJP edge gradient (laid out like W1 / W2) for its upstream gradient: G and a for the final pair, g for the row passes
 // and -h for the column passes of the loop (computed for +h, so sign -1).
 static constexpr uint64_t DRW_TAPE_MAGIC = 0x31504154574c5244ull;          // "DRLWTAP1"
 
-template <typename T> cudaError_t gather_fibers(const T* A, const T* B, InOp op, T* out, FiberGeom g, cudaStream_t st);
-template <typename T>
-cudaError_t scatter_fibers_sparse(const T* in, const uint32_t* Mk, const T* Cv, const T* A, const T* B, const T* C, InOp op, int out_op, T* X,
-                                  FiberGeom g, cudaStream_t st);
-template <typename T>
-cudaError_t prox_fibers_chunked_contig_sparse(const T* A, T* X, FiberGeom g, T lam, const T* lamv, uint32_t* Mk, T* Cv, cudaStream_t st);
-
-size_t drw_tape_bytes(size_t M, size_t N, int maxit) {
+size_t drw_tape_bytes(size_t M, size_t N, int batch, int maxit) {
     const int K = maxit <= 0 ? MAX_ITERS_DR : maxit;
-    return 256 + (size_t)(2 * K + 2) * 2 * ptvv::vjp_tape_set_bytes((long long)(M * N));
+    return 256 + (size_t)(2 * K + 2) * 2 * ptvv::vjp_tape_set_bytes((long long)(M * N * (size_t)batch));
 }
-template <typename T> size_t ws_bytes_drw_record(size_t M, size_t N) {
-    return 8 * al256(M * N * sizeof(T)) + DR2V_SCRATCH;      // t, s, u, x + the row route's staging: t1, t2, gathered W2, sparse results
+template <typename T> size_t ws_bytes_drw_record(size_t M, size_t N, int batch) {
+    return 8 * al256(M * N * (size_t)batch * sizeof(T)) + DR2V_SCRATCH;   // t, s, u, x + DrwPasses' staging: t1, t2, gathered weights, sparse results
 }
-template <typename T> size_t ws_bytes_drw_vjp(size_t M, size_t N) {
-    const long long n = (long long)(M * N);
-    const size_t s1 = ptvv::vjp_scratch_bytes((long long)N, (int)M), s2 = ptvv::vjp_scratch_bytes((long long)M, (int)N);
-    return 5 * al256((size_t)n * sizeof(T)) + 2 * al256((size_t)n * sizeof(double)) + al256(s1 > s2 ? s1 : s2) + DR2V_SCRATCH + al256(sizeof(double));
+template <typename T> size_t ws_bytes_drw_vjp(size_t M, size_t N, int batch) {
+    const long long n = (long long)(M * N * (size_t)batch);
+    const size_t s1 = ptvv::vjp_scratch_bytes((long long)N * batch, (int)M), s2 = ptvv::vjp_scratch_bytes((long long)M * batch, (int)N);
+    return 5 * al256((size_t)n * sizeof(T)) + 2 * al256((size_t)n * sizeof(double)) + al256(s1 > s2 ? s1 : s2) + DR2V_SCRATCH +
+           al256((size_t)batch * sizeof(double));
 }
 
-// Column pass: s = 2 (t - x1) - t (FINAL: s = t - x1) ; u = Y - s ; tape of x1 over the columns (contiguous, length M) with W1
+// Column pass: s = 2 (t - x1) - t (FINAL: s = t - x1) ; u = Y - s ; tape of x1 over the columns (length len, stride inc) with W1
 template <typename T, bool FINAL>
 __global__ void k_recw_cols(const T* __restrict__ x1, const T* __restrict__ t, const T* __restrict__ Y, const T* __restrict__ W1,
-                            T* __restrict__ s, T* __restrict__ u, long long n, int len, uint32_t* __restrict__ F, uint32_t* __restrict__ U,
-                            long long nwords) {
+                            T* __restrict__ s, T* __restrict__ u, long long n, int len, long long inc, uint32_t* __restrict__ F,
+                            uint32_t* __restrict__ U, long long nwords) {
     const int lane = threadIdx.x & 31;
     const long long w0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5, ws = ((long long)gridDim.x * blockDim.x) >> 5;
     for (long long q = w0; q < nwords; q += ws) {
         const long long i = q * 32 + lane;
         uint32_t f = 0, uu = 0;
         if (i < n) {
-            ptvv::vjp_tape_edge<T>(x1, i, len, 1, 0.0, W1, f, uu);
+            ptvv::vjp_tape_edge<T>(x1, i, len, inc, 0.0, W1, f, uu);
             const T tv = t[i];
             const T d = tv - x1[i];
             const T sv = FINAL ? d : T(2) * d - tv;
@@ -387,9 +383,9 @@ __global__ void k_recw_rows(const T* __restrict__ x2, const T* __restrict__ u, c
 }
 
 template <typename T>
-cudaError_t drw_record_device(size_t M, size_t N, const T* Y, const T* W1, const T* W2, T* out, int maxit, void* tape, void* ws, Engine eng,
-                              cudaStream_t st) {
-    const long long n = (long long)(M * N);
+cudaError_t drw_record_device(size_t M, size_t N, int batch, int row_major, const T* Y, const T* W1, const T* W2, T* out, int maxit, void* tape,
+                              void* ws, Engine eng, cudaStream_t st) {
+    const long long n = (long long)(M * N * (size_t)batch);
     const int K = maxit <= 0 ? MAX_ITERS_DR : maxit;
     const size_t ab = al256((size_t)n * sizeof(T)), sb = ptvv::vjp_tape_set_bytes(n);
     char* w = (char*)ws;
@@ -397,15 +393,9 @@ cudaError_t drw_record_device(size_t M, size_t N, const T* Y, const T* W1, const
     T* s = (T*)w; w += ab;
     T* u = (T*)w; w += ab;
     T* x = (T*)w; w += ab;
-    T* t1 = (T*)w; w += ab;
-    T* t2 = (T*)w; w += ab;
-    T* w2t = (T*)w; w += ab;
-    T* Cv = (T*)w; uint32_t* Mk = reinterpret_cast<uint32_t*>(Cv + (long long)M * (((long long)N + 31) / 32));   // sparse row results
-    w += ab;
+    DrwPasses<T> P;                                  // the pass routes of drw_device; the gathered weights are written first, below
+    void* stage = w; w += 4 * ab;
     double* scratch = (double*)w;
-    const FiberGeom gc{(long long)N, (int)M, 1}, gr{(long long)M, (int)N, (long long)M}, grc{(long long)M, (int)N, 1};
-    const T* W1p = M > 1 ? W1 : nullptr;
-    const T* W2p = N > 1 ? W2 : nullptr;
     auto Fp = [&](int p) { return (uint32_t*)((char*)tape + 256 + (size_t)p * 2 * sb); };
     auto Up = [&](int p) { return (uint32_t*)((char*)tape + 256 + (size_t)p * 2 * sb + sb); };
     const long long nwords = (long long)(sb / 4);
@@ -413,46 +403,30 @@ cudaError_t drw_record_device(size_t M, size_t N, const T* Y, const T* W1, const
 #define RTRY(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) return e__; } while (0)
     Dr2TapeHeader h;
     memset(&h, 0, sizeof(h));
-    h.magic = DRW_TAPE_MAGIC; h.elem = (int64_t)sizeof(T); h.M = (int64_t)M; h.N = (int64_t)N; h.batch = 1; h.K = K;
+    h.magic = DRW_TAPE_MAGIC; h.elem = (int64_t)sizeof(T); h.M = (int64_t)M; h.N = (int64_t)N; h.batch = batch; h.row_major = row_major ? 1 : 0;
+    h.K = K;
     RTRY(cudaMemcpyAsync(tape, &h, sizeof(h), cudaMemcpyHostToDevice, st));
-    // the row route of drw_device: gather -> contiguous weighted chunked kernel (sparse result) -> scatter, else the sequential kernel
-    bool fast_rows = eng != ENGINE_SEQ && N >= 64;
-    if (fast_rows) { KernelSpan sp(KC_ELEMENTWISE, 1, st);
-                     RTRY(gather_fibers<T>(W2, nullptr, IN_A, w2t, FiberGeom{(long long)M, (int)N - 1, (long long)M}, st)); }
-    RTRY(ew_image_means_x2<T>(Y, n, 1, t, scratch, st));
+    RTRY(P.init(M, N, batch, row_major, W1, W2, eng, stage, st));
+    const FiberGeom gc = P.g[0], gr = P.g[1];
+    RTRY(ew_image_means_x2<T>(Y, (long long)(M * N), batch, t, scratch, st));
     for (int k = 0; k <= K; k++) {
         const bool final = k == K;
-        RTRY(prox_fibers_ex<T>(t, nullptr, nullptr, IN_A, x, 0 /*OUT_X*/, gc, T(0), W1p, eng, nullptr, st, 0));
+        RTRY(P.run(0, t, nullptr, nullptr, IN_A, x, 0 /*OUT_X*/, st));
         { KernelSpan sp(KC_ELEMENTWISE, 1, st);
-          if (final) k_recw_cols<T, true><<<gw, 256, 0, st>>>(x, t, Y, W1p, s, u, n, gc.len, Fp(2 * k), Up(2 * k), nwords);
-          else k_recw_cols<T, false><<<gw, 256, 0, st>>>(x, t, Y, W1p, s, u, n, gc.len, Fp(2 * k), Up(2 * k), nwords);
+          if (final) k_recw_cols<T, true><<<gw, 256, 0, st>>>(x, t, Y, P.W[0], s, u, n, gc.len, gc.inc, Fp(2 * k), Up(2 * k), nwords);
+          else k_recw_cols<T, false><<<gw, 256, 0, st>>>(x, t, Y, P.W[0], s, u, n, gc.len, gc.inc, Fp(2 * k), Up(2 * k), nwords);
           RTRY(cudaGetLastError()); }
-        bool done = false;
-        if (fast_rows) {
-            { KernelSpan sp(KC_ELEMENTWISE, 1, st); RTRY(gather_fibers<T>(Y, s, IN_A_MINUS_B, t1, gr, st)); }
-            cudaError_t e;
-            { KernelSpan sp(KC_PROX_STRIDED, 1, st);
-              e = prox_fibers_chunked_contig_sparse<T>(t1, t2, grc, T(0), w2t, Mk, Cv, st);
-              if (e == cudaErrorInvalidConfiguration) sp.cancel(); }
-            if (e == cudaErrorInvalidConfiguration) { cudaGetLastError(); fast_rows = false; }
-            else {
-                RTRY(e);
-                KernelSpan sp(KC_ELEMENTWISE, 1, st);
-                RTRY(scatter_fibers_sparse<T>(t2, Mk, Cv, nullptr, nullptr, nullptr, IN_A, 0 /*OUT_X*/, x, gr, st));
-                done = true;
-            }
-        }
-        if (!done) RTRY(prox_fibers_ex<T>(u, nullptr, nullptr, IN_A, x, 0 /*OUT_X*/, gr, T(0), W2p, ENGINE_SEQ, nullptr, st, 0));
+        RTRY(P.run(1, u, nullptr, nullptr, IN_A, x, 0 /*OUT_X*/, st));
         { KernelSpan sp(KC_ELEMENTWISE, 1, st);
-          if (final) k_recw_rows<T, true><<<gw, 256, 0, st>>>(x, u, Y, s, t, out, W2p, n, gr.len, gr.inc, Fp(2 * k + 1), Up(2 * k + 1), nwords);
-          else k_recw_rows<T, false><<<gw, 256, 0, st>>>(x, u, Y, s, t, t, W2p, n, gr.len, gr.inc, Fp(2 * k + 1), Up(2 * k + 1), nwords);
+          if (final) k_recw_rows<T, true><<<gw, 256, 0, st>>>(x, u, Y, s, t, out, P.W[1], n, gr.len, gr.inc, Fp(2 * k + 1), Up(2 * k + 1), nwords);
+          else k_recw_rows<T, false><<<gw, 256, 0, st>>>(x, u, Y, s, t, t, P.W[1], n, gr.len, gr.inc, Fp(2 * k + 1), Up(2 * k + 1), nwords);
           RTRY(cudaGetLastError()); }
     }
     return cudaSuccess;
 }
 
-const char* drw_tape_check(const void* tape, size_t elem, size_t M, size_t N, int maxit, cudaStream_t st) {
-    return tape_check(DRW_TAPE_MAGIC, "not a DR2L1W_TV tape", tape, elem, M, N, 1, 0, maxit, st);
+const char* drw_tape_check(const void* tape, size_t elem, size_t M, size_t N, int batch, int row_major, int maxit, cudaStream_t st) {
+    return tape_check(DRW_TAPE_MAGIC, "not a DR2L1W_TV tape", tape, elem, M, N, batch, row_major, maxit, st);
 }
 
 template <typename T> __global__ void k_acc(double* __restrict__ acc, const T* __restrict__ gw, long long n, double sign) {
@@ -463,12 +437,13 @@ template <typename T> __global__ void k_round(const double* __restrict__ acc, T*
 }
 
 template <typename T>
-cudaError_t drw_vjp_device(size_t M, size_t N, int maxit, const void* tape, const T* gout, T* gY, T* gW1, T* gW2, void* ws, cudaStream_t st) {
-    const long long n = (long long)(M * N);
-    const long long e1 = (long long)(M - 1) * (long long)N, e2 = (long long)M * (long long)(N - 1);     // edges of W1 / W2
+cudaError_t drw_vjp_device(size_t M, size_t N, int batch, int row_major, int maxit, const void* tape, const T* gout, T* gY, T* gW1, T* gW2,
+                           void* ws, cudaStream_t st) {
+    const long long per = (long long)(M * N), n = per * batch;
+    const long long e1 = (long long)(M - 1) * (long long)N * batch, e2 = (long long)M * (long long)(N - 1) * batch;   // edges of W1 / W2
     const int K = maxit <= 0 ? MAX_ITERS_DR : maxit;
     const size_t ab = al256((size_t)n * sizeof(T)), db = al256((size_t)n * sizeof(double)), sb = ptvv::vjp_tape_set_bytes(n);
-    const size_t s1 = ptvv::vjp_scratch_bytes((long long)N, (int)M), s2 = ptvv::vjp_scratch_bytes((long long)M, (int)N);
+    const size_t s1 = ptvv::vjp_scratch_bytes((long long)N * batch, (int)M), s2 = ptvv::vjp_scratch_bytes((long long)M * batch, (int)N);
     char* w = (char*)ws;
     T* g = (T*)w; w += ab;
     T* a = (T*)w; w += ab;
@@ -480,7 +455,8 @@ cudaError_t drw_vjp_device(size_t M, size_t N, int maxit, const void* tape, cons
     void* vscr = w; w += al256(s1 > s2 ? s1 : s2);
     double* scratch = (double*)w; w += DR2V_SCRATCH;
     double* sums = (double*)w;
-    const FiberGeom gc{(long long)N, (int)M, 1}, gr{(long long)M, (int)N, (long long)M};
+    FiberGeom gc, gr;
+    dr2_geoms(M, N, batch, row_major, gc, gr);
     const bool want1 = gW1 && e1 > 0, want2 = gW2 && e2 > 0;
     const char* tb = (const char*)tape + 256;
     auto Fp = [&](int p) { return (const uint32_t*)(tb + (size_t)p * 2 * sb); };
@@ -511,8 +487,8 @@ cudaError_t drw_vjp_device(size_t M, size_t N, int maxit, const void* tape, cons
         RTRY(vjp(2 * k, h, sc, -1.0));                     // upstream of the column prox: -h
         { KernelSpan sp(KC_ELEMENTWISE, 1, st); k_b_mid2<T><<<ge, 256, 0, st>>>(a, h, sc, g, n); RTRY(cudaGetLastError()); }
     }
-    RTRY(img_sums<T>(g, n, 1, scratch, sums, nullptr, 0, 0.0, st));
-    { KernelSpan sp(KC_ELEMENTWISE, 1, st); k_b_start<T><<<ge, 256, 0, st>>>(gY, sums, n, n); RTRY(cudaGetLastError()); }
+    RTRY(img_sums<T>(g, per, batch, scratch, sums, nullptr, 0, 0.0, st));
+    { KernelSpan sp(KC_ELEMENTWISE, 1, st); k_b_start<T><<<ge, 256, 0, st>>>(gY, sums, per, n); RTRY(cudaGetLastError()); }
     if (want1) { KernelSpan sp(KC_ELEMENTWISE, 1, st); k_round<T><<<ew_grid(e1), 256, 0, st>>>(acc1, gW1, e1); RTRY(cudaGetLastError()); }
     if (want2) { KernelSpan sp(KC_ELEMENTWISE, 1, st); k_round<T><<<ew_grid(e2), 256, 0, st>>>(acc2, gW2, e2); RTRY(cudaGetLastError()); }
     return cudaSuccess;
@@ -860,10 +836,10 @@ cudaError_t pd_vjp_device(bool pd2, const int* ns, int nds, int npen, const doub
     template size_t ws_bytes_dr2_vjp<T>(size_t, size_t, int); \
     template cudaError_t dr2_record_device<T>(size_t, size_t, int, int, const T*, T, T, T*, int, void*, void*, Engine, cudaStream_t); \
     template cudaError_t dr2_vjp_device<T>(size_t, size_t, int, int, int, const void*, const T*, T*, double*, void*, cudaStream_t); \
-    template size_t ws_bytes_drw_record<T>(size_t, size_t); \
-    template size_t ws_bytes_drw_vjp<T>(size_t, size_t); \
-    template cudaError_t drw_record_device<T>(size_t, size_t, const T*, const T*, const T*, T*, int, void*, void*, Engine, cudaStream_t); \
-    template cudaError_t drw_vjp_device<T>(size_t, size_t, int, const void*, const T*, T*, T*, T*, void*, cudaStream_t);
+    template size_t ws_bytes_drw_record<T>(size_t, size_t, int); \
+    template size_t ws_bytes_drw_vjp<T>(size_t, size_t, int); \
+    template cudaError_t drw_record_device<T>(size_t, size_t, int, int, const T*, const T*, const T*, T*, int, void*, void*, Engine, cudaStream_t); \
+    template cudaError_t drw_vjp_device<T>(size_t, size_t, int, int, int, const void*, const T*, T*, T*, T*, void*, cudaStream_t);
 INST(double)
 INST(float)
 

@@ -329,14 +329,17 @@ cudaError_t prox_fibers_chunked_contig(const T* A, const T* B, const T* C, InOp 
                                        const T* lamv, cudaStream_t st, T* X2, long long inc2) {
     return launch_chunked_contig<T>(A, B, C, op, X, out_op, g, lam, lamv, st, X2, inc2, nullptr, nullptr);
 }
-// Plain prox (OUT_X) with a SPARSE result: X only holds each segment's value at its start; Mk[fiber][chunk] = start mask,
+// Plain prox (OUT_X) of A (op) B with a SPARSE result: X only holds each segment's value at its start; Mk[fiber][chunk] = start mask,
 // Cv[fiber][chunk] = value entering the chunk (chunks of 32 samples, (len + 31) / 32 per fiber).  See scatter_fibers_ex_sparse.
 template <typename T>
-cudaError_t prox_fibers_chunked_contig_sparse(const T* A, T* X, FiberGeom g, T lam, const T* lamv, uint32_t* Mk, T* Cv, cudaStream_t st) {
-    return launch_chunked_contig<T>(A, nullptr, nullptr, IN_A, X, OUT_X, g, lam, lamv, st, nullptr, 0, Mk, Cv);
+cudaError_t prox_fibers_chunked_contig_sparse(const T* A, const T* B, InOp op, T* X, FiberGeom g, T lam, const T* lamv, uint32_t* Mk, T* Cv,
+                                              cudaStream_t st) {
+    return launch_chunked_contig<T>(A, B, nullptr, op, X, OUT_X, g, lam, lamv, st, nullptr, 0, Mk, Cv);
 }
-template cudaError_t prox_fibers_chunked_contig_sparse<double>(const double*, double*, FiberGeom, double, const double*, uint32_t*, double*, cudaStream_t);
-template cudaError_t prox_fibers_chunked_contig_sparse<float>(const float*, float*, FiberGeom, float, const float*, uint32_t*, float*, cudaStream_t);
+template cudaError_t prox_fibers_chunked_contig_sparse<double>(const double*, const double*, InOp, double*, FiberGeom, double, const double*, uint32_t*,
+                                                               double*, cudaStream_t);
+template cudaError_t prox_fibers_chunked_contig_sparse<float>(const float*, const float*, InOp, float*, FiberGeom, float, const float*, uint32_t*, float*,
+                                                              cudaStream_t);
 
 template cudaError_t prox_fibers_chunked_contig<double>(const double*, const double*, const double*, InOp, double*, int, FiberGeom,
                                                         double, const double*, cudaStream_t, double*, long long);

@@ -27,7 +27,8 @@ template <typename T> cudaError_t scatter_fibers(const T* in, T* X, FiberGeom g,
 template <typename T>
 cudaError_t scatter_fibers_ex(const T* in, const T* A, const T* B, const T* C, InOp op, int out_op, T* X, FiberGeom g, cudaStream_t st);
 template <typename T>
-cudaError_t prox_fibers_chunked_contig_sparse(const T* A, T* X, FiberGeom g, T lam, const T* lamv, uint32_t* Mk, T* Cv, cudaStream_t st);
+cudaError_t prox_fibers_chunked_contig_sparse(const T* A, const T* B, InOp op, T* X, FiberGeom g, T lam, const T* lamv, uint32_t* Mk, T* Cv,
+                                              cudaStream_t st);
 template <typename T>
 cudaError_t scatter_fibers_sparse(const T* in, const uint32_t* Mk, const T* Cv, const T* A, const T* B, const T* C, InOp op, int out_op, T* X,
                                   FiberGeom g, cudaStream_t st);
@@ -104,7 +105,7 @@ cudaError_t prox_fibers_ex(const T* A, const T* B, const T* C, InOp op, T* X, in
                 const long long lpf = ((long long)g.len + 31) / 32;
                 T* Cv = scratch + 2 * n; uint32_t* Mk = reinterpret_cast<uint32_t*>(Cv + g.nf * lpf);
                 { KernelSpan span(KC_PROX_STRIDED, 1, st);
-                  e = sparse ? prox_fibers_chunked_contig_sparse<T>(t1, t2, gc, lam, nullptr, Mk, Cv, st)
+                  e = sparse ? prox_fibers_chunked_contig_sparse<T>(t1, nullptr, IN_A, t2, gc, lam, nullptr, Mk, Cv, st)
                              : prox_fibers_chunked_contig<T>(t1, nullptr, nullptr, IN_A, t2, OUT_X, gc, lam, nullptr, st);
                   if (e == cudaErrorInvalidConfiguration) span.cancel(); }
                 if (e == cudaSuccess) {

@@ -96,9 +96,26 @@ constexpr int REDUCE_BLOCKS = 1184;    // fixed, not the device's SM count (~9 p
 template <typename T> size_t ws_bytes_dr2(size_t M, size_t N, int batch);
 template <typename T> int dr2_device(size_t M, size_t N, int batch, int row_major, const T* Y, T w1, T w2, T* out, int maxit, double* info,
                                      void* ws, Engine eng, cudaStream_t st);
-// DR2L1W_TV on one M x N column-major image; W1: (M-1) x N, W2: M x (N-1) column-major; workspace of ws_bytes_dr2(M, N, 1) bytes
-template <typename T> int drw_device(size_t M, size_t N, const T* Y, const T* W1, const T* W2, T* out, int maxit, double* info, void* ws,
-                                     Engine eng, cudaStream_t st);
+// DR2L1W_TV on `batch` M x N images back to back, column-major (row_major = 0) or C order (1); W1: (M-1) x N, W2: M x (N-1) per image,
+// back to back, each laid out by the fiber rule of its pass (len - 1 samples per fiber); workspace of ws_bytes_dr2(M, N, batch) bytes
+template <typename T> int drw_device(size_t M, size_t N, int batch, int row_major, const T* Y, const T* W1, const T* W2, T* out, int maxit,
+                                     double* info, void* ws, Engine eng, cudaStream_t st);
+// The prox passes of the weighted solve, shared by drw_device and drw_record_device (solver.cu).  axis 0: the column pass (fibers of
+// length M, weights W1), axis 1: the row pass (length N, W2).  The strided axis of the storage order: gather (input op fused) ->
+// contiguous weighted chunked kernel with a sparse result -> scatter (output form fused while it expands); the other: the chunked kernel with its fill, or
+// for the weighted Douglas-Rachford forms the sparse result and expand_fibers_sparse (transpose.cu).  ENGINE_SEQ, fibers shorter than
+// 64 and a refused chunked launch: the sequential kernel.  The strided pass's weights are gathered once, by init().
+template <typename T> struct DrwPasses {
+    FiberGeom g[2];
+    const T* W[2];
+    Engine eng;
+    int strided;                 // the axis that takes the gather route: 1 (rows) for column-major images, 0 (columns) for C order
+    bool fast[2];
+    T *t1, *t2, *wg, *Cv; uint32_t* Mk;
+    // stage: 4 arrays of M N batch elements (align256 each)
+    cudaError_t init(size_t M, size_t N, int batch, int row_major, const T* W1, const T* W2, Engine eng, void* stage, cudaStream_t st);
+    cudaError_t run(int axis, const T* A, const T* B, const T* C, InOp op, T* X, int out_op, cudaStream_t st);
+};
 template <typename T> size_t ws_bytes_pd(long long n, int npen);
 // PD2_TV / PD_TV (proximal Dykstra, stop rule mean|x - x_old| <= STOP_PD).  tape: nullptr, or the recorded forward's buffer (header
 // written by the caller after the call, from info[0]): the segmentation tape of every pass
@@ -133,17 +150,17 @@ const char* dr2_tape_check(const void* tape, size_t elem, size_t M, size_t N, in
 template <typename T> cudaError_t dr2_vjp_device(size_t M, size_t N, int batch, int row_major, int maxit, const void* tape, const T* gout,
                                                  T* gY, double* glam, void* ws, cudaStream_t st);
 // ---- exact backward pass of DR2L1W_TV (dr2_vjp.cu, DESIGN.md section 12) ----
-size_t drw_tape_bytes(size_t M, size_t N, int maxit);                    // header + (2K + 2) passes x two bitsets
-template <typename T> size_t ws_bytes_drw_record(size_t M, size_t N);
-template <typename T> size_t ws_bytes_drw_vjp(size_t M, size_t N);
+size_t drw_tape_bytes(size_t M, size_t N, int batch, int maxit);         // header + (2K + 2) passes x two bitsets
+template <typename T> size_t ws_bytes_drw_record(size_t M, size_t N, int batch);
+template <typename T> size_t ws_bytes_drw_vjp(size_t M, size_t N, int batch);
 // drw_device's iteration with plain prox passes (bit for bit the same output), writing the segmentation tape of every pass.  The
 // tape's size (drw_tape_bytes) and the arguments are checked by the caller.
-template <typename T> cudaError_t drw_record_device(size_t M, size_t N, const T* Y, const T* W1, const T* W2, T* out, int maxit, void* tape,
-                                                    void* ws, Engine eng, cudaStream_t st);
-const char* drw_tape_check(const void* tape, size_t elem, size_t M, size_t N, int maxit, cudaStream_t st);
+template <typename T> cudaError_t drw_record_device(size_t M, size_t N, int batch, int row_major, const T* Y, const T* W1, const T* W2, T* out,
+                                                    int maxit, void* tape, void* ws, Engine eng, cudaStream_t st);
+const char* drw_tape_check(const void* tape, size_t elem, size_t M, size_t N, int batch, int row_major, int maxit, cudaStream_t st);
 // gY, and per-edge gW1 / gW2 unless nullptr, from the tape alone
-template <typename T> cudaError_t drw_vjp_device(size_t M, size_t N, int maxit, const void* tape, const T* gout, T* gY, T* gW1, T* gW2,
-                                                 void* ws, cudaStream_t st);
+template <typename T> cudaError_t drw_vjp_device(size_t M, size_t N, int batch, int row_major, int maxit, const void* tape, const T* gout,
+                                                 T* gY, T* gW1, T* gW2, void* ws, cudaStream_t st);
 
 // PDR_TV (src/TVNDopt.cpp:280-500): parallel Douglas-Rachford, fixed iteration count; same workspace as pd_device.  tape: nullptr, or
 // the recorded forward's buffer (header written by the caller): the segmentation tape of every pass but the last iteration's

@@ -6,6 +6,7 @@
 // here may be "improved" (SURVEY.md section 0.3).  All arrays stay in HBM for the whole solve; the only host round trip
 // is the 8-byte stop criterion of the Dykstra loops, once per iteration.
 #include "ptv_internal.h"
+#include "chunk_core.cuh"
 #include <float.h>
 #include <stdio.h>
 
@@ -33,7 +34,8 @@ template <typename T>
 cudaError_t scatter_fibers_ex_range(const T* in, const T* A, const T* B, const T* C, InOp op, int out_op, T* X, FiberGeom g,
                                     long long r_begin, long long r_end, cudaStream_t st);
 template <typename T>
-cudaError_t prox_fibers_chunked_contig_sparse(const T* A, T* X, FiberGeom g, T lam, const T* lamv, uint32_t* Mk, T* Cv, cudaStream_t st);
+cudaError_t prox_fibers_chunked_contig_sparse(const T* A, const T* B, InOp op, T* X, FiberGeom g, T lam, const T* lamv, uint32_t* Mk, T* Cv,
+                                              cudaStream_t st);
 template <typename T>
 cudaError_t scatter_fibers_ex_sparse_range(const T* in, const uint32_t* Mk, const T* Cv, const T* A, const T* B, const T* C, InOp op, int out_op,
                                            T* X, FiberGeom g, long long r_begin, long long r_end, cudaStream_t st);
@@ -108,7 +110,7 @@ static bool dr_iteration_pipelined(DrPipe& p, size_t M, size_t N, const T* Y, T*
         const long long r0 = cut(M, j, P), r1 = (j + 1 == P) ? (long long)M : cut(M, j + 1, P);
         if (r1 > r0) {
             KernelSpan sp(KC_PROX_STRIDED, 1, sc);
-            if (sparse) PCHK(prox_fibers_chunked_contig_sparse<T>(t1 + r0 * (long long)N, t2 + r0 * (long long)N, FiberGeom{r1 - r0, (int)N, 1}, w2,
+            if (sparse) PCHK(prox_fibers_chunked_contig_sparse<T>(t1 + r0 * (long long)N, nullptr, IN_A, t2 + r0 * (long long)N, FiberGeom{r1 - r0, (int)N, 1}, w2,
                                                                   nullptr, Mk + r0 * lpf, Cv + r0 * lpf, sc));
             else PCHK(prox_fibers_chunked_contig<T>(t1 + r0 * (long long)N, nullptr, nullptr, IN_A, t2 + r0 * (long long)N, 0,
                                                     FiberGeom{r1 - r0, (int)N, 1}, w2, nullptr, sc));
@@ -399,61 +401,89 @@ int dr2_device(size_t M, size_t N, int batch, int row_major, const T* Y, T w1, T
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// DR2L1W_TV (src/TV2DWopt.cpp:46-140): the Douglas-Rachford skeleton of DR2_TV with per-edge weights -- W1: (M-1) x N
-// (column fibers, contiguous, exactly the [fiber][len-1] layout of the weighted chunked kernel), W2: M x (N-1) (row
-// fibers, stride M) -- and the opposite reflection signs (:115, :125).  Rows go through the same gather -> contiguous
-// chunked kernel -> fused scatter route as DR2_TV; their weights are constant over the solve and are gathered once.
+// DR2L1W_TV (src/TV2DWopt.cpp:46-140): the Douglas-Rachford skeleton of DR2_TV with per-edge weights -- W1: (M-1) x N (column
+// fibers), W2: M x (N-1) (row fibers), each with len - 1 samples per fiber under its pass's slicing rule -- and the opposite reflection
+// signs (:115, :125).  `batch` images back to back, column-major or C order: the pass order (columns first) is the same, only the
+// stride roles swap.  The strided pass (rows of column-major images, columns of C-ordered ones) goes through the same gather ->
+// contiguous chunked kernel -> fused scatter route as DR2_TV, its weights gathered once; the contiguous pass runs the chunked kernel
+// in place (DrwPasses).
 template <typename T> cudaError_t gather_fibers(const T* A, const T* B, InOp op, T* out, FiberGeom g, cudaStream_t st);
-template <typename T>
-cudaError_t scatter_fibers_ex(const T* in, const T* A, const T* B, const T* C, InOp op, int out_op, T* X, FiberGeom g, cudaStream_t st);
 template <typename T>
 cudaError_t scatter_fibers_sparse(const T* in, const uint32_t* Mk, const T* Cv, const T* A, const T* B, const T* C, InOp op, int out_op, T* X,
                                   FiberGeom g, cudaStream_t st);
+template <typename T>
+cudaError_t expand_fibers_sparse(const T* in, const uint32_t* Mk, const T* Cv, const T* A, const T* B, const T* C, InOp op, int out_op, T* X,
+                                 FiberGeom g, cudaStream_t st);
 
 template <typename T>
-int drw_device(size_t M, size_t N, const T* Y, const T* W1, const T* W2, T* out, int maxit, double* info, void* ws, Engine eng,
-               cudaStream_t st) {
-    const long long n = (long long)M * (long long)N;
+cudaError_t DrwPasses<T>::init(size_t M, size_t N, int batch, int row_major, const T* W1, const T* W2, Engine e, void* stage, cudaStream_t st) {
+    g[0] = row_major ? FiberGeom{(long long)N * batch, (int)M, (long long)N} : FiberGeom{(long long)N * batch, (int)M, 1};
+    g[1] = row_major ? FiberGeom{(long long)M * batch, (int)N, 1} : FiberGeom{(long long)M * batch, (int)N, (long long)M};
+    W[0] = M > 1 ? W1 : nullptr; W[1] = N > 1 ? W2 : nullptr;
+    eng = e;
+    const size_t ab = align256(M * N * (size_t)batch * sizeof(T));
+    char* w = (char*)stage;
+    t1 = (T*)w; t2 = (T*)(w + ab); wg = (T*)(w + 2 * ab); Cv = (T*)(w + 3 * ab);
+    long long ncv = 0;                                        // per-chunk masks / entering values of the sparse results
+    for (int a = 0; a < 2; a++) {
+        fast[a] = eng != ENGINE_SEQ && g[a].len >= 64;
+        const long long c = g[a].nf * (((long long)g[a].len + 31) / 32);
+        if (fast[a] && c > ncv) ncv = c;
+    }
+    Mk = reinterpret_cast<uint32_t*>(Cv + ncv);
+    // by storage order, not by stride: a column-major image with M == 1 keeps the row route it always had
+    const int s = strided = row_major ? 0 : 1;
+    if (fast[s]) { KernelSpan sp(KC_ELEMENTWISE, 1, st);
+                   return gather_fibers<T>(W[s], nullptr, IN_A, wg, FiberGeom{g[s].nf, g[s].len - 1, g[s].inc}, st); }
+    return cudaSuccess;
+}
+
+template <typename T>
+cudaError_t DrwPasses<T>::run(int axis, const T* A, const T* B, const T* C, InOp op, T* X, int out_op, cudaStream_t st) {
+    const FiberGeom& G = g[axis];
+    const bool gathered = axis == strided;
+    // contiguous pass, output forms the chunked kernel's fill knows: prox_fibers_ex (chunked kernel, else the sequential one)
+    if (!gathered && out_op < OUT_DRW_ROWS) return prox_fibers_ex<T>(A, B, C, op, X, out_op, G, T(0), W[axis], eng, nullptr, st, 0);
+    if (fast[axis]) {
+        cudaError_t e;
+        if (gathered) { KernelSpan sp(KC_ELEMENTWISE, 1, st); e = gather_fibers<T>(A, B, op, t1, G, st); if (e != cudaSuccess) return e; }
+        { KernelSpan sp(gathered ? KC_PROX_STRIDED : KC_PROX_CONTIG, 1, st);
+          e = gathered ? prox_fibers_chunked_contig_sparse<T>(t1, nullptr, IN_A, t2, FiberGeom{G.nf, G.len, 1}, T(0), wg, Mk, Cv, st)
+                      : prox_fibers_chunked_contig_sparse<T>(A, B, op, t2, G, T(0), W[axis], Mk, Cv, st);      // no fill: expanded below
+          if (e == cudaErrorInvalidConfiguration) sp.cancel(); }
+        if (e == cudaErrorInvalidConfiguration) { cudaGetLastError(); fast[axis] = false; }
+        else {
+            if (e != cudaSuccess) return e;
+            KernelSpan sp(KC_ELEMENTWISE, 1, st);
+            const bool plain = out_op == OUT_X;               // the plain scatter never looks at the input
+            return gathered ? scatter_fibers_sparse<T>(t2, Mk, Cv, plain ? nullptr : A, plain ? nullptr : B, plain ? nullptr : C, op, out_op, X, G, st)
+                           : expand_fibers_sparse<T>(t2, Mk, Cv, A, B, C, op, out_op, X, G, st);
+        }
+    }
+    return prox_fibers_ex<T>(A, B, C, op, X, out_op, G, T(0), W[axis], ENGINE_SEQ, nullptr, st, 0);
+}
+
+template <typename T>
+int drw_device(size_t M, size_t N, int batch, int row_major, const T* Y, const T* W1, const T* W2, T* out, int maxit, double* info, void* ws,
+               Engine eng, cudaStream_t st) {
+    const long long n = (long long)M * (long long)N * batch;
     if (maxit <= 0) maxit = MAX_ITERS_DR;                                     // TV2DWopt.cpp:82
     if (n == 0) { if (info) { info[INFO_ITERS] = maxit; info[INFO_RC] = RC_OK; } return 0; }
     char* w = (char*)ws;
     T* t = (T*)w; w += align256(n * sizeof(T));
     T* s = (T*)w; w += align256(n * sizeof(T));
     T* x = (T*)w; w += align256(n * sizeof(T));
-    T* t1 = (T*)w; w += align256(n * sizeof(T));
-    T* t2 = (T*)w; w += align256(n * sizeof(T));
-    T* w2t = (T*)w; w += align256(n * sizeof(T));
-    T* Cv = (T*)w; uint32_t* Mk = reinterpret_cast<uint32_t*>(Cv + (long long)M * (((long long)N + 31) / 32));   // sparse row results
-    w += align256(n * sizeof(T));
+    DrwPasses<T> P;
+    PTV_TRY(P.init(M, N, batch, row_major, W1, W2, eng, w, st));
+    w += 4 * align256(n * sizeof(T));
     double* scratch = (double*)w;
-    const FiberGeom gc{(long long)N, (int)M, 1}, gr{(long long)M, (int)N, (long long)M}, grc{(long long)M, (int)N, 1};
-    bool fast_rows = eng != ENGINE_SEQ && N >= 64 && M >= 1;
-    if (fast_rows) { KernelSpan sp(KC_ELEMENTWISE, 1, st);
-                     PTV_TRY(gather_fibers<T>(W2, nullptr, IN_A, w2t, FiberGeom{(long long)M, (int)N - 1, (long long)M}, st)); }
-    PTV_TRY(ew_image_means_x2<T>(Y, n, 1, t, scratch, st));                   // :85-89
+    PTV_TRY(ew_image_means_x2<T>(Y, (long long)M * N, batch, t, scratch, st));   // :85-89
     for (int it = 0; it <= maxit; it++) {                                     // :94-119, then the final pair :122-125
         const bool final = it == maxit;
         // columns: s = 2 (t - prox_W1(t)) - t   (final: s = t - prox_W1(t))
-        PTV_TRY(prox_fibers_ex<T>(t, nullptr, nullptr, IN_A, s, final ? 2 : 1, gc, T(0), M > 1 ? W1 : nullptr, eng, nullptr, st, 0));
+        PTV_TRY(P.run(0, t, nullptr, nullptr, IN_A, s, final ? OUT_DIFF : OUT_REFLECT, st));
         // rows: in = Y - s ; tb = (in - prox_W2(in)) - Y ; tb = -2 tb - s ; t' = 0.5 (t + tb)   (final: out = -s - tb)
-        T* dst = final ? out : x;
-        const int oop = final ? 6 : 5;
-        bool done = false;
-        if (fast_rows) {
-            { KernelSpan sp(KC_ELEMENTWISE, 1, st); PTV_TRY(gather_fibers<T>(Y, s, IN_A_MINUS_B, t1, gr, st)); }
-            cudaError_t e;
-            { KernelSpan sp(KC_PROX_STRIDED, 1, st);
-              e = prox_fibers_chunked_contig_sparse<T>(t1, t2, grc, T(0), w2t, Mk, Cv, st);       // no fill: the scatter expands
-              if (e == cudaErrorInvalidConfiguration) sp.cancel(); }
-            if (e == cudaErrorInvalidConfiguration) { cudaGetLastError(); fast_rows = false; }
-            else {
-                PTV_TRY(e);
-                KernelSpan sp(KC_ELEMENTWISE, 1, st);
-                PTV_TRY(scatter_fibers_sparse<T>(t2, Mk, Cv, Y, s, t, IN_A_MINUS_B, oop, dst, gr, st));
-                done = true;
-            }
-        }
-        if (!done) PTV_TRY(prox_fibers_ex<T>(Y, s, t, IN_A_MINUS_B, dst, oop, gr, T(0), N > 1 ? W2 : nullptr, ENGINE_SEQ, nullptr, st, 0));
+        PTV_TRY(P.run(1, Y, s, t, IN_A_MINUS_B, final ? out : x, final ? OUT_DRW_ROWS_FINAL : OUT_DRW_ROWS, st));
         if (!final) { T* tmp = t; t = x; x = tmp; }
     }
     if (info) { info[INFO_ITERS] = maxit; info[INFO_RC] = RC_OK; }            // :128-131
@@ -625,7 +655,8 @@ int pdr_device(const T* y, const double* lam, const double* dims, T* x, double* 
     template size_t ws_bytes_dr2<T>(size_t, size_t, int); \
     template int dr2_device<T>(size_t, size_t, int, int, const T*, T, T, T*, int, double*, void*, Engine, cudaStream_t); \
     template int dr2_lane_pick<T>(size_t, size_t, int, int, const T*, const T*, const void*, T, T, Engine, void**); \
-    template int drw_device<T>(size_t, size_t, const T*, const T*, const T*, T*, int, double*, void*, Engine, cudaStream_t); \
+    template int drw_device<T>(size_t, size_t, int, int, const T*, const T*, const T*, T*, int, double*, void*, Engine, cudaStream_t); \
+    template struct DrwPasses<T>; \
     template size_t ws_bytes_pd<T>(long long, int); \
     template int pd2_device<T>(const T*, const double*, const double*, T*, double*, const int*, int, int, int, void*, Engine, cudaStream_t, \
                                void*); \

@@ -309,7 +309,45 @@ cudaError_t scatter_fibers_sparse(const T* in, const uint32_t* Mk, const T* Cv, 
     }
     return cudaGetLastError();
 }
+// Expand a SPARSE prox result over CONTIGUOUS fibers g (prox_fibers_chunked_contig_sparse) with a fused output form, in the fibers'
+// own layout: X[e] = apply_out_any(out_op, A[e] (op) B[e], x, A, B, C, e), x the value of the segment that covers e.  The chunked
+// kernel's fill only knows the forms of apply_out_ex (the weighted Douglas-Rachford ones would fatten its loop for every caller), so
+// the contiguous row pass of C-ordered weighted images ends here instead.  One warp per 32-sample window: its start mask and
+// entering value are one broadcast load each, the segment values lie in the window itself.  X may not alias in.
+template <typename T>
+__global__ void __launch_bounds__(256) k_expand_sparse(const T* __restrict__ in, const uint32_t* __restrict__ Mk, const T* __restrict__ Cv,
+                                                       const T* A, const T* B, const T* C, int op, int out_op, T* X, long long nf, int len) {
+    const int lane = threadIdx.x & 31;
+    const long long lpf = ((long long)len + 31) >> 5, nw = nf * lpf;
+    const uint32_t below = 0xffffffffu >> (31 - lane);
+    for (long long q = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; q < nw; q += ((long long)gridDim.x * blockDim.x) >> 5) {
+        const long long f = q / lpf, c = q - f * lpf;
+        const uint32_t m = Mk[q] & below;
+        const T cv = Cv[q];
+        const long long w0 = f * len + c * 32, k = c * 32 + lane;
+        if (k < len) {
+            const long long e = w0 + lane;
+            const T xv = m ? in[w0 + high_bit(m)] : cv;
+            T yin = A[e];
+            if (op == IN_A_MINUS_B) yin = yin - B[e]; else if (op == IN_A_PLUS_B) yin = yin + B[e];
+            X[e] = apply_out_any<T>(out_op, yin, xv, A, B, C, e);
+        }
+    }
+}
+template <typename T>
+cudaError_t expand_fibers_sparse(const T* in, const uint32_t* Mk, const T* Cv, const T* A, const T* B, const T* C, InOp op, int out_op, T* X,
+                                 FiberGeom g, cudaStream_t st) {
+    if (g.nf <= 0 || g.len <= 0) return cudaSuccess;
+    if (g.inc != 1) return cudaErrorInvalidValue;
+    const long long warps = g.nf * (((long long)g.len + 31) / 32);
+    long long blocks = (warps + 7) / 8;
+    if (blocks > 132LL * 16) blocks = 132LL * 16;
+    k_expand_sparse<T><<<(unsigned)blocks, 256, 0, st>>>(in, Mk, Cv, A, B, C, (int)op, out_op, X, g.nf, g.len);
+    return cudaGetLastError();
+}
+
 #define INST_R(T) \
+    template cudaError_t expand_fibers_sparse<T>(const T*, const uint32_t*, const T*, const T*, const T*, const T*, InOp, int, T*, FiberGeom, cudaStream_t); \
     template cudaError_t scatter_fibers_sparse<T>(const T*, const uint32_t*, const T*, const T*, const T*, const T*, InOp, int, T*, FiberGeom, cudaStream_t); \
     template cudaError_t scatter_fibers_ex_sparse_range<T>(const T*, const uint32_t*, const T*, const T*, const T*, const T*, InOp, int, T*, FiberGeom, long long, long long, cudaStream_t); \
     template cudaError_t gather_fibers_range<T>(const T*, const T*, InOp, T*, FiberGeom, int, int, cudaStream_t); \
