@@ -161,18 +161,37 @@ int run_drw(const char* fn, bool host_io, size_t M, size_t N, int batch, int row
     return 0;
 }
 
-// mode 0: PD2_TV, 1: PD_TV, 2: PDR_TV.  y/x host (host_io) or device pointers.
+// PD_TV and PDR_TV multiply the caller's penalties by the number of terms, in place (TVNDopt.cpp:100-101, :339-340); PD2_TV takes
+// them as given.
+void scale_penalties(NdSolver s, double* lambdas, int npen) {
+    if (s != ND_PD2) for (int i = 0; i < npen; i++) lambdas[i] *= npen;
+}
+
+// The device solver of s (solver.cu); tape: nullptr, or the recorded forward's buffer.
 template <typename T>
-int run_pd(const char* fn, int mode, bool host_io, const T* y, double* lambdas, double* norms, double* dims, T* x, double* info,
+int nd_solve(NdSolver s, const T* y, const double* lambdas, const double* dims, T* x, double* info, const int* ns, int nds, int npen,
+             int maxIters, void* ws, cudaStream_t st, void* tape) {
+    switch (s) {
+    case ND_PD2: return pd2_device<T>(y, lambdas, dims, x, info, ns, nds, npen, maxIters, ws, (Engine)g_engine, st, tape);
+    case ND_PD: return pd_device<T>(y, lambdas, dims, x, info, ns, nds, npen, maxIters, ws, (Engine)g_engine, st, tape);
+    default: return pdr_device<T>(y, lambdas, dims, x, info, ns, nds, npen, maxIters, ws, (Engine)g_engine, st, tape);
+    }
+}
+
+// y/x host (host_io) or device pointers.
+template <typename T>
+int run_pd(const char* fn, NdSolver s, bool host_io, const T* y, double* lambdas, double* norms, double* dims, T* x, double* info,
            int* ns, int nds, int npen, int maxIters, cudaStream_t st) {
     if (!have_device(fn, info)) return 0;
     if (norms) for (int i = 0; i < npen; i++) if (norms[i] != 1.0) {
         fail(fn, "only p = 1 (TV-L1) penalty terms are implemented on the GPU path", info); return 0; }
     if (nds <= 0 || !ns) { fail(fn, "invalid dimensions", info); return 0; }
-    long long n = 1; for (int i = 0; i < nds; i++) n *= ns[i];
+    NdTerms t;
+    nd_terms(ns, nds, 0, nullptr, &t);                 // the element count; the solver checks the terms
+    const long long n = t.n;
     WsGuard guard(st);
-    if (mode >= 1) for (int i = 0; i < npen; i++) lambdas[i] *= npen;                   // TVNDopt.cpp:100-101, :339-340 (in place)
-    void* ws = g_ws.get(ws_bytes_pd<T>(n, npen > 2 ? npen : 2));
+    scale_penalties(s, lambdas, npen);
+    void* ws = g_ws.get(ws_bytes_pd<T>(n, npen));
     if (!ws) { fail(fn, "out of memory", info); return 0; }
     const T* dy = y; T* dx = x;
     if (host_io && n > 0) {
@@ -181,10 +200,7 @@ int run_pd(const char* fn, int mode, bool host_io, const T* y, double* lambdas, 
         dy = (T*)d; dx = (T*)(d + al((size_t)n * sizeof(T)));
         if (!cuda_ok(fn, cudaMemcpyAsync((void*)dy, y, (size_t)n * sizeof(T), cudaMemcpyHostToDevice, st), info)) return 0;
     }
-    int rc = mode == 0 ? pd2_device<T>(dy, lambdas, dims, dx, info, ns, nds, npen, maxIters, ws, (Engine)g_engine, st)
-           : mode == 1 ? pd_device<T>(dy, lambdas, dims, dx, info, ns, nds, npen, maxIters, ws, (Engine)g_engine, st)
-                       : pdr_device<T>(dy, lambdas, dims, dx, info, ns, nds, npen, maxIters, ws, (Engine)g_engine, st);
-    if (!rc) return 0;
+    if (!nd_solve<T>(s, dy, lambdas, dims, dx, info, ns, nds, npen, maxIters, ws, st, nullptr)) return 0;
     if (host_io && n > 0) {
         if (!cuda_ok(fn, cudaMemcpyAsync(x, dx, (size_t)n * sizeof(T), cudaMemcpyDeviceToHost, st), info)) return 0;
         if (!cuda_ok(fn, cudaStreamSynchronize(st), info)) return 0;
@@ -312,96 +328,66 @@ static int dev_drw_vjp(const char* fn, size_t M, size_t N, int batch, int row_ma
     return cuda_ok(fn, drw_vjp_device<T>(M, N, batch, row_major, maxit, tape, gout, gY, gW1, gW2, ws, (cudaStream_t)stream), nullptr);
 }
 
-// Arguments of the PDR_TV tape entry points: nullptr when valid, else the reason.
-const char* pdr_args_check(const int* ns, int nds, int npen, const double* dims) {
+// The shape bounds of the tape paths (the header holds up to PDR_TAPE_MAX_DIMS axes): nullptr when valid, else the reason.
+const char* nd_shape_check(NdSolver s, const int* ns, int nds, int npen) {
+    if (s == ND_PD2 && (npen < 1 || npen > 2)) return "PD2_TV takes 1 or 2 penalty terms";
     if (nds < 1 || nds > PDR_TAPE_MAX_DIMS) return "invalid dimensions (need 1 <= nds <= 16)";
     for (int i = 0; i < nds; i++) if (ns[i] < 0) return "invalid dimensions (negative size)";
     if (npen < 1 || npen > 64) return "need 1 to 64 penalty terms";
-    long long n = 1; for (int i = 0; i < nds; i++) n *= ns[i];
-    FiberGeom g;
-    for (int i = 0; i < npen; i++) if (!geom_of(ns, nds, dims[i], n, &g)) return "invalid penalty dimensions";
     return nullptr;
 }
 
-// PDR_TV as proxtv_PDR_TV_dev_* computes it (the same pdr_device call), writing the tape; every refusal comes before anything is
-// written, lambdas included.
-template <typename T>
-static int dev_pdr_record(const char* fn, const T* y, double* lambdas, const double* dims, T* x, double* info, const int* ns, int nds,
-                          int npen, int maxIters, void* tape, size_t tape_bytes, void* stream) {
-    if (!y || !x || !lambdas || !dims || !ns || !tape) { fail(fn, "NULL array", info); return 0; }
-    if (const char* why = pdr_args_check(ns, nds, npen, dims)) { fail(fn, why, info); return 0; }
-    for (int i = 0; i < npen; i++) if (!(lambdas[i] >= 0)) { fail(fn, "negative penalty", info); return 0; }
-    const size_t need = pdr_tape_bytes(ns, nds, npen, maxIters);
-    if (need == 0) { fail(fn, "tape size does not fit in size_t (maxIters too large)", info); return 0; }
-    if (tape_bytes < need) { fail(fn, "tape_bytes smaller than proxtv_PDR_TV_tape_bytes()", info); return 0; }
-    if (!have_device(fn, info)) return 0;
-    WsGuard guard((cudaStream_t)stream);
-    long long n = 1; for (int i = 0; i < nds; i++) n *= ns[i];
-    void* ws = g_ws.get(ws_bytes_pd<T>(n, npen > 2 ? npen : 2));
-    if (!ws) { fail(fn, "out of memory", info); return 0; }
-    if (!cuda_ok(fn, pdr_tape_header(tape, sizeof(T), ns, nds, npen, dims, maxIters, (cudaStream_t)stream), info)) return 0;
-    for (int i = 0; i < npen; i++) lambdas[i] *= npen;                                  // as run_pd
-    if (!pdr_device<T>(y, lambdas, dims, x, info, ns, nds, npen, maxIters, ws, (Engine)g_engine, (cudaStream_t)stream, tape)) {
-        fail(fn, "device solver failed", info); return 0; }
-    return 1;
+// Arguments of the tape entry points: nullptr when valid (t filled), else the reason.
+const char* nd_args_check(NdSolver s, const int* ns, int nds, int npen, const double* dims, NdTerms* t) {
+    if (const char* why = nd_shape_check(s, ns, nds, npen)) return why;
+    return nd_terms(ns, nds, npen, dims, t);
 }
 
-template <typename T>
-static int dev_pdr_vjp(const char* fn, const int* ns, int nds, int npen, const double* dims, int maxIters, const void* tape, const T* gout,
-                       T* gY, double* glam, void* stream) {
-    if (!ns || !dims || !tape || !gout || !gY) { fail(fn, "NULL array", nullptr); return 0; }
-    if (const char* why = pdr_args_check(ns, nds, npen, dims)) { fail(fn, why, nullptr); return 0; }
-    if (!have_device(fn, nullptr)) return 0;
-    WsGuard guard((cudaStream_t)stream);
-    if (const char* why = pdr_tape_check(tape, sizeof(T), ns, nds, npen, dims, maxIters, (cudaStream_t)stream)) { fail(fn, why, nullptr); return 0; }
-    void* ws = g_ws.get(ws_bytes_pdr_vjp<T>(ns, nds, npen, dims, glam != nullptr));
-    if (!ws) { fail(fn, "out of memory", nullptr); return 0; }
-    return cuda_ok(fn, pdr_vjp_device<T>(ns, nds, npen, dims, maxIters, tape, gout, gY, glam, ws, (cudaStream_t)stream), nullptr);
+size_t nd_tape_bytes_checked(NdSolver s, const int* ns, int nds, int npen, int maxIters) {
+    return !ns || nd_shape_check(s, ns, nds, npen) ? 0 : nd_tape_bytes(s, ns, nds, npen, maxIters);
 }
 
-// PD_TV (pd2 false) or PD2_TV as proxtv_PD_TV_dev_* / proxtv_PD2_TV_dev_* compute it (the same pd_device / pd2_device call), writing
-// the tape and, after the solve, its header with the iterations run; every refusal comes before anything is written, lambdas included.
+// The solver s as proxtv_<solver>_dev_* computes it (the same device solver call), writing the tape and, after the solve, its header;
+// every refusal comes before anything is written, lambdas included.
 template <typename T>
-static int dev_pd_record(const char* fn, bool pd2, const T* y, double* lambdas, const double* dims, T* x, double* info, const int* ns,
+static int dev_nd_record(const char* fn, NdSolver s, const T* y, double* lambdas, const double* dims, T* x, double* info, const int* ns,
                          int nds, int npen, int maxIters, void* tape, size_t tape_bytes, void* stream) {
+    static const char* const too_small[3] = {"tape_bytes smaller than proxtv_PD2_TV_tape_bytes()",
+                                             "tape_bytes smaller than proxtv_PD_TV_tape_bytes()",
+                                             "tape_bytes smaller than proxtv_PDR_TV_tape_bytes()"};
     if (!y || !x || !lambdas || !dims || !ns || !tape) { fail(fn, "NULL array", info); return 0; }
-    if (pd2 && (npen < 1 || npen > 2)) { fail(fn, "PD2_TV takes 1 or 2 penalty terms", info); return 0; }
-    if (const char* why = pdr_args_check(ns, nds, npen, dims)) { fail(fn, why, info); return 0; }
+    NdTerms t;
+    if (const char* why = nd_args_check(s, ns, nds, npen, dims, &t)) { fail(fn, why, info); return 0; }
     for (int i = 0; i < npen; i++) if (!(lambdas[i] >= 0)) { fail(fn, "negative penalty", info); return 0; }
-    const size_t need = pd_tape_bytes(pd2, ns, nds, npen, maxIters);
+    const size_t need = nd_tape_bytes(s, ns, nds, npen, maxIters);
     if (need == 0) { fail(fn, "tape size does not fit in size_t (maxIters too large)", info); return 0; }
-    if (tape_bytes < need) {
-        fail(fn, pd2 ? "tape_bytes smaller than proxtv_PD2_TV_tape_bytes()" : "tape_bytes smaller than proxtv_PD_TV_tape_bytes()", info);
-        return 0;
-    }
+    if (tape_bytes < need) { fail(fn, too_small[s], info); return 0; }
     if (!have_device(fn, info)) return 0;
     WsGuard guard((cudaStream_t)stream);
-    long long n = 1; for (int i = 0; i < nds; i++) n *= ns[i];
-    void* ws = g_ws.get(ws_bytes_pd<T>(n, npen > 2 ? npen : 2));
+    void* ws = g_ws.get(ws_bytes_pd<T>(t.n, npen));
     if (!ws) { fail(fn, "out of memory", info); return 0; }
     double linfo[3] = {0, 0, RC_OK};                   // the header needs the iteration count even when the caller passes no info
     double* pinfo = info ? info : linfo;
-    if (!pd2) for (int i = 0; i < npen; i++) lambdas[i] *= npen;                        // as run_pd
-    const int ok = pd2 ? pd2_device<T>(y, lambdas, dims, x, pinfo, ns, nds, npen, maxIters, ws, (Engine)g_engine, (cudaStream_t)stream, tape)
-                       : pd_device<T>(y, lambdas, dims, x, pinfo, ns, nds, npen, maxIters, ws, (Engine)g_engine, (cudaStream_t)stream, tape);
-    if (!ok) { fail(fn, "device solver failed", info); return 0; }
-    return cuda_ok(fn, pd_tape_header(pd2, tape, sizeof(T), ns, nds, npen, dims, maxIters, (int)pinfo[INFO_ITERS], (cudaStream_t)stream),
+    scale_penalties(s, lambdas, npen);
+    if (!nd_solve<T>(s, y, lambdas, dims, x, pinfo, ns, nds, npen, maxIters, ws, (cudaStream_t)stream, tape)) {
+        fail(fn, "device solver failed", info); return 0; }
+    return cuda_ok(fn, nd_tape_header(s, tape, sizeof(T), ns, nds, npen, dims, maxIters, (int)pinfo[INFO_ITERS], (cudaStream_t)stream),
                    info) ? 1 : 0;
 }
 
 template <typename T>
-static int dev_pd_vjp(const char* fn, bool pd2, const int* ns, int nds, int npen, const double* dims, int maxIters, int iters,
+static int dev_nd_vjp(const char* fn, NdSolver s, const int* ns, int nds, int npen, const double* dims, int maxIters, int iters,
                       const void* tape, const T* gout, T* gY, double* glam, void* stream) {
     if (!ns || !dims || !tape || !gout || !gY) { fail(fn, "NULL array", nullptr); return 0; }
-    if (pd2 && (npen < 1 || npen > 2)) { fail(fn, "PD2_TV takes 1 or 2 penalty terms", nullptr); return 0; }
-    if (const char* why = pdr_args_check(ns, nds, npen, dims)) { fail(fn, why, nullptr); return 0; }
+    NdTerms t;
+    if (const char* why = nd_args_check(s, ns, nds, npen, dims, &t)) { fail(fn, why, nullptr); return 0; }
     if (!have_device(fn, nullptr)) return 0;
     WsGuard guard((cudaStream_t)stream);
-    if (const char* why = pd_tape_check(pd2, tape, sizeof(T), ns, nds, npen, dims, maxIters, iters, (cudaStream_t)stream)) {
+    if (const char* why = nd_tape_check(s, tape, sizeof(T), ns, nds, npen, dims, maxIters, iters, (cudaStream_t)stream)) {
         fail(fn, why, nullptr); return 0; }
-    void* ws = g_ws.get(ws_bytes_pdr_vjp<T>(ns, nds, npen, dims, glam != nullptr));
+    void* ws = g_ws.get(ws_bytes_nd_vjp<T>(t, npen, glam != nullptr));
     if (!ws) { fail(fn, "out of memory", nullptr); return 0; }
-    return cuda_ok(fn, pd_vjp_device<T>(pd2, ns, nds, npen, dims, iters, tape, gout, gY, glam, ws, (cudaStream_t)stream), nullptr);
+    return cuda_ok(fn, nd_vjp_device<T>(s, t, npen, maxIters, iters, tape, gout, gY, glam, ws, (cudaStream_t)stream), nullptr);
 }
 
 }  // namespace
@@ -520,15 +506,15 @@ int DR2L1W_TV(size_t M, size_t N, double* unary, double* W1, double* W2, double*
 }
 int PD2_TV(double* y, double* lambdas, double* norms, double* dims, double* x, double* info, int* ns, int nds, int npen, int,
            int maxIters) {
-    return run_pd<double>("PD2_TV", 0, true, y, lambdas, norms, dims, x, info, ns, nds, npen, maxIters, 0);
+    return run_pd<double>("PD2_TV", ND_PD2, true, y, lambdas, norms, dims, x, info, ns, nds, npen, maxIters, 0);
 }
 int PD_TV(double* y, double* lambdas, double* norms, double* dims, double* x, double* info, int* ns, int nds, int npen, int,
           int maxIters) {
-    return run_pd<double>("PD_TV", 1, true, y, lambdas, norms, dims, x, info, ns, nds, npen, maxIters, 0);
+    return run_pd<double>("PD_TV", ND_PD, true, y, lambdas, norms, dims, x, info, ns, nds, npen, maxIters, 0);
 }
 int PDR_TV(double* y, double* lambdas, double* norms, double* dims, double* x, double* info, int* ns, int nds, int npen, int,
            int maxIters) {
-    return run_pd<double>("PDR_TV", 2, true, y, lambdas, norms, dims, x, info, ns, nds, npen, maxIters, 0);
+    return run_pd<double>("PDR_TV", ND_PDR, true, y, lambdas, norms, dims, x, info, ns, nds, npen, maxIters, 0);
 }
 
 // ---- Part 2: extensions ----
@@ -648,66 +634,57 @@ int proxtv_DR2L1W_TV_batched_f32(size_t M, size_t N, int batch, int row_major, c
     return run_drw<float>("proxtv_DR2L1W_TV_batched_f32", true, M, N, batch, row_major, Y, W1, W2, out, maxit, info, 0); }
 
 int proxtv_PD2_TV_dev_f64(const double* y, double* lambdas, double* dims, double* x, double* info, int* ns, int nds, int npen, int maxIters, void* stream) {
-    return run_pd<double>("proxtv_PD2_TV_dev_f64", 0, false, y, lambdas, nullptr, dims, x, info, ns, nds, npen, maxIters, (cudaStream_t)stream); }
+    return run_pd<double>("proxtv_PD2_TV_dev_f64", ND_PD2, false, y, lambdas, nullptr, dims, x, info, ns, nds, npen, maxIters, (cudaStream_t)stream); }
 int proxtv_PD2_TV_dev_f32(const float* y, double* lambdas, double* dims, float* x, double* info, int* ns, int nds, int npen, int maxIters, void* stream) {
-    return run_pd<float>("proxtv_PD2_TV_dev_f32", 0, false, y, lambdas, nullptr, dims, x, info, ns, nds, npen, maxIters, (cudaStream_t)stream); }
+    return run_pd<float>("proxtv_PD2_TV_dev_f32", ND_PD2, false, y, lambdas, nullptr, dims, x, info, ns, nds, npen, maxIters, (cudaStream_t)stream); }
 int proxtv_PD_TV_dev_f64(const double* y, double* lambdas, double* dims, double* x, double* info, int* ns, int nds, int npen, int maxIters, void* stream) {
-    return run_pd<double>("proxtv_PD_TV_dev_f64", 1, false, y, lambdas, nullptr, dims, x, info, ns, nds, npen, maxIters, (cudaStream_t)stream); }
+    return run_pd<double>("proxtv_PD_TV_dev_f64", ND_PD, false, y, lambdas, nullptr, dims, x, info, ns, nds, npen, maxIters, (cudaStream_t)stream); }
 int proxtv_PD_TV_dev_f32(const float* y, double* lambdas, double* dims, float* x, double* info, int* ns, int nds, int npen, int maxIters, void* stream) {
-    return run_pd<float>("proxtv_PD_TV_dev_f32", 1, false, y, lambdas, nullptr, dims, x, info, ns, nds, npen, maxIters, (cudaStream_t)stream); }
+    return run_pd<float>("proxtv_PD_TV_dev_f32", ND_PD, false, y, lambdas, nullptr, dims, x, info, ns, nds, npen, maxIters, (cudaStream_t)stream); }
 int proxtv_PDR_TV_dev_f64(const double* y, double* lambdas, double* dims, double* x, double* info, int* ns, int nds, int npen, int maxIters, void* stream) {
-    return run_pd<double>("proxtv_PDR_TV_dev_f64", 2, false, y, lambdas, nullptr, dims, x, info, ns, nds, npen, maxIters, (cudaStream_t)stream); }
+    return run_pd<double>("proxtv_PDR_TV_dev_f64", ND_PDR, false, y, lambdas, nullptr, dims, x, info, ns, nds, npen, maxIters, (cudaStream_t)stream); }
 int proxtv_PDR_TV_dev_f32(const float* y, double* lambdas, double* dims, float* x, double* info, int* ns, int nds, int npen, int maxIters, void* stream) {
-    return run_pd<float>("proxtv_PDR_TV_dev_f32", 2, false, y, lambdas, nullptr, dims, x, info, ns, nds, npen, maxIters, (cudaStream_t)stream); }
-size_t proxtv_PDR_TV_tape_bytes(const int* ns, int nds, int npen, int maxIters) {
-    if (!ns || nds < 1 || nds > PDR_TAPE_MAX_DIMS || npen < 1 || npen > 64) return 0;
-    for (int i = 0; i < nds; i++) if (ns[i] < 0) return 0;
-    return pdr_tape_bytes(ns, nds, npen, maxIters);
-}
+    return run_pd<float>("proxtv_PDR_TV_dev_f32", ND_PDR, false, y, lambdas, nullptr, dims, x, info, ns, nds, npen, maxIters, (cudaStream_t)stream); }
+size_t proxtv_PDR_TV_tape_bytes(const int* ns, int nds, int npen, int maxIters) { return nd_tape_bytes_checked(ND_PDR, ns, nds, npen, maxIters); }
 int proxtv_PDR_TV_record_dev_f64(const double* y, double* lambdas, double* dims, double* x, double* info, int* ns, int nds, int npen,
                                  int maxIters, void* tape, size_t tape_bytes, void* stream) {
-    return dev_pdr_record<double>("proxtv_PDR_TV_record_dev_f64", y, lambdas, dims, x, info, ns, nds, npen, maxIters, tape, tape_bytes, stream); }
+    return dev_nd_record<double>("proxtv_PDR_TV_record_dev_f64", ND_PDR, y, lambdas, dims, x, info, ns, nds, npen, maxIters, tape, tape_bytes, stream); }
 int proxtv_PDR_TV_record_dev_f32(const float* y, double* lambdas, double* dims, float* x, double* info, int* ns, int nds, int npen,
                                  int maxIters, void* tape, size_t tape_bytes, void* stream) {
-    return dev_pdr_record<float>("proxtv_PDR_TV_record_dev_f32", y, lambdas, dims, x, info, ns, nds, npen, maxIters, tape, tape_bytes, stream); }
+    return dev_nd_record<float>("proxtv_PDR_TV_record_dev_f32", ND_PDR, y, lambdas, dims, x, info, ns, nds, npen, maxIters, tape, tape_bytes, stream); }
 int proxtv_PDR_TV_vjp_dev_f64(const int* ns, int nds, int npen, const double* dims, int maxIters, const void* tape, const double* gout,
                               double* gY, double* glam, void* stream) {
-    return dev_pdr_vjp<double>("proxtv_PDR_TV_vjp_dev_f64", ns, nds, npen, dims, maxIters, tape, gout, gY, glam, stream); }
+    return dev_nd_vjp<double>("proxtv_PDR_TV_vjp_dev_f64", ND_PDR, ns, nds, npen, dims, maxIters, 0, tape, gout, gY, glam, stream); }
 int proxtv_PDR_TV_vjp_dev_f32(const int* ns, int nds, int npen, const double* dims, int maxIters, const void* tape, const float* gout,
                               float* gY, double* glam, void* stream) {
-    return dev_pdr_vjp<float>("proxtv_PDR_TV_vjp_dev_f32", ns, nds, npen, dims, maxIters, tape, gout, gY, glam, stream); }
-static size_t pd_tape_bytes_checked(bool pd2, const int* ns, int nds, int npen, int maxIters) {
-    if (!ns || nds < 1 || nds > PDR_TAPE_MAX_DIMS || npen < 1 || npen > (pd2 ? 2 : 64)) return 0;
-    for (int i = 0; i < nds; i++) if (ns[i] < 0) return 0;
-    return pd_tape_bytes(pd2, ns, nds, npen, maxIters);
-}
-size_t proxtv_PD_TV_tape_bytes(const int* ns, int nds, int npen, int maxIters) { return pd_tape_bytes_checked(false, ns, nds, npen, maxIters); }
-size_t proxtv_PD2_TV_tape_bytes(const int* ns, int nds, int npen, int maxIters) { return pd_tape_bytes_checked(true, ns, nds, npen, maxIters); }
+    return dev_nd_vjp<float>("proxtv_PDR_TV_vjp_dev_f32", ND_PDR, ns, nds, npen, dims, maxIters, 0, tape, gout, gY, glam, stream); }
+size_t proxtv_PD_TV_tape_bytes(const int* ns, int nds, int npen, int maxIters) { return nd_tape_bytes_checked(ND_PD, ns, nds, npen, maxIters); }
+size_t proxtv_PD2_TV_tape_bytes(const int* ns, int nds, int npen, int maxIters) { return nd_tape_bytes_checked(ND_PD2, ns, nds, npen, maxIters); }
 int proxtv_PD_TV_record_dev_f64(const double* y, double* lambdas, double* dims, double* x, double* info, int* ns, int nds, int npen,
                                 int maxIters, void* tape, size_t tape_bytes, void* stream) {
-    return dev_pd_record<double>("proxtv_PD_TV_record_dev_f64", false, y, lambdas, dims, x, info, ns, nds, npen, maxIters, tape, tape_bytes, stream); }
+    return dev_nd_record<double>("proxtv_PD_TV_record_dev_f64", ND_PD, y, lambdas, dims, x, info, ns, nds, npen, maxIters, tape, tape_bytes, stream); }
 int proxtv_PD_TV_record_dev_f32(const float* y, double* lambdas, double* dims, float* x, double* info, int* ns, int nds, int npen,
                                 int maxIters, void* tape, size_t tape_bytes, void* stream) {
-    return dev_pd_record<float>("proxtv_PD_TV_record_dev_f32", false, y, lambdas, dims, x, info, ns, nds, npen, maxIters, tape, tape_bytes, stream); }
+    return dev_nd_record<float>("proxtv_PD_TV_record_dev_f32", ND_PD, y, lambdas, dims, x, info, ns, nds, npen, maxIters, tape, tape_bytes, stream); }
 int proxtv_PD2_TV_record_dev_f64(const double* y, double* lambdas, double* dims, double* x, double* info, int* ns, int nds, int npen,
                                  int maxIters, void* tape, size_t tape_bytes, void* stream) {
-    return dev_pd_record<double>("proxtv_PD2_TV_record_dev_f64", true, y, lambdas, dims, x, info, ns, nds, npen, maxIters, tape, tape_bytes, stream); }
+    return dev_nd_record<double>("proxtv_PD2_TV_record_dev_f64", ND_PD2, y, lambdas, dims, x, info, ns, nds, npen, maxIters, tape, tape_bytes, stream); }
 int proxtv_PD2_TV_record_dev_f32(const float* y, double* lambdas, double* dims, float* x, double* info, int* ns, int nds, int npen,
                                  int maxIters, void* tape, size_t tape_bytes, void* stream) {
-    return dev_pd_record<float>("proxtv_PD2_TV_record_dev_f32", true, y, lambdas, dims, x, info, ns, nds, npen, maxIters, tape, tape_bytes, stream); }
+    return dev_nd_record<float>("proxtv_PD2_TV_record_dev_f32", ND_PD2, y, lambdas, dims, x, info, ns, nds, npen, maxIters, tape, tape_bytes, stream); }
 int proxtv_PD_TV_vjp_dev_f64(const int* ns, int nds, int npen, const double* dims, int maxIters, int iters, const void* tape,
                              const double* gout, double* gY, double* glam, void* stream) {
-    return dev_pd_vjp<double>("proxtv_PD_TV_vjp_dev_f64", false, ns, nds, npen, dims, maxIters, iters, tape, gout, gY, glam, stream); }
+    return dev_nd_vjp<double>("proxtv_PD_TV_vjp_dev_f64", ND_PD, ns, nds, npen, dims, maxIters, iters, tape, gout, gY, glam, stream); }
 int proxtv_PD_TV_vjp_dev_f32(const int* ns, int nds, int npen, const double* dims, int maxIters, int iters, const void* tape,
                              const float* gout, float* gY, double* glam, void* stream) {
-    return dev_pd_vjp<float>("proxtv_PD_TV_vjp_dev_f32", false, ns, nds, npen, dims, maxIters, iters, tape, gout, gY, glam, stream); }
+    return dev_nd_vjp<float>("proxtv_PD_TV_vjp_dev_f32", ND_PD, ns, nds, npen, dims, maxIters, iters, tape, gout, gY, glam, stream); }
 int proxtv_PD2_TV_vjp_dev_f64(const int* ns, int nds, int npen, const double* dims, int maxIters, int iters, const void* tape,
                               const double* gout, double* gY, double* glam, void* stream) {
-    return dev_pd_vjp<double>("proxtv_PD2_TV_vjp_dev_f64", true, ns, nds, npen, dims, maxIters, iters, tape, gout, gY, glam, stream); }
+    return dev_nd_vjp<double>("proxtv_PD2_TV_vjp_dev_f64", ND_PD2, ns, nds, npen, dims, maxIters, iters, tape, gout, gY, glam, stream); }
 int proxtv_PD2_TV_vjp_dev_f32(const int* ns, int nds, int npen, const double* dims, int maxIters, int iters, const void* tape,
                               const float* gout, float* gY, double* glam, void* stream) {
-    return dev_pd_vjp<float>("proxtv_PD2_TV_vjp_dev_f32", true, ns, nds, npen, dims, maxIters, iters, tape, gout, gY, glam, stream); }
+    return dev_nd_vjp<float>("proxtv_PD2_TV_vjp_dev_f32", ND_PD2, ns, nds, npen, dims, maxIters, iters, tape, gout, gY, glam, stream); }
 int proxtv_PD_TV_f32(const float* y, double* lambdas, double* dims, float* x, double* info, int* ns, int nds, int npen, int maxIters) {
-    return run_pd<float>("proxtv_PD_TV_f32", 1, true, y, lambdas, nullptr, dims, x, info, ns, nds, npen, maxIters, 0); }
+    return run_pd<float>("proxtv_PD_TV_f32", ND_PD, true, y, lambdas, nullptr, dims, x, info, ns, nds, npen, maxIters, 0); }
 
 }  // extern "C"

@@ -516,22 +516,36 @@ struct PdrTapeHeader {
     uint8_t pad[256 - 8 - 16 - 4 * PDR_TAPE_MAX_DIMS - 64 - 4];
 };
 static_assert(sizeof(PdrTapeHeader) == 256, "tape header is 256 bytes");
-static constexpr uint64_t PDR_TAPE_MAGIC = 0x3150415452524450ull;          // "PDRRTAP1"
-static constexpr uint64_t PD_TAPE_MAGIC = 0x3150415456544450ull;           // "PDTVTAP1"
-static constexpr uint64_t PD2_TAPE_MAGIC = 0x3150415454324450ull;          // "PD2TTAP1"
 
-static long long pdr_elems(const int* ns, int nds) { long long n = 1; for (int i = 0; i < nds; i++) n *= ns[i]; return n; }
-
-// 256 + passes x two bitsets of n-element passes, in 64-bit arithmetic; 0 when that does not fit in size_t
-static size_t nd_tape_bytes(unsigned long long passes, long long n) {
-    const unsigned long long set2 = 2ull * (unsigned long long)ptvv::vjp_tape_set_bytes(n);
-    if (set2 && passes > (SIZE_MAX - 256) / set2) return 0;
-    return 256 + (size_t)(passes * set2);
+// What tells the three N-D tapes apart, by NdSolver: the magic, the refusal of another solver's tape, the default maxIters
+struct NdTapeKind { uint64_t magic; const char* not_ours; int default_iters; };
+static const NdTapeKind ND_TAPE[3] = {
+    {0x3150415454324450ull, "not a PD2_TV tape", MAX_ITERS_PD},             // "PD2TTAP1"
+    {0x3150415456544450ull, "not a PD_TV tape", MAX_ITERS_PD},              // "PDTVTAP1"
+    {0x3150415452524450ull, "not a PDR_TV tape", MAX_ITERS_DR},             // "PDRRTAP1"
+};
+// the capacity in iterations
+static int nd_cap(NdSolver s, int maxIters) { return maxIters <= 0 ? ND_TAPE[s].default_iters : maxIters; }
+// the iterations the recorded passes come from: PDR_TV runs its capacity, PD_TV and PD2_TV what their stop rule let run
+static int nd_K(NdSolver s, int maxIters, int iters) { return s == ND_PDR ? nd_cap(s, maxIters) : iters; }
+// the passes of K iterations that reach the output (sections 13 and 14)
+static unsigned long long nd_passes(NdSolver s, int npen, int K) {
+    const unsigned long long k = (unsigned long long)K;
+    switch (s) {
+    case ND_PD2: return npen == 1 ? (K > 0 ? 1 : 0) : 2 * k;
+    case ND_PD: return k * (unsigned long long)npen;
+    default: return (unsigned long long)(K - 1) * (unsigned long long)npen;
+    }
 }
 
-size_t pdr_tape_bytes(const int* ns, int nds, int npen, int maxIters) {
-    const int K = maxIters <= 0 ? MAX_ITERS_DR : maxIters;
-    return nd_tape_bytes((unsigned long long)(K - 1) * (unsigned long long)npen, pdr_elems(ns, nds));
+// 256 + passes x two bitsets of n-element passes, in 64-bit arithmetic; 0 when that does not fit in size_t
+size_t nd_tape_bytes(NdSolver s, const int* ns, int nds, int npen, int maxIters) {
+    NdTerms t;
+    nd_terms(ns, nds, 0, nullptr, &t);
+    const unsigned long long passes = nd_passes(s, npen, nd_cap(s, maxIters));
+    const unsigned long long set2 = 2ull * (unsigned long long)ptvv::vjp_tape_set_bytes(t.n);
+    if (set2 && passes > (SIZE_MAX - 256) / set2) return 0;
+    return 256 + (size_t)(passes * set2);
 }
 
 template <typename T> cudaError_t pdr_tape_pass(void* tape, long long n, long long p, const T* y, FiberGeom g, T lam, cudaStream_t st) {
@@ -540,29 +554,32 @@ template <typename T> cudaError_t pdr_tape_pass(void* tape, long long n, long lo
     return ptvv::fiber_tape<T>(y, g.nf, g.len, g.inc, lam, nullptr, F, F + sb / 4, st);
 }
 
-static PdrTapeHeader nd_header(uint64_t magic, size_t elem, const int* ns, int nds, int npen, const double* dims, int K, int cap) {
+// K: the iterations recorded; cap: the capacity (PDR_TV, whose K is its capacity: 0)
+static PdrTapeHeader nd_header(NdSolver s, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters, int iters) {
     PdrTapeHeader h;
     memset(&h, 0, sizeof(h));
-    h.magic = magic; h.elem = (int32_t)elem; h.K = K; h.npen = npen; h.nds = nds; h.cap = cap;
+    h.magic = ND_TAPE[s].magic; h.elem = (int32_t)elem; h.K = nd_K(s, maxIters, iters); h.npen = npen; h.nds = nds;
+    h.cap = s == ND_PDR ? 0 : nd_cap(s, maxIters);
     for (int i = 0; i < nds; i++) h.ns[i] = ns[i];
     for (int i = 0; i < npen; i++) h.axis[i] = (uint8_t)(int)(dims[i] - 1);
     return h;
 }
 
-cudaError_t pdr_tape_header(void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters, cudaStream_t st) {
-    const PdrTapeHeader h = nd_header(PDR_TAPE_MAGIC, elem, ns, nds, npen, dims, maxIters <= 0 ? MAX_ITERS_DR : maxIters, 0);
+cudaError_t nd_tape_header(NdSolver s, void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters, int iters,
+                           cudaStream_t st) {
+    const PdrTapeHeader h = nd_header(s, elem, ns, nds, npen, dims, maxIters, iters);
     return cudaMemcpyAsync(tape, &h, sizeof(h), cudaMemcpyHostToDevice, st);
 }
 
-// the header check of the three N-D tapes: magic (not_ours when it is not this solver's), dtype, shape, terms, capacity, K
-static const char* nd_tape_check(uint64_t magic, const char* not_ours, const void* tape, size_t elem, const int* ns, int nds, int npen,
-                                 const double* dims, int K, int cap, cudaStream_t st) {
+// magic (not_ours when it is not this solver's), dtype, shape, terms, capacity, K
+const char* nd_tape_check(NdSolver s, const void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters,
+                          int iters, cudaStream_t st) {
     PdrTapeHeader h;
     if (cudaMemcpyAsync(&h, tape, sizeof(h), cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) {
         cudaGetLastError(); return "cannot read the tape header";
     }
-    const PdrTapeHeader w = nd_header(magic, elem, ns, nds, npen, dims, K, cap);
-    if (h.magic != w.magic) return not_ours;
+    const PdrTapeHeader w = nd_header(s, elem, ns, nds, npen, dims, maxIters, iters);
+    if (h.magic != w.magic) return ND_TAPE[s].not_ours;
     if (h.elem != w.elem) return "tape recorded with another dtype";
     if (h.nds != w.nds || memcmp(h.ns, w.ns, sizeof(h.ns)) != 0) return "tape recorded for another shape";
     if (h.npen != w.npen || memcmp(h.axis, w.axis, sizeof(h.axis)) != 0) return "tape recorded with other penalty terms";
@@ -571,24 +588,39 @@ static const char* nd_tape_check(uint64_t magic, const char* not_ours, const voi
     return nullptr;
 }
 
-const char* pdr_tape_check(const void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters,
-                           cudaStream_t st) {
-    return nd_tape_check(PDR_TAPE_MAGIC, "not a PDR_TV tape", tape, elem, ns, nds, npen, dims, maxIters <= 0 ? MAX_ITERS_DR : maxIters, 0, st);
-}
+template <typename T> struct PdrvPtrs { T* gz[64]; };
 
-template <typename T> size_t ws_bytes_pdr_vjp(const int* ns, int nds, int npen, const double* dims, bool want_glam) {
-    const long long n = pdr_elems(ns, nds);
+// The backward workspace of the three solvers, in order: npen arrays a.gz (PD2_TV: gp, and gq when npen = 2), Sk (PD_TV: Gk; PD2_TV
+// with npen = 1: gq), h, sc, gw (only when glam is wanted), the VJP scratch of the largest term, the double sums.  Returns its size
+// and, unless ws is nullptr, splits ws into *L.
+template <typename T> struct NdVjpWs {
+    PdrvPtrs<T> a;
+    T *Sk, *h, *sc, *gw;
+    void* vscr;
+    double* scratch;
+};
+template <typename T> static size_t nd_vjp_ws(const NdTerms& t, int npen, bool want_glam, char* ws, NdVjpWs<T>* L) {
+    const size_t ab = al256((size_t)t.n * sizeof(T));
     size_t vs = 0;
     for (int i = 0; i < npen; i++) {
-        FiberGeom g{0, 0, 1};
-        geom_of(ns, nds, dims[i], n, &g);
-        const size_t b = ptvv::vjp_scratch_bytes(g.nf, g.len);
+        const size_t b = ptvv::vjp_scratch_bytes(t.g[i].nf, t.g[i].len);
         if (b > vs) vs = b;
     }
-    return (size_t)(npen + 3 + (want_glam ? 1 : 0)) * al256((size_t)n * sizeof(T)) + al256(vs) + DR2V_SCRATCH;
+    size_t off = 0;
+    auto take = [&](size_t bytes) { char* p = ws ? ws + off : nullptr; off += bytes; return p; };
+    for (int i = 0; i < npen; i++) L->a.gz[i] = (T*)take(ab);
+    L->Sk = (T*)take(ab);
+    L->h = (T*)take(ab);
+    L->sc = (T*)take(ab);
+    L->gw = want_glam ? (T*)take(ab) : nullptr;
+    L->vscr = take(al256(vs));
+    L->scratch = (double*)take(DR2V_SCRATCH);
+    return off;
 }
-
-template <typename T> struct PdrvPtrs { T* gz[64]; };
+template <typename T> size_t ws_bytes_nd_vjp(const NdTerms& t, int npen, bool want_glam) {
+    NdVjpWs<T> L;
+    return nd_vjp_ws<T>(t, npen, want_glam, nullptr, &L);
+}
 
 // start: v = G / kk, every gz_l = v.  Else the step after term i's VJP pass (result sc): gz_i = (gz_i - sk) + sc, then h = 2 sk - gz_{i+1}
 // for the next term.  After the last term (and at the start): s = (gz_0 + gz_1) + ... ; more: sk = s / kk, h = 2 sk - gz_0 ; else gY = s.
@@ -621,53 +653,6 @@ __global__ void k_pdrv(PdrvPtrs<T> a, int npen, int i, bool start, bool more, co
     }
 }
 
-template <typename T>
-cudaError_t pdr_vjp_device(const int* ns, int nds, int npen, const double* dims, int maxIters, const void* tape, const T* gout, T* gY,
-                           double* glam, void* ws, cudaStream_t st) {
-#define RTRY(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) return e__; } while (0)
-    const long long n = pdr_elems(ns, nds);
-    const int K = maxIters <= 0 ? MAX_ITERS_DR : maxIters;
-    if (glam) RTRY(cudaMemsetAsync(glam, 0, (size_t)npen * sizeof(double), st));
-    if (n == 0) return cudaSuccess;
-    const size_t ab = al256((size_t)n * sizeof(T)), sb = ptvv::vjp_tape_set_bytes(n);
-    FiberGeom g[64];
-    size_t vs = 0;
-    for (int i = 0; i < npen; i++) {
-        geom_of(ns, nds, dims[i], n, &g[i]);
-        const size_t b = ptvv::vjp_scratch_bytes(g[i].nf, g[i].len);
-        if (b > vs) vs = b;
-    }
-    char* w = (char*)ws;
-    PdrvPtrs<T> a;
-    for (int i = 0; i < npen; i++) { a.gz[i] = (T*)w; w += ab; }
-    T* Sk = (T*)w; w += ab;
-    T* h = (T*)w; w += ab;
-    T* sc = (T*)w; w += ab;
-    T* gw = nullptr;
-    if (glam) { gw = (T*)w; w += ab; }
-    void* vscr = w; w += al256(vs);
-    double* scratch = (double*)w;
-    const char* tb = (const char*)tape + 256;
-    const unsigned ge = ew_grid(n);
-    auto step = [&](bool start, int i, bool more) -> cudaError_t {
-        KernelSpan sp(KC_ELEMENTWISE, 1, st);
-        k_pdrv<T><<<ge, 256, 0, st>>>(a, npen, i, start, more, gout, sc, Sk, h, gY, n);
-        return cudaGetLastError();
-    };
-    RTRY(step(true, npen - 1, K >= 2));
-    for (int j = K - 2; j >= 0; j--) {
-        for (int i = 0; i < npen; i++) {
-            const uint32_t* F = (const uint32_t*)(tb + ((size_t)j * npen + i) * 2 * sb);
-            RTRY(ptvv::vjp_fibers_tape<T>(F, F + sb / 4, h, sc, gw, g[i].nf, g[i].len, g[i].inc, vscr, st));
-            // one "image" of all edges: img_sums adds its sum to glam[2 * 0 + i]
-            if (glam) RTRY(img_sums<T>(gw, g[i].nf * (long long)(g[i].len - 1), 1, scratch, nullptr, glam, i, 1.0, st));
-            RTRY(step(false, i, j > 0));
-        }
-    }
-    return cudaSuccess;
-#undef RTRY
-}
-
 // ================================================================ PD_TV and PD2_TV (DESIGN.md section 14)
 // Both are the solvers of solver.cu themselves; the function differentiated is K iterations, K = the count the forward ran (info[0],
 // the header's K): the stop test only picks K.  P_i is the 1D prox along axis dims[i], S_{j,i} its segment-mean Jacobian.
@@ -685,27 +670,6 @@ cudaError_t pdr_vjp_device(const int* ns, int nds, int npen, const double* dims,
 //                  gu = S_0(h) ; gp = gp + gu ; j > 0: h = gp - gq ; j = 0: gY = gp                           (mode 2)
 // Penalty gradients: glam_i = 0.0 ; glam_i = glam_i + sum(gw) per pass of term i in backward order, gw the pass's edge gradients for
 // its upstream gradient h, each sum img_sums' fixed two-stage double sum.  No atomics.
-static int pd_cap(int maxIters) { return maxIters <= 0 ? MAX_ITERS_PD : maxIters; }
-static unsigned long long pd_passes(bool pd2, int npen, int K) {
-    const unsigned long long k = (unsigned long long)K;
-    return pd2 ? (npen == 1 ? (K > 0 ? 1 : 0) : 2 * k) : k * (unsigned long long)npen;
-}
-
-size_t pd_tape_bytes(bool pd2, const int* ns, int nds, int npen, int maxIters) {
-    return nd_tape_bytes(pd_passes(pd2, npen, pd_cap(maxIters)), pdr_elems(ns, nds));
-}
-
-cudaError_t pd_tape_header(bool pd2, void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters, int iters,
-                           cudaStream_t st) {
-    const PdrTapeHeader h = nd_header(pd2 ? PD2_TAPE_MAGIC : PD_TAPE_MAGIC, elem, ns, nds, npen, dims, iters, pd_cap(maxIters));
-    return cudaMemcpyAsync(tape, &h, sizeof(h), cudaMemcpyHostToDevice, st);
-}
-
-const char* pd_tape_check(bool pd2, const void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters,
-                          int iters, cudaStream_t st) {
-    return nd_tape_check(pd2 ? PD2_TAPE_MAGIC : PD_TAPE_MAGIC, pd2 ? "not a PD2_TV tape" : "not a PD_TV tape", tape, elem, ns, nds, npen,
-                         dims, iters, pd_cap(maxIters), st);
-}
 
 // start: every a_l = 0, gk = G / kk, h = gk - a_0.  Else the step after term i's VJP pass (result sc): a_i = a_i + sc, then h = gk - a_{i+1}
 // for the next term; after the last term s = (a_0 + a_1) + ... ; more: gk = s / kk, h = gk - a_0 ; else gY = s.
@@ -758,44 +722,43 @@ __global__ void k_pd2v(int mode, bool more, const T* __restrict__ G, const T* __
 }
 
 template <typename T>
-cudaError_t pd_vjp_device(bool pd2, const int* ns, int nds, int npen, const double* dims, int iters, const void* tape, const T* gout, T* gY,
+cudaError_t nd_vjp_device(NdSolver s, const NdTerms& t, int npen, int maxIters, int iters, const void* tape, const T* gout, T* gY,
                           double* glam, void* ws, cudaStream_t st) {
 #define RTRY(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) return e__; } while (0)
-    const long long n = pdr_elems(ns, nds);
-    const int K = iters;
+    const long long n = t.n;
+    const int K = nd_K(s, maxIters, iters);
     if (glam) RTRY(cudaMemsetAsync(glam, 0, (size_t)npen * sizeof(double), st));
     if (n == 0 || K <= 0) return cudaSuccess;
-    const size_t ab = al256((size_t)n * sizeof(T)), sb = ptvv::vjp_tape_set_bytes(n);
-    FiberGeom g[64];
-    size_t vs = 0;
-    for (int i = 0; i < npen; i++) {
-        geom_of(ns, nds, dims[i], n, &g[i]);
-        const size_t b = ptvv::vjp_scratch_bytes(g[i].nf, g[i].len);
-        if (b > vs) vs = b;
-    }
-    char* w = (char*)ws;                       // the layout of ws_bytes_pdr_vjp: npen + 3 arrays (PD2_TV uses 4), gw, VJP scratch, sums
-    PdrvPtrs<T> a;
-    for (int i = 0; i < npen; i++) { a.gz[i] = (T*)w; w += ab; }
-    T* Gk = (T*)w; w += ab;
-    T* h = (T*)w; w += ab;
-    T* sc = (T*)w; w += ab;
-    T* gw = nullptr;
-    if (glam) { gw = (T*)w; w += ab; }
-    void* vscr = w; w += al256(vs);
-    double* scratch = (double*)w;
+    NdVjpWs<T> L;
+    nd_vjp_ws<T>(t, npen, glam != nullptr, (char*)ws, &L);
+    const size_t sb = ptvv::vjp_tape_set_bytes(n);
     const char* tb = (const char*)tape + 256;
     const unsigned ge = ew_grid(n);
     // the VJP of pass p (term i) for the upstream h into sc, and its edge gradients into glam[i]
     auto pass = [&](long long p, int i) -> cudaError_t {
+        const FiberGeom& g = t.g[i];
         const uint32_t* F = (const uint32_t*)(tb + (size_t)p * 2 * sb);
-        RTRY(ptvv::vjp_fibers_tape<T>(F, F + sb / 4, h, sc, gw, g[i].nf, g[i].len, g[i].inc, vscr, st));
-        if (glam) RTRY(img_sums<T>(gw, g[i].nf * (long long)(g[i].len - 1), 1, scratch, nullptr, glam, i, 1.0, st));
+        RTRY(ptvv::vjp_fibers_tape<T>(F, F + sb / 4, L.h, L.sc, L.gw, g.nf, g.len, g.inc, L.vscr, st));
+        // one "image" of all edges: img_sums adds its sum to glam[2 * 0 + i]
+        if (glam) RTRY(img_sums<T>(L.gw, g.nf * (long long)(g.len - 1), 1, L.scratch, nullptr, glam, i, 1.0, st));
         return cudaSuccess;
     };
-    if (!pd2) {
+    if (s == ND_PDR) {
         auto step = [&](bool start, int i, bool more) -> cudaError_t {
             KernelSpan sp(KC_ELEMENTWISE, 1, st);
-            k_pdv<T><<<ge, 256, 0, st>>>(a, npen, i, start, more, gout, sc, Gk, h, gY, n);
+            k_pdrv<T><<<ge, 256, 0, st>>>(L.a, npen, i, start, more, gout, L.sc, L.Sk, L.h, gY, n);
+            return cudaGetLastError();
+        };
+        RTRY(step(true, npen - 1, K >= 2));
+        for (int j = K - 2; j >= 0; j--)
+            for (int i = 0; i < npen; i++) {
+                RTRY(pass((long long)j * npen + i, i));
+                RTRY(step(false, i, j > 0));
+            }
+    } else if (s == ND_PD) {
+        auto step = [&](bool start, int i, bool more) -> cudaError_t {
+            KernelSpan sp(KC_ELEMENTWISE, 1, st);
+            k_pdv<T><<<ge, 256, 0, st>>>(L.a, npen, i, start, more, gout, L.sc, L.Sk, L.h, gY, n);
             return cudaGetLastError();
         };
         RTRY(step(true, 0, true));
@@ -805,11 +768,11 @@ cudaError_t pd_vjp_device(bool pd2, const int* ns, int nds, int npen, const doub
                 RTRY(step(false, i, j > 0));
             }
     } else {
-        T* gp = a.gz[0];                       // npen + 3 >= 4 arrays: gp, gq (= Gk's slot when npen = 1), h, sc
-        T* gq = npen >= 2 ? a.gz[1] : Gk;
+        T* gp = L.a.gz[0];
+        T* gq = npen >= 2 ? L.a.gz[1] : L.Sk;
         auto step = [&](int mode, bool more) -> cudaError_t {
             KernelSpan sp(KC_ELEMENTWISE, 1, st);
-            k_pd2v<T><<<ge, 256, 0, st>>>(mode, more, gout, sc, gp, gq, h, gY, n);
+            k_pd2v<T><<<ge, 256, 0, st>>>(mode, more, gout, L.sc, gp, gq, L.h, gY, n);
             return cudaGetLastError();
         };
         RTRY(step(0, true));
@@ -828,10 +791,8 @@ cudaError_t pd_vjp_device(bool pd2, const int* ns, int nds, int npen, const doub
 
 #define INST(T) \
     template cudaError_t pdr_tape_pass<T>(void*, long long, long long, const T*, FiberGeom, T, cudaStream_t); \
-    template size_t ws_bytes_pdr_vjp<T>(const int*, int, int, const double*, bool); \
-    template cudaError_t pdr_vjp_device<T>(const int*, int, int, const double*, int, const void*, const T*, T*, double*, void*, cudaStream_t); \
-    template cudaError_t pd_vjp_device<T>(bool, const int*, int, int, const double*, int, const void*, const T*, T*, double*, void*, \
-                                          cudaStream_t); \
+    template size_t ws_bytes_nd_vjp<T>(const NdTerms&, int, bool); \
+    template cudaError_t nd_vjp_device<T>(NdSolver, const NdTerms&, int, int, int, const void*, const T*, T*, double*, void*, cudaStream_t); \
     template size_t ws_bytes_dr2_record<T>(size_t, size_t, int); \
     template size_t ws_bytes_dr2_vjp<T>(size_t, size_t, int); \
     template cudaError_t dr2_record_device<T>(size_t, size_t, int, int, const T*, T, T, T*, int, void*, void*, Engine, cudaStream_t); \

@@ -116,6 +116,17 @@ template <typename T> struct DrwPasses {
     cudaError_t init(size_t M, size_t N, int batch, int row_major, const T* W1, const T* W2, Engine eng, void* stage, cudaStream_t st);
     cudaError_t run(int axis, const T* A, const T* B, const T* C, InOp op, T* X, int out_op, cudaStream_t st);
 };
+// ---- the N-D solvers PD2_TV, PD_TV, PDR_TV (solver.cu; backward passes in dr2_vjp.cu) ----
+enum NdSolver { ND_PD2 = 0, ND_PD = 1, ND_PDR = 2 };
+// The element count of a column-major array of dims ns[0..nds) and the fibers of each penalty term along it
+struct NdTerms {
+    long long n;
+    FiberGeom g[64];
+};
+// Fills t: n, then the fibers of term i along its 1-based axis dims[i] (npen = 0: n only).  nullptr when every axis is valid, else the
+// reason: more than 64 terms (no fibers filled) or an axis outside 1..nds.
+const char* nd_terms(const int* ns, int nds, int npen, const double* dims, NdTerms* t);
+// the forward workspace of the three N-D solvers for n elements and npen terms
 template <typename T> size_t ws_bytes_pd(long long n, int npen);
 // PD2_TV / PD_TV (proximal Dykstra, stop rule mean|x - x_old| <= STOP_PD).  tape: nullptr, or the recorded forward's buffer (header
 // written by the caller after the call, from info[0]): the segmentation tape of every pass
@@ -167,34 +178,26 @@ template <typename T> cudaError_t drw_vjp_device(size_t M, size_t N, int batch, 
 template <typename T> int pdr_device(const T* y, const double* lambdas_scaled, const double* dims, T* x, double* info,
                                      const int* ns, int nds, int npen, int maxIters, void* ws, Engine eng, cudaStream_t st,
                                      void* tape = nullptr);
-// the fibers of an n-element column-major array of dims ns[0..nds) along the 1-based axis `dim`; false when dim is not an axis
-bool geom_of(const int* ns, int nds, double dim, long long n, FiberGeom* g);
-// ---- exact backward pass of PDR_TV (dr2_vjp.cu, DESIGN.md section 13) ----
+// ---- exact backward passes of the N-D solvers (dr2_vjp.cu, DESIGN.md sections 13 and 14) ----
+// The tape of a recorded forward: a 256-byte header, then the segmentation tape of each pass that reaches the output.  maxIters <= 0
+// means the solver's default (35).  PDR_TV runs K = maxIters iterations and records the (K - 1) npen passes of all but the last; PD_TV
+// and PD2_TV stop early, so their tape holds the capacity of maxIters iterations -- maxIters npen passes (PD_TV), 2 maxIters (PD2_TV; 1
+// when npen = 1) -- and the header the iterations run, `iters` (info[0]; ignored for PDR_TV).
 constexpr int PDR_TAPE_MAX_DIMS = 16;                                    // axes the tape header holds
-size_t pdr_tape_bytes(const int* ns, int nds, int npen, int maxIters);    // header + (K - 1) npen passes x two bitsets; 0: too large
+// header + passes x two bitsets; 0 when the byte count does not fit in size_t
+size_t nd_tape_bytes(NdSolver s, const int* ns, int nds, int npen, int maxIters);
 // the tape of pass p (output y over the fibers g, penalty lam) into a tape of n-element passes
 template <typename T> cudaError_t pdr_tape_pass(void* tape, long long n, long long p, const T* y, FiberGeom g, T lam, cudaStream_t st);
-// writes the 256-byte header (arguments checked by the caller; axes = dims - 1)
-cudaError_t pdr_tape_header(void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters, cudaStream_t st);
+// writes the 256-byte header after the solve (arguments checked by the caller; axes = dims - 1)
+cudaError_t nd_tape_header(NdSolver s, void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters, int iters,
+                           cudaStream_t st);
 // validates a tape's header against the arguments (one stream synchronisation): nullptr ok, else the reason
-const char* pdr_tape_check(const void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters,
-                           cudaStream_t st);
-template <typename T> size_t ws_bytes_pdr_vjp(const int* ns, int nds, int npen, const double* dims, bool want_glam);
-// gY, and glam[npen] (d/d of the scaled penalties) unless nullptr, from the tape alone; arguments checked by the caller
-template <typename T> cudaError_t pdr_vjp_device(const int* ns, int nds, int npen, const double* dims, int maxIters, const void* tape,
-                                                 const T* gout, T* gY, double* glam, void* ws, cudaStream_t st);
-// ---- exact backward passes of PD_TV and PD2_TV (dr2_vjp.cu, DESIGN.md section 14); pd2 selects PD2_TV ----
-// header + the capacity of maxIters (0: 35) iterations: maxIters npen passes (PD_TV), 2 maxIters (PD2_TV; 1 when npen = 1); 0 when
-// the byte count does not fit in size_t
-size_t pd_tape_bytes(bool pd2, const int* ns, int nds, int npen, int maxIters);
-// writes the 256-byte header after the solve: capacity maxIters, iters = the iterations run (info[0])
-cudaError_t pd_tape_header(bool pd2, void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters, int iters,
-                           cudaStream_t st);
-const char* pd_tape_check(bool pd2, const void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters,
+const char* nd_tape_check(NdSolver s, const void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters,
                           int iters, cudaStream_t st);
-// gY, and glam[npen] unless nullptr (PD_TV: d/d of the scaled penalties; PD2_TV: of the penalties as given), from the tape of a solve
-// that ran `iters` iterations; arguments checked by the caller; workspace ws_bytes_pdr_vjp
-template <typename T> cudaError_t pd_vjp_device(bool pd2, const int* ns, int nds, int npen, const double* dims, int iters, const void* tape,
+template <typename T> size_t ws_bytes_nd_vjp(const NdTerms& t, int npen, bool want_glam);
+// gY, and glam[npen] unless nullptr (PD_TV / PDR_TV: d/d of the scaled penalties; PD2_TV: of the penalties as given), from the tape
+// alone; arguments checked by the caller; workspace ws_bytes_nd_vjp
+template <typename T> cudaError_t nd_vjp_device(NdSolver s, const NdTerms& t, int npen, int maxIters, int iters, const void* tape,
                                                 const T* gout, T* gY, double* glam, void* ws, cudaStream_t st);
 
 }  // namespace ptv

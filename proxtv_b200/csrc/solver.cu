@@ -497,13 +497,19 @@ template <typename T> size_t ws_bytes_pd(long long n, int npen) {
     return (size_t)arrays * align256((size_t)n * sizeof(T)) + SCRATCH_BYTES + align256(2 * 64 * sizeof(void*));
 }
 
-bool geom_of(const int* ns, int nds, double dim, long long n, FiberGeom* g) {
-    int d = (int)(dim - 1);                                                   // TV2Dopt.cpp:171, TVNDopt.cpp:175
-    if (d < 0 || d >= nds) return false;
-    long long inc = 1;
-    for (int i = 0; i < d; i++) inc *= ns[i];                                 // TVNDopt.cpp:133-138
-    g->len = ns[d]; g->inc = inc; g->nf = ns[d] ? n / ns[d] : 0;
-    return true;
+const char* nd_terms(const int* ns, int nds, int npen, const double* dims, NdTerms* t) {
+    long long n = 1;
+    for (int i = 0; i < nds; i++) n *= ns[i];
+    t->n = n;
+    if (npen > 64) return "more than 64 penalty terms are not supported";
+    for (int i = 0; i < npen; i++) {
+        const int d = (int)(dims[i] - 1);                                     // TV2Dopt.cpp:171, TVNDopt.cpp:175
+        if (d < 0 || d >= nds) return "invalid penalty dimensions";
+        long long inc = 1;
+        for (int a = 0; a < d; a++) inc *= ns[a];                             // TVNDopt.cpp:133-138
+        t->g[i] = FiberGeom{ns[d] ? n / ns[d] : 0, ns[d], inc};
+    }
+    return nullptr;
 }
 
 static int read_stop(const double* dres, double* stop, cudaStream_t st) {
@@ -519,12 +525,14 @@ int pd2_device(const T* y, const double* lambdas, const double* dims, T* x, doub
                int maxIters, void* ws, Engine eng, cudaStream_t st, void* tape) {
     if (npen > 2) { printf("PD2_TV: this algorithm can not work with more than 2 penalties\n");      // :95-96
                     if (info) info[INFO_RC] = RC_ERROR; return 0; }
-    long long n = 1; for (int i = 0; i < nds; i++) n *= ns[i];
+    NdTerms t;
+    const char* why = nd_terms(ns, nds, npen, dims, &t);
+    const long long n = t.n;
     if (maxIters <= 0) maxIters = MAX_ITERS_PD;
     if (npen >= 1) eng = lane_guard<T>(eng, y, n, npen >= 2 && lambdas[1] > lambdas[0] ? lambdas[1] : lambdas[0], st);
-    FiberGeom g0{0, 0, 1}, g1{0, 0, 1};
-    if (npen < 1 || !geom_of(ns, nds, dims[0], n, &g0) || (npen >= 2 && !geom_of(ns, nds, dims[1], n, &g1))) {
-        printf("PD2_TV: invalid penalty dimensions\n"); if (info) info[INFO_RC] = RC_ERROR; return 0; }
+    if (npen < 1 || why) { printf("PD2_TV: invalid penalty dimensions\n"); if (info) info[INFO_RC] = RC_ERROR; return 0; }
+    const FiberGeom& g0 = t.g[0];
+    const FiberGeom& g1 = t.g[1];                    // npen >= 2 only
     double stop = DBL_MAX; int iters = 0;
     if (n > 0) {
         char* w = (char*)ws; const size_t ab = align256((size_t)n * sizeof(T));
@@ -556,40 +564,61 @@ int pd2_device(const T* y, const double* lambdas, const double* dims, T* x, doub
     return 1;
 }
 
+// The checks PD_TV and PDR_TV share, in this order: the term count; the lane guard over the largest penalty; the axes.  Refused:
+// "<name>: <reason>" on stdout, info[RC] = RC_ERROR, false.
+template <typename T>
+static bool pd_start(const char* name, const T* y, const double* lam, const double* dims, double* info, const int* ns, int nds, int npen,
+                     NdTerms* t, Engine* eng, cudaStream_t st) {
+    const char* why = nd_terms(ns, nds, npen, dims, t);
+    if (npen <= 64) {
+        double lmax = 0.0; for (int i = 0; i < npen; i++) if (lam[i] > lmax) lmax = lam[i];
+        *eng = lane_guard<T>(*eng, y, t->n, lmax, st);
+    }
+    if (why) { printf("%s: %s\n", name, why); if (info) info[INFO_RC] = RC_ERROR; return false; }
+    return true;
+}
+
+// The workspace of pd_device and pdr_device (ws_bytes_pd): p_i and z_i of each term interleaved, the staging of strided passes (2
+// arrays + per-chunk masks / entering values), the reduction scratch, then the device tables dp / dz of the p_i / z_i.
+template <typename T> struct PdWs {
+    T* hp[64]; T* hz[64];
+    T* scr; double* scratch; double* dres;
+    T** dp; T** dz;
+};
+template <typename T> static cudaError_t pd_ws(void* ws, long long n, int npen, PdWs<T>* W, cudaStream_t st) {
+    char* w = (char*)ws; const size_t ab = align256((size_t)n * sizeof(T));
+    for (int i = 0; i < npen; i++) { W->hp[i] = (T*)w; w += ab; W->hz[i] = (T*)w; w += ab; }
+    W->scr = (T*)w; w += 3 * ab;
+    W->scratch = (double*)w; W->dres = W->scratch + REDUCE_BLOCKS; w += SCRATCH_BYTES;
+    W->dp = (T**)w; W->dz = W->dp + 64;
+    cudaError_t e = cudaMemcpyAsync(W->dp, W->hp, sizeof(T*) * npen, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(W->dz, W->hz, sizeof(T*) * npen, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);    // W lives on the host stack
+    return e;
+}
+
 // tape != nullptr (the recorded forward, dr2_vjp.cu): after each pass the segmentation tape of its output p_i is written as pass
 // iters * npen + i; nothing else changes.
 template <typename T>
 int pd_device(const T* y, const double* lam, const double* dims, T* x, double* info, const int* ns, int nds, int npen,
               int maxIters, void* ws, Engine eng, cudaStream_t st, void* tape) {
-    long long n = 1; for (int i = 0; i < nds; i++) n *= ns[i];
     if (maxIters <= 0) maxIters = MAX_ITERS_PD;
-    if (npen > 64) { printf("PD_TV: more than 64 penalty terms are not supported\n"); if (info) info[INFO_RC] = RC_ERROR; return 0; }
-    { double lmax = 0.0; for (int i = 0; i < npen; i++) if (lam[i] > lmax) lmax = lam[i];
-      eng = lane_guard<T>(eng, y, n, lmax, st); }
-    FiberGeom g[64];
-    for (int i = 0; i < npen; i++)
-        if (!geom_of(ns, nds, dims[i], n, &g[i])) { printf("PD_TV: invalid penalty dimensions\n");
-                                                     if (info) info[INFO_RC] = RC_ERROR; return 0; }
+    NdTerms t;
+    if (!pd_start<T>("PD_TV", y, lam, dims, info, ns, nds, npen, &t, &eng, st)) return 0;
+    const long long n = t.n;
     double stop = DBL_MAX; int iters = 0;
     if (n > 0 && npen > 0) {
-        char* w = (char*)ws; const size_t ab = align256((size_t)n * sizeof(T));
-        T* hp[64]; T* hz[64];
-        for (int i = 0; i < npen; i++) { hp[i] = (T*)w; w += ab; hz[i] = (T*)w; w += ab; }
-        T* scr = (T*)w; w += 3 * ab;
-        double* scratch = (double*)w; double* dres = scratch + REDUCE_BLOCKS; w += SCRATCH_BYTES;
-        T** dp = (T**)w; T** dz = dp + 64;
-        PTV_TRY(cudaMemcpyAsync(dp, hp, sizeof(T*) * npen, cudaMemcpyHostToDevice, st));
-        PTV_TRY(cudaMemcpyAsync(dz, hz, sizeof(T*) * npen, cudaMemcpyHostToDevice, st));
-        PTV_TRY(cudaStreamSynchronize(st));    // hp/hz are stack arrays
+        PdWs<T> W;
+        PTV_TRY(pd_ws<T>(ws, n, npen, &W, st));
         PTV_TRY(cudaMemsetAsync(x, 0, (size_t)n * sizeof(T), st));                                    // :125-130
-        for (int i = 0; i < npen; i++) PTV_TRY(cudaMemcpyAsync(hz[i], y, (size_t)n * sizeof(T), cudaMemcpyDeviceToDevice, st));
+        for (int i = 0; i < npen; i++) PTV_TRY(cudaMemcpyAsync(W.hz[i], y, (size_t)n * sizeof(T), cudaMemcpyDeviceToDevice, st));
         while (stop > STOP_PD && iters < maxIters) {                                                  // :151
             for (int i = 0; i < npen; i++) {
-                PTV_TRY(prox_fibers<T>(hz[i], nullptr, IN_A, hp[i], 0, g[i], (T)lam[i], nullptr, eng, scr, st, 3 * n));  // :171-208
-                if (tape) PTV_TRY(pdr_tape_pass<T>(tape, n, (long long)iters * npen + i, hp[i], g[i], (T)lam[i], st));
+                PTV_TRY(prox_fibers<T>(W.hz[i], nullptr, IN_A, W.hp[i], 0, t.g[i], (T)lam[i], nullptr, eng, W.scr, st, 3 * n));  // :171-208
+                if (tape) PTV_TRY(pdr_tape_pass<T>(tape, n, (long long)iters * npen + i, W.hp[i], t.g[i], (T)lam[i], st));
             }
-            PTV_TRY(ew_pd_combine<T>(dp, dz, hp, hz, npen, x, n, scratch, dres, st));                         // :212-227
-            if (!read_stop(dres, &stop, st)) { PTV_TRY(cudaGetLastError()); PTV_TRY(cudaErrorUnknown); }
+            PTV_TRY(ew_pd_combine<T>(W.dp, W.dz, W.hp, W.hz, npen, x, n, W.scratch, W.dres, st));             // :212-227
+            if (!read_stop(W.dres, &stop, st)) { PTV_TRY(cudaGetLastError()); PTV_TRY(cudaErrorUnknown); }
             iters++;
         }
     } else if (n > 0) {
@@ -611,37 +640,26 @@ int pd_device(const T* y, const double* lam, const double* dims, T* x, double* i
 template <typename T>
 int pdr_device(const T* y, const double* lam, const double* dims, T* x, double* info, const int* ns, int nds, int npen,
                int maxIters, void* ws, Engine eng, cudaStream_t st, void* tape) {
-    long long n = 1; for (int i = 0; i < nds; i++) n *= ns[i];
     if (maxIters <= 0) maxIters = MAX_ITERS_DR;                                                       // :320
-    if (npen > 64) { printf("PDR_TV: more than 64 penalty terms are not supported\n"); if (info) info[INFO_RC] = RC_ERROR; return 0; }
-    { double lmax = 0.0; for (int i = 0; i < npen; i++) if (lam[i] > lmax) lmax = lam[i];
-      eng = lane_guard<T>(eng, y, n, lmax, st); }
-    FiberGeom g[64];
-    for (int i = 0; i < npen; i++)
-        if (!geom_of(ns, nds, dims[i], n, &g[i])) { printf("PDR_TV: invalid penalty dimensions\n");
-                                                     if (info) info[INFO_RC] = RC_ERROR; return 0; }
+    NdTerms t;
+    if (!pd_start<T>("PDR_TV", y, lam, dims, info, ns, nds, npen, &t, &eng, st)) return 0;
+    const long long n = t.n;
     double stop = 0; int iters = 0;
     if (n > 0 && npen > 0) {
-        char* w = (char*)ws; const size_t ab = align256((size_t)n * sizeof(T));
-        T* hp[64]; T* hz[64];
-        for (int i = 0; i < npen; i++) { hp[i] = (T*)w; w += ab; hz[i] = (T*)w; w += ab; }
-        T* scr = (T*)w; w += 3 * ab;
-        double* scratch = (double*)w; double* dres = scratch + REDUCE_BLOCKS; w += SCRATCH_BYTES;
-        T** dp = (T**)w; T** dz = dp + 64;
-        PTV_TRY(cudaMemcpyAsync(dp, hp, sizeof(T*) * npen, cudaMemcpyHostToDevice, st));
-        PTV_TRY(cudaMemcpyAsync(dz, hz, sizeof(T*) * npen, cudaMemcpyHostToDevice, st));
-        PTV_TRY(cudaStreamSynchronize(st));    // hp/hz are stack arrays
+        PdWs<T> W;
+        PTV_TRY(pd_ws<T>(ws, n, npen, &W, st));
         PTV_TRY(ew_div_scalar<T>(y, x, n, (T)npen, st));                                              // :365-370
-        for (int i = 0; i < npen; i++) PTV_TRY(cudaMemcpyAsync(hz[i], y, (size_t)n * sizeof(T), cudaMemcpyDeviceToDevice, st));
+        for (int i = 0; i < npen; i++) PTV_TRY(cudaMemcpyAsync(W.hz[i], y, (size_t)n * sizeof(T), cudaMemcpyDeviceToDevice, st));
         while (iters < maxIters) {                                                                    // :394
             for (int i = 0; i < npen; i++) {
-                PTV_TRY(prox_fibers<T>(hz[i], nullptr, IN_A, hp[i], 0, g[i], (T)lam[i], nullptr, eng, scr, st, 3 * n));  // :409-449
-                if (tape && iters < maxIters - 1) PTV_TRY(pdr_tape_pass<T>(tape, n, (long long)iters * npen + i, hp[i], g[i], (T)lam[i], st));
+                PTV_TRY(prox_fibers<T>(W.hz[i], nullptr, IN_A, W.hp[i], 0, t.g[i], (T)lam[i], nullptr, eng, W.scr, st, 3 * n));  // :409-449
+                if (tape && iters < maxIters - 1)
+                    PTV_TRY(pdr_tape_pass<T>(tape, n, (long long)iters * npen + i, W.hp[i], t.g[i], (T)lam[i], st));
             }
-            PTV_TRY(ew_pdr_combine<T>(dp, dz, hp, hz, npen, x, n, scratch, dres, st));                        // :456-475
+            PTV_TRY(ew_pdr_combine<T>(W.dp, W.dz, W.hp, W.hz, npen, x, n, W.scratch, W.dres, st));            // :456-475
             iters++;
         }
-        if (iters > 0 && !read_stop(dres, &stop, st)) { PTV_TRY(cudaGetLastError()); PTV_TRY(cudaErrorUnknown); }
+        if (iters > 0 && !read_stop(W.dres, &stop, st)) { PTV_TRY(cudaGetLastError()); PTV_TRY(cudaErrorUnknown); }
     } else if (n > 0) {
         PTV_TRY(cudaMemsetAsync(x, 0, (size_t)n * sizeof(T), st));
         iters = maxIters;
