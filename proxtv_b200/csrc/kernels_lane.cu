@@ -101,7 +101,10 @@ template <typename T, int OP> struct PassOp {
     // what a lane scans, from the landed tiles (staged forms only; every other form scans A as it is)
     static __device__ __forceinline__ T in(T a, T b, T c) {
         if (!OpTraits<OP>::staged) return a;
-        const T d = c - b;                                   // t - prox_cols(t)              (src/TV2Dopt.cpp:545-546)
+        return in_d(a, c - b, c);                            // d = t - prox_cols(t)          (src/TV2Dopt.cpp:545-546)
+    }
+    // the same from d = c - b, rounded once (the landing keeps it for the drain: out_d)
+    static __device__ __forceinline__ T in_d(T a, T d, T c) {
         if (OP == LOP_DR_B) return a - (T(2) * d - c);       // Y - s, s = 2 (t - x) - t      (:411, :515)
         return a - d;                                        // final: s = t - x              (:427)
     }
@@ -113,6 +116,37 @@ template <typename T, int OP> struct PassOp {
         else if (OP == LOP_DRA_FINAL) o1 = b - (c - x);      // u = Y - (t - x_cols)          (:427)
         else if (OP == LOP_DRB) o1 = b + x;                  // b = d: t' = (t - x_cols) + x_rows
         else o1 = x;
+    }
+    // LOP_DR_B from the d the landing computed: (c - b) + x above, on the same rounded c - b
+    static __device__ __forceinline__ T out_d(T x, T d) { return d + x; }
+};
+
+// d = t - x1 of the staged row pass (LOP_DR_B), carried in registers from the landing of a tile to its drain instead of being read
+// again from global memory.  One slot of 8 values per lane and tile slot of the window (W / 8 slots), indexed by the ABSOLUTE tile
+// index row0 / 8 -- the window's ring position: halo tiles and tiles past the chunk's end are landed but never drained, so
+// push / pop counters would drift -- and the window itself keeps a slot from being landed again before its rows are swept (a tile
+// is requested only when row_req + 8 <= row_lo + W, and row_lo <= the next row to sweep).  The slot is warp-uniform; every access
+// goes through at(), whose cases name the slot's registers at compile time, so that the ring stays in registers.  512 bytes per
+// lane (128 registers) for float64 with a 64-row window and float32 with a 128-row one; larger rings keep the re-reading drain.
+template <typename T, int W, int OP> struct DRing {
+    static constexpr int NS = W / 8;
+    static constexpr bool on = OP == LOP_DR_B && NS * 8 * (int)sizeof(T) <= 512;
+    T d[on ? NS : 1][8];
+    __device__ __forceinline__ static unsigned slot(int row0) { return ((unsigned)row0 / 8u) % (unsigned)NS; }
+    // f(d[k]) for the slot k of the tile at row0: one case per slot, each with its own copy of f working on its own registers, so
+    // that selecting the slot is a jump (the whole landing combine or drain store of a tile is inside f: a body too large to be
+    // turned into selects over every slot, which a bare copy in and out of the ring would be)
+    template <class F> __device__ __forceinline__ void at(int row0, F f) {
+        if constexpr (on) {
+#define PTV_RING_CASE(k) case k: if constexpr (k < NS) f(d[k < NS ? k : 0]); break;
+            switch (slot(row0)) {
+                PTV_RING_CASE(0) PTV_RING_CASE(1) PTV_RING_CASE(2) PTV_RING_CASE(3) PTV_RING_CASE(4) PTV_RING_CASE(5) PTV_RING_CASE(6)
+                PTV_RING_CASE(7) PTV_RING_CASE(8) PTV_RING_CASE(9) PTV_RING_CASE(10) PTV_RING_CASE(11) PTV_RING_CASE(12) PTV_RING_CASE(13)
+                PTV_RING_CASE(14) PTV_RING_CASE(15)
+                default: break;
+            }
+#undef PTV_RING_CASE
+        }
     }
 };
 
@@ -237,7 +271,10 @@ template <typename T, int W, int RT, int OP> struct FeedStrided {
     static constexpr int NST = 2;                       // staging tiles for the B / C operands of the fused forms
     static constexpr int MAXQ = OpTraits<OP>::staged ? NST : W / RT;
     static constexpr int NBAR = W / RT;
+    using Ring = DRing<T, W, OP>;
+    static_assert(!Ring::on || RT == 8, "the d ring holds one 8-row drain group per tile");
     const LaneArgs<T>* a; T* win; T* stB; T* stC; uint64_t* bar; int x0, z, q0, lane;
+    Ring* ring;                                         // d = t - x1 of the landed tiles (Ring::on), read by the drain
     template <class Env> __device__ __forceinline__ void request(Env&, int row0) {
         __syncwarp();
         if (lane == 0) {
@@ -250,8 +287,14 @@ template <typename T, int W, int RT, int OP> struct FeedStrided {
             if (OP == LOP_DRA || OP == LOP_DRA_FINAL) tma_load_3d(win + ((row0 & (W - 1)) << 5), &a->tmA, x0, row0, z, b);
             else tma_load_3d_hint(win + ((row0 & (W - 1)) << 5), &a->tmA, x0, row0, z, b, policy_evict_first());
             if (OpTraits<OP>::staged) {
-                tma_load_3d(stB + (q % NST) * R * LANES, &a->tmB, x0, row0, z, b);
-                tma_load_3d(stC + (q % NST) * R * LANES, &a->tmC, x0, row0, z, b);
+                // with the d ring the drain does not come back for B and C either (LOP_DR_B_FINAL never does): single use
+                if (Ring::on || OP == LOP_DR_B_FINAL) {
+                    tma_load_3d_hint(stB + (q % NST) * R * LANES, &a->tmB, x0, row0, z, b, policy_evict_first());
+                    tma_load_3d_hint(stC + (q % NST) * R * LANES, &a->tmC, x0, row0, z, b, policy_evict_first());
+                } else {
+                    tma_load_3d(stB + (q % NST) * R * LANES, &a->tmB, x0, row0, z, b);
+                    tma_load_3d(stC + (q % NST) * R * LANES, &a->tmC, x0, row0, z, b);
+                }
             }
         }
     }
@@ -267,8 +310,16 @@ template <typename T, int W, int RT, int OP> struct FeedStrided {
         if (OpTraits<OP>::staged) {
             const T* sb = stB + (q % NST) * R * LANES; const T* sc = stC + (q % NST) * R * LANES;
             T* wr = win + ((row0 & (W - 1)) << 5);
+            auto combine = [&](T* d) {
 #pragma unroll
-            for (int r = 0; r < R; r++) wr[r * LANES + lane] = PassOp<T, OP>::in(wr[r * LANES + lane], sb[r * LANES + lane], sc[r * LANES + lane]);
+                for (int r = 0; r < R; r++) {
+                    const T c = sc[r * LANES + lane];
+                    d[r] = c - sb[r * LANES + lane];
+                    wr[r * LANES + lane] = PassOp<T, OP>::in_d(wr[r * LANES + lane], d[r], c);
+                }
+            };
+            if constexpr (Ring::on) ring->at(row0, combine);          // d of this tile kept in its ring slot
+            else { T d[R]; combine(d); }
         }
         __syncwarp();
         return true;
@@ -322,7 +373,12 @@ __device__ __forceinline__ void store8_transposed(const Window<T, W>& w, int r0,
 
 template <typename T, int W, int OP> struct DrainStrided {
     using TR = OpTraits<OP>;
+    using Ring = DRing<T, W, OP>;
+    // operand loads of a whole group: none when the feed's d ring holds what they would bring (the partial last group and the
+    // repair path still read B and C)
+    static constexpr int group_reads = Ring::on ? 0 : TR::drain_reads;
     const T* __restrict__ B; const T* __restrict__ C; T* __restrict__ X; T* __restrict__ X2;
+    Ring* ring;
     long long gbase, stride;          // this lane's fiber: element of row 0, element stride between rows
     int ce;                           // end of the chunk (rows beyond are not this task's)
     long long tbase, n; int nvalid;   // transposed results: element (fiber 0 of the group, row 0) of the fiber-major array; fibers in the group
@@ -336,7 +392,7 @@ template <typename T, int W, int OP> struct DrainStrided {
         for (int u = 0; u < 8; u++) { pb[u] = ld_last(qb, pol); qb += stride; if (TR::drain_reads > 1) { pc[u] = ld_last(qc, pol); qc += stride; } }
     }
     __device__ __forceinline__ void prefetch(int r0, int ce, bool valid) {
-        if (TR::drain_reads == 0 || !valid || r0 + 8 > ce || r0 == pf_row) return;
+        if (group_reads == 0 || !valid || r0 + 8 > ce || r0 == pf_row) return;
         fetch(r0); pf_row = r0;
     }
     __device__ __forceinline__ void rows8(const Window<T, W>& w, int r0, int cnt, int lane, const T* xs, bool valid) {
@@ -344,9 +400,18 @@ template <typename T, int W, int OP> struct DrainStrided {
         const long long g0 = gbase + (long long)r0 * stride;
         if (cnt == 8) {                                     // whole group
             T o1[8], o2[8];
-            if (TR::drain_reads > 0 && valid && r0 != pf_row) fetch(r0);
+            if constexpr (Ring::on) {                           // t' = d + x from the ring slot of this tile, stored (not transposed)
+                ring->at(r0, [&](const T* d) {
+                    T* __restrict__ px = X + g0;
 #pragma unroll
-            for (int u = 0; u < 8; u++) PassOp<T, OP>::out(xs[u], pb[u], pc[u], o1[u], o2[u]);
+                    for (int u = 0; u < 8; u++) { st_stream(px, PassOp<T, OP>::out_d(xs[u], d[u]), pol); px += stride; }
+                });
+                return;
+            } else {
+                if (group_reads > 0 && valid && r0 != pf_row) fetch(r0);
+#pragma unroll
+                for (int u = 0; u < 8; u++) PassOp<T, OP>::out(xs[u], pb[u], pc[u], o1[u], o2[u]);
+            }
             pf_row = -1;
             if (TR::tout) {
                 store8_transposed<T, W>(w, r0, lane, o1, X + tbase + r0, n, nvalid, pol);
@@ -494,8 +559,13 @@ __device__ __noinline__ int repair_fiber(const LaneArgs<T>* a, const ChunkPlan p
 __device__ __forceinline__ unsigned long long gtimer() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 __device__ __forceinline__ unsigned smid() { unsigned r; asm volatile("mov.u32 %0, %%smid;" : "=r"(r)); return r; }
 
+// Residency the register allocation is held to: 12 warps per SM (three CTAs of 4 warps: at most 168 registers per thread), except
+// for the staged forms, whose 8 KB of operand staging per warp leave room for 8 warps only (two CTAs: up to 255 registers -- the d
+// ring of LOP_DR_B lives in what the third CTA would have used).
+template <int OP, int NW> constexpr int lane_min_ctas() { return ((OpTraits<OP>::staged ? 8 : 12) + NW - 1) / NW; }
+
 template <typename T, int W, int RT, int TITER, int OP, int NW, int LAY, bool LOG>
-__global__ void __launch_bounds__(NW * 32, (12 + NW - 1) / NW) k_lane(const __grid_constant__ LaneArgs<T> a) {
+__global__ void __launch_bounds__(NW * 32, lane_min_ctas<OP, NW>()) k_lane(const __grid_constant__ LaneArgs<T> a) {
     using SM = LaneSmem<T, W, RT, OP, LAY, NW>;
     extern __shared__ __align__(1024) unsigned char smem[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -551,8 +621,9 @@ __global__ void __launch_bounds__(NW * 32, (12 + NW - 1) / NW) k_lane(const __gr
         DrainContig<T, W> drain{&a, stB, x0, lane, g.ce};
         warp_task<T, W, TITER>(env, feed, drain, w, rcp, g, a.lam, TITER + TITER / 2 + FeedContig<T, W>::R, sp);
     } else {
-        FeedStrided<T, W, RT, OP> feed{&a, win, stB, stC, bar, x0, z, g.p0 / RT, lane};
-        DrainStrided<T, W, OP> drain; drain.B = a.B; drain.C = a.C; drain.X = a.X; drain.X2 = a.X2; drain.gbase = gbase; drain.stride = a.inc;
+        DRing<T, W, OP> ring;
+        FeedStrided<T, W, RT, OP> feed{&a, win, stB, stC, bar, x0, z, g.p0 / RT, lane, &ring};
+        DrainStrided<T, W, OP> drain; drain.ring = &ring; drain.B = a.B; drain.C = a.C; drain.X = a.X; drain.X2 = a.X2; drain.gbase = gbase; drain.stride = a.inc;
         drain.pf_row = -1; drain.pol = policy_evict_first(); drain.ce = g.ce; drain.tbase = tgroup; drain.n = pl.n; drain.nvalid = (int)(a.per_slab - x0 < LANES ? a.per_slab - x0 : LANES);
         warp_task<T, W, TITER>(env, feed, drain, w, rcp, g, a.lam, TITER + TITER / 2 + RT, sp);
     }

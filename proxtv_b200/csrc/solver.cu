@@ -200,16 +200,15 @@ static int dr2_lane_body(size_t M, size_t N, int batch, const T* Y, T w1, T w2, 
                          void* lscr, cudaStream_t st) {
 #define LTRY(expr) do { cudaError_t e__ = (expr); if (e__ == cudaErrorInvalidConfiguration) { cudaGetLastError(); return 2; } \
     if (e__ != cudaSuccess) { fprintf(stderr, "proxtv_b200: CUDA error %s at %s:%d\n", cudaGetErrorString(e__), __FILE__, __LINE__); return 1; } } while (0)
-    const long long n = (long long)M * N * batch;
     LTRY(ew_image_means_x2<T>(Y, (long long)M * N, batch, t, scratch, st));                                   // t = 2 mean (:390-395)
     for (int it = 0; it <= maxit; it++) {
         const bool final = it == maxit, first = it == 0 && maxit > 0;
-        if (first) LTRY(cudaMemcpyAsync(x1, t, (size_t)n * sizeof(T), cudaMemcpyDeviceToDevice, st));
-        else { KernelSpan sp(KC_PROX_CONTIG, 1, st);
-               LTRY(ptvl::lane_prox<T>(ptvl::LANE_PLAIN, t, nullptr, nullptr, x1, (long long)N * batch, (int)M, 1, w1, lscr, st)); }
+        // first half-iteration: prox_cols of the constant t is t itself, so the row pass takes t as x1 (d = t - t = 0 exactly)
+        if (!first) { KernelSpan sp(KC_PROX_CONTIG, 1, st);
+                      LTRY(ptvl::lane_prox<T>(ptvl::LANE_PLAIN, t, nullptr, nullptr, x1, (long long)N * batch, (int)M, 1, w1, lscr, st)); }
         { KernelSpan sp(KC_PROX_STRIDED, 1, st);
-          LTRY(ptvl::lane_prox<T>(final ? ptvl::LANE_DR_B_FINAL : ptvl::LANE_DR_B, Y, x1, t, final ? out : t2, (long long)M * batch, (int)N,
-                                  (long long)M, w2, lscr, st)); }
+          LTRY(ptvl::lane_prox<T>(final ? ptvl::LANE_DR_B_FINAL : ptvl::LANE_DR_B, Y, first ? t : x1, t, final ? out : t2, (long long)M * batch,
+                                  (int)N, (long long)M, w2, lscr, st)); }
         if (!final) { T* tmp = t; t = t2; t2 = tmp; }
     }
     return 0;
