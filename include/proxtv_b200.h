@@ -74,6 +74,12 @@ int DR2_TV(size_t M, size_t N, double *unary, double W1, double W2, double norm1
  * info = {maxit, untouched, RC_OK}; returns 0 on success AND on error, like the reference (:135, :64-68).  nThreads is
  * ignored.  Fibers of length 1 (M == 1 or N == 1) are left unchanged (the reference reads past an empty weight line). */
 int DR2L1W_TV(size_t M, size_t N, double *unary, double *W1, double *W2, double *s, int nThreads, int maxit, double *info);
+/* replaces src/TV2Dopt.cpp:587 (src/TVopt.h:129): the 2D TV-L1 prox by Condat's (alg 0), Chambolle-Pock's (alg 1) or the accelerated
+ * Chambolle-Pock (alg 2) primal-dual iteration, run until the relative change of X is 0 or maxit iterations (<= 0: 2500).  Y, X: M x N
+ * column-major.  Bit for bit the reference's result; info = {iterations run + 1, untouched, RC_OK}; returns 1.  Another alg prints
+ * "Condat2_TV: Algorithm parameter has an invalid value", sets info[2] = 3 and returns 0.  M == 1 or N == 1: the missing difference
+ * term is left out (the reference reads outside its empty dual array). */
+int CondatChambollePock2_TV(size_t M, size_t N, double *Y, double lambda, double *X, short alg, int maxit, double *info);
 /* replaces src/TV2Dopt.cpp:59 (src/TVopt.h:126).  npen <= 2, norms must be 1, dims are 1-based; info = {iters, stop, RC};
  * RC_ITERS is set when iters >= 35 regardless of maxIters (:289); returns 1 ok / 0 error. */
 int PD2_TV(double *y, double *lambdas, double *norms, double *dims, double *x, double *info, int *ns, int nds, int npen,
@@ -185,6 +191,20 @@ int proxtv_DR2_TV_vjp_dev_f32(size_t M, size_t N, int batch, int row_major, int 
 int proxtv_DR2_TV_batched_f64(size_t M, size_t N, int batch, const double *Y, double W1, double W2, double *out, int maxit,
                               double *info);
 int proxtv_DR2_TV_batched_f32(size_t M, size_t N, int batch, const float *Y, float W1, float W2, float *out, int maxit,
+                              double *info);
+
+/* CondatChambollePock2_TV on `batch` independent M x N images stored back to back, column-major (row_major = 0) or C order (1); the
+ * same bits in both orders.  Each image runs until its own stop test holds.  info: host, 3 doubles per image ({iterations run + 1,
+ * untouched, RC}), may be NULL.  float32: float32 arithmetic, step sizes rounded once from float64, stop sums in float64.  The dev
+ * form reads a running-image count back every 64 iterations to end early and synchronises the stream before it returns; the
+ * batched form takes host arrays.  Returns 1 ok / 0 error (info[2] = 3 for every image). */
+int proxtv_CP2_TV_dev_f64(size_t M, size_t N, int batch, int row_major, const double *Y, double lambda, double *X, int alg, int maxit,
+                          double *info, void *stream);
+int proxtv_CP2_TV_dev_f32(size_t M, size_t N, int batch, int row_major, const float *Y, double lambda, float *X, int alg, int maxit,
+                          double *info, void *stream);
+int proxtv_CP2_TV_batched_f64(size_t M, size_t N, int batch, int row_major, const double *Y, double lambda, double *X, int alg, int maxit,
+                              double *info);
+int proxtv_CP2_TV_batched_f32(size_t M, size_t N, int batch, int row_major, const float *Y, double lambda, float *X, int alg, int maxit,
                               double *info);
 
 /* DR2L1W_TV with device arrays (layouts as above; f32 is an extension the reference lacks). */

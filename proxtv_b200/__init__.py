@@ -9,7 +9,7 @@ device the calls raise.
 Extensions the reference lacks (SURVEY.md section 8b): a leading batch dimension (``tv1_1d_batched``,
 ``tv1w_1d_batched``, ``tv1_2d_batched``, ``tv1w_2d_batched``), float32, and torch CUDA tensors as inputs (device-resident path: no PCIe
 traffic, no host transposes -- a C-ordered tensor is handled by swapping the kernels' stride roles).  The batched 1D functions,
-``tv1_2d`` (both methods) / ``tv1_2d_batched``, ``tv1w_2d`` / ``tv1w_2d_batched`` and the N-D ``tvgen`` / ``tvgen_pdr`` are differentiable on torch
+``tv1_2d`` ('dr' and 'pd') / ``tv1_2d_batched`` ('dr'), ``tv1w_2d`` / ``tv1w_2d_batched`` and the N-D ``tvgen`` / ``tvgen_pdr`` are differentiable on torch
 tensors (exact backward kernels).
 """
 import ctypes as C
@@ -277,14 +277,18 @@ def tv1w_1d_batched(x, w):
 # 2D
 # ======================================================================================================================
 _TV1_2D_METHODS = ("yang", "dr", "pd", "kolmogorov", "condat", "chambolle-pock", "chambolle-pock-acc")  # :391-399
+_CP2_ALGS = {"condat": 0, "chambolle-pock": 1, "chambolle-pock-acc": 2}                          # the `alg` of CondatChambollePock2_TV
+_TV1_2D_GPU_METHODS = ("dr", "pd") + tuple(_CP2_ALGS)
 
 
 def tv1_2d(x, w, n_threads=1, max_iters=0, method="dr"):
     r"""2D anisotropic TV-L1 prox (prox_tv/__init__.py:355-416).
 
     ``method='dr'`` (default) reproduces the reference's DR2_TV iteration exactly (35 fixed iterations unless
-    ``max_iters`` > 0 -- NOT a converged solve, see SURVEY.md section 0.3); ``'pd'`` reproduces PD2_TV.  The other
-    reference methods are slower CPU baselines for the same problem and are not provided.  ``n_threads`` is ignored.
+    ``max_iters`` > 0 -- NOT a converged solve, see SURVEY.md section 0.3); ``'pd'`` reproduces PD2_TV.  ``'condat'``,
+    ``'chambolle-pock'`` and ``'chambolle-pock-acc'`` reproduce CondatChambollePock2_TV bit for bit (float64): primal-dual
+    iterations run until X stops changing or ``max_iters`` (0: 2500) -- the converged prox (DESIGN.md section 15); they have no
+    backward pass.  ``'yang'`` and ``'kolmogorov'`` are not provided.  ``n_threads`` is ignored.
     numpy input: returns a Fortran-ordered float64 array like the reference.  torch CUDA tensor input (2D, float64 or
     float32): stays on the device and returns a tensor of the same dtype/layout.
 
@@ -297,8 +301,10 @@ def tv1_2d(x, w, n_threads=1, max_iters=0, method="dr"):
     """
     assert w >= 0
     assert method in _TV1_2D_METHODS
-    if method not in ("dr", "pd"):
-        raise NotImplementedError("proxtv_b200 implements the 'dr' and 'pd' 2D solvers (the GPU hot path); got %r" % method)
+    if method not in _TV1_2D_GPU_METHODS:
+        raise NotImplementedError("proxtv_b200 implements the 2D solvers %s; got %r" % (", ".join(map(repr, _TV1_2D_GPU_METHODS)), method))
+    if method in _CP2_ALGS:
+        return _cp2(x, w, max_iters, method, batched=False)
     if _is_torch(x):
         if method == "pd":
             assert x.dim() == 2
@@ -486,13 +492,18 @@ def _dr2_solve(xin, w, geom, tape=None):
     return out
 
 
-def tv1_2d_batched(x, w, max_iters=0):
-    """``tv1_2d(method='dr')`` on every image of x (B, H, W)  -- BASELINE config 5.
+def tv1_2d_batched(x, w, max_iters=0, method="dr"):
+    """``tv1_2d(method=method)`` on every image of x (B, H, W)  -- BASELINE config 5 with the default ``method='dr'``.
 
     numpy: float64 or float32, C-ordered (B, H, W); torch: CUDA tensor (B, H, W).  Each image is solved independently with
     exactly the single-image iteration (its own 2*mean initialisation).  torch: differentiable like ``tv1_2d``.
+    ``method`` 'condat', 'chambolle-pock' or 'chambolle-pock-acc': each image runs until its own stop test holds (float32: float32
+    arithmetic); numpy results are C-ordered arrays of x's dtype, tensors keep their layout; no backward pass.
     """
     assert w >= 0
+    assert method == "dr" or method in _CP2_ALGS, "method must be 'dr', 'condat', 'chambolle-pock' or 'chambolle-pock-acc'"
+    if method in _CP2_ALGS:
+        return _cp2(x, w, max_iters, method, batched=True)
     if _is_torch(x):
         return _dr2_torch(x, w, max_iters, batched=True)
     x = np.asarray(x)
@@ -508,6 +519,47 @@ def tv1_2d_batched(x, w, max_iters=0):
     fn(H, W, B, _ptr(xt), float(w), float(w), _ptr(out), int(max_iters), _ptr(info))
     _check(info[2] != 3, "DR2_TV (batched)")
     return np.transpose(out, (0, 2, 1))
+
+
+def _cp2(x, w, max_iters, method, batched):
+    """CondatChambollePock2_TV for tv1_2d / tv1_2d_batched.  numpy 2D: the reference's entry point on a Fortran-ordered float64 copy;
+    numpy 3D: proxtv_CP2_TV_batched_* on the C-ordered (B, H, W) array; torch: proxtv_CP2_TV_dev_* on either memory order
+    (_dr2_layout), result in the solved tensor's layout."""
+    alg = _CP2_ALGS[method]
+    if _is_torch(x):
+        if _needs_grad(x, w):
+            raise NotImplementedError("tv1_2d method %r has no backward pass; use method='dr' or 'pd' for gradients, or call it "
+                                      "under torch.no_grad() / on a detached tensor" % method)
+        import torch
+        wf = float(w.detach()) if _is_torch(w) else float(w)
+        M, N, batch, row_major, xin = _dr2_layout(x, batched)
+        out = torch.empty_strided(xin.shape, xin.stride(), dtype=xin.dtype, device=xin.device)
+        info = np.zeros(_N_INFO * batch)
+        _dev_call("CP2_TV_dev", xin, M, N, batch, row_major, xin, wf, out, alg, int(max_iters), info, info=info)
+        return out
+    w = force_float_scalar(w)
+    if not batched:
+        x = np.asfortranarray(x, dtype="float64")
+        assert x.ndim == 2
+        lib = require_device()
+        y = _pool.empty(x.shape, np.float64, "F")
+        info = np.zeros(_N_INFO)
+        ok = lib.CondatChambollePock2_TV(x.shape[0], x.shape[1], _ptr(x), w, _ptr(y), alg, int(max_iters), _ptr(info))
+        _check(ok and info[2] != 3, "CondatChambollePock2_TV")
+        return y
+    x = np.asarray(x)
+    assert x.ndim == 3
+    dt = np.float32 if x.dtype == np.float32 else np.float64
+    x = np.ascontiguousarray(x, dtype=dt)
+    B, H, W = x.shape
+    out = _pool.empty(x.shape, dt, "C")
+    if x.size:
+        info = np.zeros(_N_INFO * B)
+        lib = require_device()
+        fn = lib.proxtv_CP2_TV_batched_f32 if dt == np.float32 else lib.proxtv_CP2_TV_batched_f64
+        ok = fn(H, W, B, 1, _ptr(x), w, _ptr(out), alg, int(max_iters), _ptr(info))
+        _check(ok and not np.any(info[2::3] == 3), "CondatChambollePock2_TV (batched)")
+    return out
 
 
 # ======================================================================================================================

@@ -36,6 +36,7 @@ SIGNATURES = {
     "PD2_TV": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int]),
     "PD_TV": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int]),
     "PDR_TV": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "CondatChambollePock2_TV": (C.c_int, [C.c_size_t, C.c_size_t, _vp, C.c_double, _vp, C.c_short, C.c_int, _vp]),
     # Part 2: extensions
     "proxtv_device_count": (C.c_int, []),
     "proxtv_last_error": (C.c_char_p, []),
@@ -54,6 +55,10 @@ SIGNATURES = {
     "proxtv_prox_fibers_f32": (C.c_int, [_vp, _vp, C.c_longlong, C.c_int, C.c_longlong, C.c_float, _vp]),
     "proxtv_DR2_TV_dev_f64": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, C.c_int, _vp, C.c_double, C.c_double, _vp, C.c_int, _vp, _vp]),
     "proxtv_DR2_TV_dev_f32": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, C.c_int, _vp, C.c_float, C.c_float, _vp, C.c_int, _vp, _vp]),
+    "proxtv_CP2_TV_dev_f64": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, C.c_int, _vp, C.c_double, _vp, C.c_int, C.c_int, _vp, _vp]),
+    "proxtv_CP2_TV_dev_f32": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, C.c_int, _vp, C.c_double, _vp, C.c_int, C.c_int, _vp, _vp]),
+    "proxtv_CP2_TV_batched_f64": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, C.c_int, _vp, C.c_double, _vp, C.c_int, C.c_int, _vp]),
+    "proxtv_CP2_TV_batched_f32": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, C.c_int, _vp, C.c_double, _vp, C.c_int, C.c_int, _vp]),
     "proxtv_DR2L1W_TV_dev_f64": (C.c_int, [C.c_size_t, C.c_size_t, _vp, _vp, _vp, _vp, C.c_int, _vp, _vp]),
     "proxtv_DR2L1W_TV_dev_f32": (C.c_int, [C.c_size_t, C.c_size_t, _vp, _vp, _vp, _vp, C.c_int, _vp, _vp]),
     "proxtv_DR2L1W_TV_tape_bytes": (C.c_size_t, [C.c_size_t, C.c_size_t, C.c_int]),

@@ -161,6 +161,44 @@ int run_drw(const char* fn, bool host_io, size_t M, size_t N, int batch, int row
     return 0;
 }
 
+// CondatChambollePock2_TV with host (host_io) or device arrays: `batch` images back to back, column-major (row_major = 0) or C order
+// (1); info: host, 3 doubles per image, or NULL.  Returns 1 on success, 0 on failure (src/TV2Dopt.cpp:600-602, :750-756).
+template <typename T>
+int run_cp2(const char* fn, bool host_io, size_t M, size_t N, int batch, int row_major, const T* Y, double lambda, T* X, int alg, int maxit,
+            double* info, cudaStream_t st) {
+    auto fail_all = [&](const char* msg) {          // msg nullptr: already reported
+        if (msg) fail(fn, msg, info); else if (info) info[INFO_RC] = RC_ERROR;
+        if (info) for (int b = 1; b < batch; b++) info[3 * (size_t)b + INFO_RC] = RC_ERROR;
+        return 0;
+    };
+    if (alg != 0 && alg != 1 && alg != 2) return fail_all("Algorithm parameter has an invalid value");
+    if (batch < 0) { fail(fn, "invalid shape (need batch >= 0)", info); return 0; }
+    if (batch == 0) return 1;
+    if (M < 1 || N < 1 || M > 0x7fffffff || N > 0x7fffffff) return fail_all("invalid shape (need 1 <= M, N < 2^31)");
+    if (!Y || !X) return fail_all("NULL array");
+    if (!have_device(fn, nullptr)) return fail_all(nullptr);
+    WsGuard guard(st);
+    const size_t n = M * N * (size_t)batch;
+    void* ws = g_ws.get(ws_bytes_cp2(M, N, batch, sizeof(T)));
+    if (!ws) return fail_all("out of memory");
+    const T* dY = Y; T* dX = X;
+    if (host_io) {
+        char* d = (char*)g_io.get(2 * al(n * sizeof(T)));
+        if (!d) return fail_all("out of memory");
+        dY = (T*)d; dX = (T*)(d + al(n * sizeof(T)));
+        if (!cuda_ok(fn, cudaMemcpyAsync((void*)dY, Y, n * sizeof(T), cudaMemcpyHostToDevice, st), nullptr)) return fail_all(nullptr);
+    }
+    std::vector<int> iters(info ? batch : 0);
+    if (!cuda_ok(fn, cp2_device<T>(M, N, batch, row_major, dY, lambda, dX, alg, maxit, info ? iters.data() : nullptr, ws, st), nullptr))
+        return fail_all(nullptr);
+    if (host_io) {
+        if (!cuda_ok(fn, cudaMemcpyAsync(X, dX, n * sizeof(T), cudaMemcpyDeviceToHost, st), nullptr)) return fail_all(nullptr);
+        if (!cuda_ok(fn, cudaStreamSynchronize(st), nullptr)) return fail_all(nullptr);
+    }
+    if (info) for (int b = 0; b < batch; b++) { info[3 * (size_t)b + INFO_ITERS] = iters[b]; info[3 * (size_t)b + INFO_RC] = RC_OK; }
+    return 1;
+}
+
 // PD_TV and PDR_TV multiply the caller's penalties by the number of terms, in place (TVNDopt.cpp:100-101, :339-340); PD2_TV takes
 // them as given.
 void scale_penalties(NdSolver s, double* lambdas, int npen) {
@@ -504,6 +542,9 @@ int DR2_TV(size_t M, size_t N, double* unary, double W1, double W2, double norm1
 int DR2L1W_TV(size_t M, size_t N, double* unary, double* W1, double* W2, double* s, int, int maxit, double* info) {
     return run_drw<double>("DR2L1W_TV", true, M, N, 1, 0, unary, W1, W2, s, maxit, info, 0);
 }
+int CondatChambollePock2_TV(size_t M, size_t N, double* Y, double lambda, double* X, short alg, int maxit, double* info) {
+    return run_cp2<double>("Condat2_TV", true, M, N, 1, 0, Y, lambda, X, alg, maxit, info, 0);
+}
 int PD2_TV(double* y, double* lambdas, double* norms, double* dims, double* x, double* info, int* ns, int nds, int npen, int,
            int maxIters) {
     return run_pd<double>("PD2_TV", ND_PD2, true, y, lambdas, norms, dims, x, info, ns, nds, npen, maxIters, 0);
@@ -587,6 +628,19 @@ int proxtv_DR2_TV_batched_f64(size_t M, size_t N, int batch, const double* Y, do
     return host_dr2<double>("proxtv_DR2_TV_batched_f64", M, N, batch, Y, W1, W2, out, maxit, info); }
 int proxtv_DR2_TV_batched_f32(size_t M, size_t N, int batch, const float* Y, float W1, float W2, float* out, int maxit, double* info) {
     return host_dr2<float>("proxtv_DR2_TV_batched_f32", M, N, batch, Y, W1, W2, out, maxit, info); }
+
+int proxtv_CP2_TV_dev_f64(size_t M, size_t N, int batch, int row_major, const double* Y, double lambda, double* X, int alg, int maxit,
+                          double* info, void* stream) {
+    return run_cp2<double>("proxtv_CP2_TV_dev_f64", false, M, N, batch, row_major, Y, lambda, X, alg, maxit, info, (cudaStream_t)stream); }
+int proxtv_CP2_TV_dev_f32(size_t M, size_t N, int batch, int row_major, const float* Y, double lambda, float* X, int alg, int maxit,
+                          double* info, void* stream) {
+    return run_cp2<float>("proxtv_CP2_TV_dev_f32", false, M, N, batch, row_major, Y, lambda, X, alg, maxit, info, (cudaStream_t)stream); }
+int proxtv_CP2_TV_batched_f64(size_t M, size_t N, int batch, int row_major, const double* Y, double lambda, double* X, int alg, int maxit,
+                              double* info) {
+    return run_cp2<double>("proxtv_CP2_TV_batched_f64", true, M, N, batch, row_major, Y, lambda, X, alg, maxit, info, 0); }
+int proxtv_CP2_TV_batched_f32(size_t M, size_t N, int batch, int row_major, const float* Y, double lambda, float* X, int alg, int maxit,
+                              double* info) {
+    return run_cp2<float>("proxtv_CP2_TV_batched_f32", true, M, N, batch, row_major, Y, lambda, X, alg, maxit, info, 0); }
 
 int proxtv_DR2L1W_TV_dev_f64(size_t M, size_t N, const double* Y, const double* W1, const double* W2, double* out, int maxit, double* info, void* stream) {
     return run_drw<double>("proxtv_DR2L1W_TV_dev_f64", false, M, N, 1, 0, Y, W1, W2, out, maxit, info, (cudaStream_t)stream); }

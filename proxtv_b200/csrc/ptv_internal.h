@@ -200,6 +200,15 @@ template <typename T> size_t ws_bytes_nd_vjp(const NdTerms& t, int npen, bool wa
 template <typename T> cudaError_t nd_vjp_device(NdSolver s, const NdTerms& t, int npen, int maxIters, int iters, const void* tape,
                                                 const T* gout, T* gY, double* glam, void* ws, cudaStream_t st);
 
+// ---- CondatChambollePock2_TV (cp2.cu, DESIGN.md section 15): Condat (alg 0), Chambolle-Pock (1) and accelerated Chambolle-Pock (2) ----
+size_t ws_bytes_cp2(size_t M, size_t N, int batch, size_t elem);
+// `batch` M x N images back to back, column-major (row_major = 0) or C order (1); alg in 0..2 (checked by the caller); maxit <= 0:
+// 2500.  iters: nullptr, or host memory for each image's final `it` (iterations run + 1; the call then synchronises the stream).
+// Reads the running-image count back every 64 iterations (one stream synchronisation each).
+template <typename T>
+cudaError_t cp2_device(size_t M, size_t N, int batch, int row_major, const T* Y, double lambda, T* out, int alg, int maxit, int* iters,
+                       void* ws, cudaStream_t st);
+
 }  // namespace ptv
 
 // ---- lane-per-fiber streaming engine (kernels_lane.cu): slope-form scan, TMA-tiled windows, no transposed copies ----
