@@ -337,6 +337,54 @@ int proxtv_PD2_TV_vjp_dev_f32(const int *ns, int nds, int npen, const double *di
 int proxtv_PD_TV_f32(const float *y, double *lambdas, double *dims, float *x, double *info, int *ns, int nds, int npen,
                      int maxIters);                                          /* host pointers, float32 */
 
+/* Batched PD_TV / PD2_TV (DESIGN.md section 16): `batch` items, each a column-major array of dims ns[0..nds), back to back at stride
+ * prod(ns) in y and x; dims are axes of an item.  Every item runs its own loop and stop rule (PD_TV: while stop_b > 1e-6 and it < maxIters;
+ * PD2_TV: the same, and one iteration only when npen = 1), and info[3 b .. 3 b + 2] = [K_b, stop_b, RC_b] as the single-item call gives
+ * it.  Under the seq and chunked engines every item's x and info row equal proxtv_PD*_TV_dev_* on that item (into an aligned buffer)
+ * bit for bit, whatever batch is and wherever the item sits; under auto / lane the engine is picked for the whole batch.  An item that
+ * has stopped costs no more prox work.  lambdas are the penalties as given (PD_TV applies its factor npen to a copy) and are never
+ * written.  Same refusals, in the same order, as the single-item entry points, plus batch < 1; a refusal writes nothing but
+ * info[3 b + 2] = 3 for every item, and returns 0.  The dev and record entries read the stop values back once per iteration.
+ * tape_bytes: nd_head + P 2 align256(4 ceil(n batch / 32)), nd_head = 256 + align256(4 batch), P as for the single-item tape, in 64-bit
+ * arithmetic, 0 for invalid arguments or a size that does not fit.  The tape carries its own magic (neither the single-item tapes nor
+ * the other solver's are accepted), batch, and each item's K.  vjp: from the tape alone (one stream synchronisation reads its header
+ * and K table), gY of every item bit for bit the single-item vjp's for that item's K; glam unless NULL: batch x npen doubles, the
+ * gradients of the penalties AS GIVEN for both solvers. */
+size_t proxtv_PD_TV_batched_tape_bytes(const int *ns, int nds, int npen, int batch, int maxIters);
+size_t proxtv_PD2_TV_batched_tape_bytes(const int *ns, int nds, int npen, int batch, int maxIters);
+int proxtv_PD_TV_batched_dev_f64(const double *y, const double *lambdas, const double *dims, double *x, double *info, const int *ns, int nds,
+                              int npen, int batch, int maxIters, void *stream);
+int proxtv_PD_TV_batched_f64(const double *y, const double *lambdas, const double *dims, double *x, double *info, const int *ns, int nds, int npen,
+                          int batch, int maxIters);                 /* host pointers */
+int proxtv_PD_TV_batched_record_dev_f64(const double *y, const double *lambdas, const double *dims, double *x, double *info, const int *ns,
+                                     int nds, int npen, int batch, int maxIters, void *tape, size_t tape_bytes, void *stream);
+int proxtv_PD_TV_batched_vjp_dev_f64(const int *ns, int nds, int npen, const double *dims, int batch, int maxIters, const void *tape,
+                                  const double *gout, double *gY, double *glam, void *stream);
+int proxtv_PD_TV_batched_dev_f32(const float *y, const double *lambdas, const double *dims, float *x, double *info, const int *ns, int nds,
+                              int npen, int batch, int maxIters, void *stream);
+int proxtv_PD_TV_batched_f32(const float *y, const double *lambdas, const double *dims, float *x, double *info, const int *ns, int nds, int npen,
+                          int batch, int maxIters);                 /* host pointers */
+int proxtv_PD_TV_batched_record_dev_f32(const float *y, const double *lambdas, const double *dims, float *x, double *info, const int *ns,
+                                     int nds, int npen, int batch, int maxIters, void *tape, size_t tape_bytes, void *stream);
+int proxtv_PD_TV_batched_vjp_dev_f32(const int *ns, int nds, int npen, const double *dims, int batch, int maxIters, const void *tape,
+                                  const float *gout, float *gY, double *glam, void *stream);
+int proxtv_PD2_TV_batched_dev_f64(const double *y, const double *lambdas, const double *dims, double *x, double *info, const int *ns, int nds,
+                              int npen, int batch, int maxIters, void *stream);
+int proxtv_PD2_TV_batched_f64(const double *y, const double *lambdas, const double *dims, double *x, double *info, const int *ns, int nds, int npen,
+                          int batch, int maxIters);                 /* host pointers */
+int proxtv_PD2_TV_batched_record_dev_f64(const double *y, const double *lambdas, const double *dims, double *x, double *info, const int *ns,
+                                     int nds, int npen, int batch, int maxIters, void *tape, size_t tape_bytes, void *stream);
+int proxtv_PD2_TV_batched_vjp_dev_f64(const int *ns, int nds, int npen, const double *dims, int batch, int maxIters, const void *tape,
+                                  const double *gout, double *gY, double *glam, void *stream);
+int proxtv_PD2_TV_batched_dev_f32(const float *y, const double *lambdas, const double *dims, float *x, double *info, const int *ns, int nds,
+                              int npen, int batch, int maxIters, void *stream);
+int proxtv_PD2_TV_batched_f32(const float *y, const double *lambdas, const double *dims, float *x, double *info, const int *ns, int nds, int npen,
+                          int batch, int maxIters);                 /* host pointers */
+int proxtv_PD2_TV_batched_record_dev_f32(const float *y, const double *lambdas, const double *dims, float *x, double *info, const int *ns,
+                                     int nds, int npen, int batch, int maxIters, void *tape, size_t tape_bytes, void *stream);
+int proxtv_PD2_TV_batched_vjp_dev_f32(const int *ns, int nds, int npen, const double *dims, int batch, int maxIters, const void *tape,
+                                  const float *gout, float *gY, double *glam, void *stream);
+
 /* Launch accounting and optional CUDA-event timing per kernel class (0: prox over contiguous fibers, 1: prox over strided
  * fibers, 2: elementwise/reduction helpers).  Launch counters always run; event timing only while enabled.  read():
  * arrays of 3; ms = summed event time, launches = kernels launched, spans = timed brackets; synchronises the events. */

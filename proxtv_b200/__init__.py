@@ -22,7 +22,7 @@ from . import _lib
 from ._lib import ProxTVError, load, require_device  # noqa: F401
 
 __all__ = ["tv1_1d", "tv1w_1d", "tv1_2d", "tv1w_2d", "tvgen", "tvgen_pdr", "tv1_1d_batched", "tv1w_1d_batched", "tv1_2d_batched",
-           "tv1w_2d_batched", "set_engine", "set_pinned_results", "ProxTVError"]
+           "tv1w_2d_batched", "tvgen_batched", "set_engine", "set_pinned_results", "ProxTVError"]
 
 _N_INFO = 3                      # prox_tv/__init__.py:67
 ENGINES = {"auto": 0, "seq": 1, "chunked": 2, "chunked-strided": 3, "pipelined": 4, "tspace": 5, "tpose": 6, "lane": 7, "lane-t": 8}
@@ -678,20 +678,102 @@ def _nd_torch(solver, x, lam, ws_t, ds, max_iters):
     return _nd_solve(xin, *args)[0]
 
 
-def _nd_solve(xin, solver, nsa, dsa, lama, max_iters, tape=None):
+def _nd_solve(xin, solver, nsa, dsa, lama, max_iters, tape=None, batch=0):
     """proxtv_<solver>_dev_* (solver: "PDR_TV", "PD_TV" or "PD2_TV") on xin, column-major over nsa (see _pdr_layout), or given a tape
     (a uint8 CUDA tensor, proxtv_<solver>_tape_bytes() long) proxtv_<solver>_record_dev_*, the same solve recording every prox pass's
-    segmentation.  Sets the last_info of the public function that runs the solver; returns (result in xin's layout, info)."""
+    segmentation.  batch >= 1 (PD_TV / PD2_TV): xin holds `batch` items over nsa back to back, solved by proxtv_<solver>_batched_dev_* /
+    _batched_record_dev_*, and info is (batch, 3).  Sets the last_info of the public function that runs the solver; returns (result in
+    xin's layout, info)."""
     import torch
     out = torch.empty_strided(xin.shape, xin.stride(), dtype=xin.dtype, device=xin.device)
-    info = np.zeros(_N_INFO)
-    args = (xin, lama, dsa, out, info, nsa, len(nsa), len(lama), max_iters)
+    info = np.zeros(_N_INFO * max(batch, 1))
+    bat = (batch,) if batch else ()
+    kind = "_batched" if batch else ""
+    args = (xin, lama, dsa, out, info, nsa, len(nsa), len(lama)) + bat + (max_iters,)
     if tape is None:
-        _dev_call(solver + "_dev", xin, *args, info=info)
+        _dev_call(solver + kind + "_dev", xin, *args, info=info)
     else:
-        _dev_call(solver + "_record_dev", xin, *args, tape, tape.numel(), info=info)
-    (tvgen_pdr if solver == "PDR_TV" else tvgen).last_info = info
+        _dev_call(solver + kind + "_record_dev", xin, *args, tape, tape.numel(), info=info)
+    if batch:
+        info = info.reshape(batch, _N_INFO)
+        tvgen_batched.last_info = info
+    else:
+        (tvgen_pdr if solver == "PDR_TV" else tvgen).last_info = info
     return out, info
+
+
+def tvgen_batched(x, ws, ds, ps, max_iters=0):
+    r"""``tvgen`` over a batch: x of shape (B, \*s) holds B independent items of shape s, and item b is solved as ``tvgen(x[b], ws, ds,
+    ps, max_iters=max_iters)`` would solve it, with its own stop test.
+
+    ``ds`` are 1-based axes of an item (1..len(s)); two terms go to PD2_TV and any other count to PD_TV, as in ``tvgen``; p = 1 terms
+    only (anything else raises NotImplementedError).  ``ws`` is shared by every item -- a list, an ndarray or a 1-D tensor -- and is
+    never written (``tvgen``'s in-place scaling of a float64 ndarray is not carried over).
+    Per-item stop rule: item b iterates while mean|x_b - x_b,last| > 1e-6 and it < ``max_iters`` (0: 35) -- PD2_TV with one term runs
+    one iteration -- so an item's result does not depend on the rest of the batch, and an item that has stopped costs no more prox
+    work.  ``tvgen_batched.last_info`` is a (B, 3) array, row b = [K_b, stop_b, RC_b] as ``tvgen.last_info`` gives it for that item.
+    Under the bit-faithful engines (``set_engine('seq')`` / ``'chunked'``) every item's result and info row equal the single-item
+    solve of that item (``proxtv_PD*_TV_dev_*`` into an aligned buffer) bit for bit, in float64 and float32, whatever B is, wherever
+    the item sits and whenever the others stop.  Under ``'auto'`` and ``'lane'`` the fiber route and the lane engine's suitability test
+    are decided once for the whole batch (its fiber count, its first 2^18 elements), so an item's bits can differ from its single
+    solve's (the lane engine computes in slope form); the results agree to about 1e-12 relative.
+    numpy: float64, or float32 solved in float32, with both solvers; items are solved in column-major order, so item b is bit for bit
+    ``tvgen(x[b], ...)`` under ``'chunked'``; returns a (B, \*s) array of x's dtype.
+    torch: a CUDA tensor (float32 or float64, ndim >= 2) is solved on its device and current stream.  A C-ordered tensor is taken as
+    it is (each item is the column-major array of its reversed shape), and so is one whose items are column-major and contiguous with
+    the batch axis slowest; anything else is made C-contiguous; the result has the solved tensor's layout.  Differentiable with
+    respect to x and a ``ws`` tensor: the forward records the segmentation tape of every prox pass and each item's K, and the backward
+    is, for every item, the exact vector-Jacobian product of the K_b iterations that item ran (``proxtv_PD*_TV_batched_vjp_dev_*``,
+    DESIGN.md section 16); the ``ws`` gradient is the per-item penalty gradients summed in float64.  K_b has no derivative: where a
+    perturbation changes it the map jumps.  The tape is allocated for ``max_iters`` iterations of the whole batch, B times the single
+    capacity: PD_TV with 3 terms at 35 iterations takes about 1.64 GiB per 512 x 512 x 256 item.  Double backward is not supported.
+    """
+    assert len(ws) == len(ds)
+    assert len(ws) == len(ps)
+    assert max_iters >= 0
+    if np.any(force_float_matrix(ps) != 1):
+        raise NotImplementedError("proxtv_b200 implements TV-L1 (p = 1) penalty terms only")
+    lam, ws_t = _ws_floats(ws)
+    assert ws_t is None or tuple(ws_t.shape) in ((), (len(lam),)), "ws must be one penalty per term, or one 0-dim penalty for all"
+    solver = "PD2_TV" if len(lam) == 2 else "PD_TV"
+    lama = np.array(lam, dtype=np.float64)
+    if _is_torch(x):
+        import torch
+        assert x.is_cuda and x.dtype in (torch.float64, torch.float32) and x.dim() >= 2
+        B, s = int(x.shape[0]), [int(n) for n in x.shape[1:]]
+        if B == 0:
+            tvgen_batched.last_info = np.zeros((0, _N_INFO))
+            return torch.empty_like(x)
+        if not x.is_contiguous() and _f_contiguous(x[0]) and (B == 1 or x.stride(0) == int(np.prod(s))):
+            xin, ns, dims = x, s, [float(d) for d in ds]              # items column-major, back to back
+        else:
+            xin = x.contiguous()
+            ns, dims = _pdr_c_order(s, ds)
+        args = (solver, np.array(ns, dtype=np.int32), np.array(dims, dtype=np.float64), lama, int(max_iters))
+        if _needs_grad(x, ws_t):
+            return _autograd().ND.apply(xin, ws_t, *args, B)
+        return _nd_solve(xin, *args, None, B)[0]
+    x = np.asarray(x)
+    f32 = x.dtype == np.float32
+    assert x.ndim >= 2
+    B = x.shape[0]
+    if B == 0:
+        tvgen_batched.last_info = np.zeros((0, _N_INFO))
+        return np.zeros(x.shape, dtype=np.float32 if f32 else np.float64)
+    rev = (0,) + tuple(range(x.ndim - 1, 0, -1))                    # (B, s_k .. s_1) in C order: every item column-major
+    xt = np.ascontiguousarray(np.transpose(x, rev), dtype=np.float32 if f32 else np.float64)
+    out = np.empty_like(xt)
+    info = np.zeros(_N_INFO * B)
+    ns = np.array(x.shape[1:], dtype=np.int32)
+    dsa = np.array(ds, dtype=np.float64)
+    fn = getattr(require_device(), "proxtv_%s_batched_%s" % (solver, "f32" if f32 else "f64"))
+    ok = fn(_ptr(xt), _ptr(lama), _ptr(dsa), _ptr(out), _ptr(info), _ptr(ns), len(ns), len(lama), B, int(max_iters))
+    _check(ok and not np.any(info[2::3] == 3), "tvgen_batched")
+    tvgen_batched.last_info = info.reshape(B, _N_INFO)
+    return np.transpose(out, rev)
+
+
+tvgen_batched.last_info = None
 
 
 def tvgen_pdr(x, ws, ds, ps, n_threads=1, max_iters=0):
@@ -839,17 +921,24 @@ def _autograd():
             return (gY if need_x else None), None, g_w, None
 
     class ND(torch.autograd.Function):
-        """apply(xin, ws_t, solver, nsa, dsa, lama, max_iters) of _nd_solve; ctx also keeps the iteration count the solve ran (the
-        Dykstra solvers' stop rule picks it).  backward: proxtv_<solver>_vjp_dev_*; the gradient of ws_t is npen * glam for PDR_TV
-        and PD_TV (glam: the gradients of the scaled penalties), glam for PD2_TV."""
+        """apply(xin, ws_t, solver, nsa, dsa, lama, max_iters[, batch]) of _nd_solve; ctx also keeps the iteration count the solve ran
+        (the Dykstra solvers' stop rule picks it; batch >= 1: each item's K).  backward: proxtv_<solver>_vjp_dev_*; the gradient of ws_t
+        is npen * glam for PDR_TV and PD_TV (glam: the gradients of the scaled penalties), glam for PD2_TV.  batch >= 1:
+        proxtv_<solver>_batched_vjp_dev_*, whose per-item glam is of the penalties as given for both solvers, summed over the items."""
         @staticmethod
-        def forward(ctx, xin, ws_t, solver, nsa, dsa, lama, max_iters):
-            tape_bytes = getattr(require_device(), "proxtv_%s_tape_bytes" % solver)
-            nb = int(tape_bytes(_ptr(nsa), len(nsa), len(lama), max_iters))      # 0: too large; the record call refuses it
+        def forward(ctx, xin, ws_t, solver, nsa, dsa, lama, max_iters, batch=0):
+            lib = require_device()
+            if batch:
+                tape_bytes = getattr(lib, "proxtv_%s_batched_tape_bytes" % solver)
+                nb = int(tape_bytes(_ptr(nsa), len(nsa), len(lama), batch, max_iters))
+            else:
+                tape_bytes = getattr(lib, "proxtv_%s_tape_bytes" % solver)
+                nb = int(tape_bytes(_ptr(nsa), len(nsa), len(lama), max_iters))  # 0: too large; the record call refuses it
             tape = torch.empty(max(nb, 256), dtype=torch.uint8, device=xin.device)
-            out, info = _nd_solve(xin, solver, nsa, dsa, lama, max_iters, tape)
+            out, info = _nd_solve(xin, solver, nsa, dsa, lama, max_iters, tape, batch)
             ctx.save_for_backward(tape)
-            ctx.geom, ctx.layout = (solver, nsa, dsa, max_iters, int(info[0])), (out.shape, out.stride(), out.dtype)
+            iters = info[:, 0].astype(np.int64) if batch else int(info[0])
+            ctx.geom, ctx.layout = (solver, nsa, dsa, max_iters, iters, batch), (out.shape, out.stride(), out.dtype)
             ctx.ws_like = (ws_t.dtype, ws_t.device, ws_t.shape) if ws_t is not None else None
             return out
 
@@ -857,17 +946,22 @@ def _autograd():
         @once_differentiable
         def backward(ctx, gout):
             (tape,) = ctx.saved_tensors
-            solver, nsa, dsa, max_iters, iters = ctx.geom
+            solver, nsa, dsa, max_iters, iters, batch = ctx.geom
             shape, stride, dt = ctx.layout
             need_x, need_ws = ctx.needs_input_grad[:2]
             npen = len(dsa)
             g = torch.empty_strided(shape, stride, dtype=dt, device=tape.device)      # the upstream gradient in the output's layout
             g.copy_(gout)
             gY = torch.empty_strided(shape, stride, dtype=dt, device=tape.device)
-            glam = torch.empty(npen, dtype=torch.float64, device=tape.device) if need_ws else None
+            glam = torch.empty(npen * max(batch, 1), dtype=torch.float64, device=tape.device) if need_ws else None
+            rest = (None,) * (len(ctx.needs_input_grad) - 2)
+            if batch:
+                _dev_call(solver + "_batched_vjp_dev", g, nsa, len(nsa), npen, dsa, batch, max_iters, tape, g, gY, glam)
+                g_ws = _penalty_grad(glam.view(batch, npen).sum(0, dtype=torch.float64), ctx.ws_like) if need_ws else None
+                return (gY if need_x else None), g_ws, *rest
             it = () if solver == "PDR_TV" else (iters,)                               # PDR_TV runs exactly max_iters iterations
             _dev_call(solver + "_vjp_dev", g, nsa, len(nsa), npen, dsa, max_iters, *it, tape, g, gY, glam)
             g_ws = _penalty_grad(glam if solver == "PD2_TV" else glam * float(npen), ctx.ws_like) if need_ws else None
-            return (gY if need_x else None), g_ws, None, None, None, None, None
+            return (gY if need_x else None), g_ws, *rest
 
     return types.SimpleNamespace(ProxRows=ProxRows, DRW=DRW, DR2=DR2, ND=ND)

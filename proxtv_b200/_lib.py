@@ -106,6 +106,28 @@ SIGNATURES = {
     "proxtv_PD2_TV_vjp_dev_f64": (C.c_int, [_vp, C.c_int, C.c_int, _vp, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp]),
     "proxtv_PD2_TV_vjp_dev_f32": (C.c_int, [_vp, C.c_int, C.c_int, _vp, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp]),
     "proxtv_PD_TV_f32": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int]),
+    "proxtv_PD_TV_batched_tape_bytes": (C.c_size_t, [_vp, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "proxtv_PD2_TV_batched_tape_bytes": (C.c_size_t, [_vp, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "proxtv_PD_TV_batched_dev_f64": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp]),
+    "proxtv_PD_TV_batched_f64": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "proxtv_PD_TV_batched_record_dev_f64": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp, C.c_size_t,
+                                                     _vp]),
+    "proxtv_PD_TV_batched_vjp_dev_f64": (C.c_int, [_vp, C.c_int, C.c_int, _vp, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp]),
+    "proxtv_PD_TV_batched_dev_f32": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp]),
+    "proxtv_PD_TV_batched_f32": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "proxtv_PD_TV_batched_record_dev_f32": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp, C.c_size_t,
+                                                     _vp]),
+    "proxtv_PD_TV_batched_vjp_dev_f32": (C.c_int, [_vp, C.c_int, C.c_int, _vp, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp]),
+    "proxtv_PD2_TV_batched_dev_f64": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp]),
+    "proxtv_PD2_TV_batched_f64": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "proxtv_PD2_TV_batched_record_dev_f64": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp, C.c_size_t,
+                                                     _vp]),
+    "proxtv_PD2_TV_batched_vjp_dev_f64": (C.c_int, [_vp, C.c_int, C.c_int, _vp, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp]),
+    "proxtv_PD2_TV_batched_dev_f32": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp]),
+    "proxtv_PD2_TV_batched_f32": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "proxtv_PD2_TV_batched_record_dev_f32": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp, C.c_size_t,
+                                                     _vp]),
+    "proxtv_PD2_TV_batched_vjp_dev_f32": (C.c_int, [_vp, C.c_int, C.c_int, _vp, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp]),
     "proxtv_PDR_TV_dev_f64": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, _vp]),
     "proxtv_PDR_TV_dev_f32": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, _vp]),
     "proxtv_lane_prox_dev_f64": (C.c_int, [C.c_int, _vp, _vp, _vp, _vp, C.c_longlong, C.c_int, C.c_longlong, C.c_double, _vp]),

@@ -428,6 +428,86 @@ static int dev_nd_vjp(const char* fn, NdSolver s, const int* ns, int nds, int np
     return cuda_ok(fn, nd_vjp_device<T>(s, t, npen, maxIters, iters, tape, gout, gY, glam, ws, (cudaStream_t)stream), nullptr);
 }
 
+// ---- batched PD_TV / PD2_TV (DESIGN.md section 16): `batch` items of prod(ns) elements back to back, each with its own stop rule ----
+// Every refusal writes info[3 b + RC] = RC_ERROR for every item and nothing else; lambdas are never written (PD_TV's factor npen is
+// applied to a copy).
+static void mark_items(double* info, int batch) { if (info) for (int b = 0; b < batch; b++) info[3 * (size_t)b + INFO_RC] = RC_ERROR; }
+static void fail_items(const char* fn, const char* msg, double* info, int batch) { fail(fn, msg, nullptr); mark_items(info, batch); }
+
+// The solve (host_io: y and x are host arrays) or, given a tape, the recorded solve and then the tape's header and K table.
+template <typename T>
+static int run_pd_batched(const char* fn, NdSolver s, bool host_io, bool record, const T* y, const double* lambdas, const double* dims, T* x, double* info,
+                          const int* ns, int nds, int npen, int batch, int maxIters, void* tape, size_t tape_bytes, cudaStream_t st) {
+    static const char* const too_small[2] = {"tape_bytes smaller than proxtv_PD2_TV_batched_tape_bytes()",
+                                             "tape_bytes smaller than proxtv_PD_TV_batched_tape_bytes()"};
+    NdTerms t;
+    if (record) {                                      // the order of the single-item record entry points
+        if (!y || !x || !lambdas || !dims || !ns || !tape) { fail_items(fn, "NULL array", info, batch); return 0; }
+        if (batch < 1) { fail_items(fn, "invalid batch (need batch >= 1)", info, batch); return 0; }
+        if (const char* why = nd_args_check(s, ns, nds, npen, dims, &t)) { fail_items(fn, why, info, batch); return 0; }
+        for (int i = 0; i < npen; i++) if (!(lambdas[i] >= 0)) { fail_items(fn, "negative penalty", info, batch); return 0; }
+        const size_t need = nd_tape_bytes(s, ns, nds, npen, maxIters, batch);
+        if (need == 0) { fail_items(fn, "tape size does not fit in size_t (maxIters too large)", info, batch); return 0; }
+        if (tape_bytes < need) { fail_items(fn, too_small[s], info, batch); return 0; }
+        if (!have_device(fn, nullptr)) { mark_items(info, batch); return 0; }
+    } else {                                           // the order of the single-item solve entry points
+        if (!have_device(fn, nullptr)) { mark_items(info, batch); return 0; }
+        if (nds <= 0 || !ns) { fail_items(fn, "invalid dimensions", info, batch); return 0; }
+        if (batch < 1) { fail_items(fn, "invalid batch (need batch >= 1)", info, batch); return 0; }
+        if (!y || !x || (npen > 0 && (!lambdas || !dims))) { fail_items(fn, "NULL array", info, batch); return 0; }
+        if (s == ND_PD2 && npen > 2) { fail_items(fn, "this algorithm can not work with more than 2 penalties", info, batch); return 0; }
+        if (s == ND_PD2 && npen < 1) { fail_items(fn, "invalid penalty dimensions", info, batch); return 0; }
+        if (const char* why = nd_terms(ns, nds, npen, dims, &t)) { fail_items(fn, why, info, batch); return 0; }
+    }
+    const long long n = t.n;
+    WsGuard guard(st);
+    std::vector<double> lam(lambdas ? lambdas : nullptr, lambdas ? lambdas + (npen > 0 ? npen : 0) : nullptr);
+    scale_penalties(s, lam.data(), npen);
+    void* ws = g_ws.get(ws_bytes_pd<T>(n, npen, batch));
+    if (!ws) { fail_items(fn, "out of memory", info, batch); return 0; }
+    std::vector<double> linfo(3 * (size_t)batch);      // the tape's K table needs the rows even when the caller passes no info
+    double* pinfo = info ? info : linfo.data();
+    const size_t nt = (size_t)n * batch;
+    const T* dy = y; T* dx = x;
+    if (host_io && nt > 0) {
+        char* d = (char*)g_io.get(2 * al(nt * sizeof(T)));
+        if (!d) { fail_items(fn, "out of memory", info, batch); return 0; }
+        dy = (T*)d; dx = (T*)(d + al(nt * sizeof(T)));
+        if (!cuda_ok(fn, cudaMemcpyAsync((void*)dy, y, nt * sizeof(T), cudaMemcpyHostToDevice, st), nullptr)) { mark_items(info, batch); return 0; }
+    }
+    const int ok = s == ND_PD2 ? pd2_device<T>(dy, lam.data(), dims, dx, pinfo, ns, nds, npen, maxIters, ws, (Engine)g_engine, st, tape, batch)
+                               : pd_device<T>(dy, lam.data(), dims, dx, pinfo, ns, nds, npen, maxIters, ws, (Engine)g_engine, st, tape, batch);
+    if (!ok) { fail_items(fn, "device solver failed", info, batch); return 0; }
+    if (record && !cuda_ok(fn, nd_tape_header_batched(s, tape, sizeof(T), ns, nds, npen, dims, maxIters, batch, pinfo, st), nullptr)) {
+        mark_items(info, batch); return 0; }
+    if (host_io && nt > 0) {
+        if (!cuda_ok(fn, cudaMemcpyAsync(x, dx, nt * sizeof(T), cudaMemcpyDeviceToHost, st), nullptr) ||
+            !cuda_ok(fn, cudaStreamSynchronize(st), nullptr)) { mark_items(info, batch); return 0; }
+    }
+    return 1;
+}
+
+template <typename T>
+static int dev_nd_vjp_batched(const char* fn, NdSolver s, const int* ns, int nds, int npen, const double* dims, int batch, int maxIters,
+                              const void* tape, const T* gout, T* gY, double* glam, void* stream) {
+    if (!ns || !dims || !tape || !gout || !gY) { fail(fn, "NULL array", nullptr); return 0; }
+    if (batch < 1) { fail(fn, "invalid batch (need batch >= 1)", nullptr); return 0; }
+    NdTerms t;
+    if (const char* why = nd_args_check(s, ns, nds, npen, dims, &t)) { fail(fn, why, nullptr); return 0; }
+    if (!have_device(fn, nullptr)) return 0;
+    WsGuard guard((cudaStream_t)stream);
+    std::vector<int> K(batch);
+    if (const char* why = nd_tape_check_batched(s, tape, sizeof(T), ns, nds, npen, dims, maxIters, batch, K.data(), (cudaStream_t)stream)) {
+        fail(fn, why, nullptr); return 0; }
+    void* ws = g_ws.get(ws_bytes_nd_vjp<T>(t, npen, glam != nullptr, batch));
+    if (!ws) { fail(fn, "out of memory", nullptr); return 0; }
+    return cuda_ok(fn, nd_vjp_device<T>(s, t, npen, maxIters, 0, tape, gout, gY, glam, ws, (cudaStream_t)stream, batch, K.data()), nullptr);
+}
+
+size_t nd_tape_bytes_batched(NdSolver s, const int* ns, int nds, int npen, int batch, int maxIters) {
+    return !ns || batch < 1 || nd_shape_check(s, ns, nds, npen) ? 0 : nd_tape_bytes(s, ns, nds, npen, maxIters, batch);
+}
+
 }  // namespace
 
 extern "C" {
@@ -740,5 +820,66 @@ int proxtv_PD2_TV_vjp_dev_f32(const int* ns, int nds, int npen, const double* di
     return dev_nd_vjp<float>("proxtv_PD2_TV_vjp_dev_f32", ND_PD2, ns, nds, npen, dims, maxIters, iters, tape, gout, gY, glam, stream); }
 int proxtv_PD_TV_f32(const float* y, double* lambdas, double* dims, float* x, double* info, int* ns, int nds, int npen, int maxIters) {
     return run_pd<float>("proxtv_PD_TV_f32", ND_PD, true, y, lambdas, nullptr, dims, x, info, ns, nds, npen, maxIters, 0); }
+
+int proxtv_PD_TV_batched_dev_f64(const double* y, const double* lambdas, const double* dims, double* x, double* info, const int* ns, int nds,
+                                 int npen, int batch, int maxIters, void* stream) {
+    return run_pd_batched<double>("proxtv_PD_TV_batched_dev_f64", ND_PD, false, false, y, lambdas, dims, x, info, ns, nds, npen, batch, maxIters, nullptr, 0,
+                                (cudaStream_t)stream); }
+int proxtv_PD_TV_batched_f64(const double* y, const double* lambdas, const double* dims, double* x, double* info, const int* ns, int nds, int npen,
+                             int batch, int maxIters) {
+    return run_pd_batched<double>("proxtv_PD_TV_batched_f64", ND_PD, true, false, y, lambdas, dims, x, info, ns, nds, npen, batch, maxIters, nullptr, 0, 0); }
+int proxtv_PD_TV_batched_record_dev_f64(const double* y, const double* lambdas, const double* dims, double* x, double* info, const int* ns, int nds,
+                                        int npen, int batch, int maxIters, void* tape, size_t tape_bytes, void* stream) {
+    return run_pd_batched<double>("proxtv_PD_TV_batched_record_dev_f64", ND_PD, false, true, y, lambdas, dims, x, info, ns, nds, npen, batch, maxIters,
+                                tape, tape_bytes, (cudaStream_t)stream); }
+int proxtv_PD_TV_batched_vjp_dev_f64(const int* ns, int nds, int npen, const double* dims, int batch, int maxIters, const void* tape,
+                                     const double* gout, double* gY, double* glam, void* stream) {
+    return dev_nd_vjp_batched<double>("proxtv_PD_TV_batched_vjp_dev_f64", ND_PD, ns, nds, npen, dims, batch, maxIters, tape, gout, gY, glam, stream); }
+int proxtv_PD_TV_batched_dev_f32(const float* y, const double* lambdas, const double* dims, float* x, double* info, const int* ns, int nds,
+                                 int npen, int batch, int maxIters, void* stream) {
+    return run_pd_batched<float>("proxtv_PD_TV_batched_dev_f32", ND_PD, false, false, y, lambdas, dims, x, info, ns, nds, npen, batch, maxIters, nullptr, 0,
+                                (cudaStream_t)stream); }
+int proxtv_PD_TV_batched_f32(const float* y, const double* lambdas, const double* dims, float* x, double* info, const int* ns, int nds, int npen,
+                             int batch, int maxIters) {
+    return run_pd_batched<float>("proxtv_PD_TV_batched_f32", ND_PD, true, false, y, lambdas, dims, x, info, ns, nds, npen, batch, maxIters, nullptr, 0, 0); }
+int proxtv_PD_TV_batched_record_dev_f32(const float* y, const double* lambdas, const double* dims, float* x, double* info, const int* ns, int nds,
+                                        int npen, int batch, int maxIters, void* tape, size_t tape_bytes, void* stream) {
+    return run_pd_batched<float>("proxtv_PD_TV_batched_record_dev_f32", ND_PD, false, true, y, lambdas, dims, x, info, ns, nds, npen, batch, maxIters,
+                                tape, tape_bytes, (cudaStream_t)stream); }
+int proxtv_PD_TV_batched_vjp_dev_f32(const int* ns, int nds, int npen, const double* dims, int batch, int maxIters, const void* tape,
+                                     const float* gout, float* gY, double* glam, void* stream) {
+    return dev_nd_vjp_batched<float>("proxtv_PD_TV_batched_vjp_dev_f32", ND_PD, ns, nds, npen, dims, batch, maxIters, tape, gout, gY, glam, stream); }
+size_t proxtv_PD_TV_batched_tape_bytes(const int* ns, int nds, int npen, int batch, int maxIters) {
+    return nd_tape_bytes_batched(ND_PD, ns, nds, npen, batch, maxIters); }
+int proxtv_PD2_TV_batched_dev_f64(const double* y, const double* lambdas, const double* dims, double* x, double* info, const int* ns, int nds,
+                                 int npen, int batch, int maxIters, void* stream) {
+    return run_pd_batched<double>("proxtv_PD2_TV_batched_dev_f64", ND_PD2, false, false, y, lambdas, dims, x, info, ns, nds, npen, batch, maxIters, nullptr, 0,
+                                (cudaStream_t)stream); }
+int proxtv_PD2_TV_batched_f64(const double* y, const double* lambdas, const double* dims, double* x, double* info, const int* ns, int nds, int npen,
+                             int batch, int maxIters) {
+    return run_pd_batched<double>("proxtv_PD2_TV_batched_f64", ND_PD2, true, false, y, lambdas, dims, x, info, ns, nds, npen, batch, maxIters, nullptr, 0, 0); }
+int proxtv_PD2_TV_batched_record_dev_f64(const double* y, const double* lambdas, const double* dims, double* x, double* info, const int* ns, int nds,
+                                        int npen, int batch, int maxIters, void* tape, size_t tape_bytes, void* stream) {
+    return run_pd_batched<double>("proxtv_PD2_TV_batched_record_dev_f64", ND_PD2, false, true, y, lambdas, dims, x, info, ns, nds, npen, batch, maxIters,
+                                tape, tape_bytes, (cudaStream_t)stream); }
+int proxtv_PD2_TV_batched_vjp_dev_f64(const int* ns, int nds, int npen, const double* dims, int batch, int maxIters, const void* tape,
+                                     const double* gout, double* gY, double* glam, void* stream) {
+    return dev_nd_vjp_batched<double>("proxtv_PD2_TV_batched_vjp_dev_f64", ND_PD2, ns, nds, npen, dims, batch, maxIters, tape, gout, gY, glam, stream); }
+int proxtv_PD2_TV_batched_dev_f32(const float* y, const double* lambdas, const double* dims, float* x, double* info, const int* ns, int nds,
+                                 int npen, int batch, int maxIters, void* stream) {
+    return run_pd_batched<float>("proxtv_PD2_TV_batched_dev_f32", ND_PD2, false, false, y, lambdas, dims, x, info, ns, nds, npen, batch, maxIters, nullptr, 0,
+                                (cudaStream_t)stream); }
+int proxtv_PD2_TV_batched_f32(const float* y, const double* lambdas, const double* dims, float* x, double* info, const int* ns, int nds, int npen,
+                             int batch, int maxIters) {
+    return run_pd_batched<float>("proxtv_PD2_TV_batched_f32", ND_PD2, true, false, y, lambdas, dims, x, info, ns, nds, npen, batch, maxIters, nullptr, 0, 0); }
+int proxtv_PD2_TV_batched_record_dev_f32(const float* y, const double* lambdas, const double* dims, float* x, double* info, const int* ns, int nds,
+                                        int npen, int batch, int maxIters, void* tape, size_t tape_bytes, void* stream) {
+    return run_pd_batched<float>("proxtv_PD2_TV_batched_record_dev_f32", ND_PD2, false, true, y, lambdas, dims, x, info, ns, nds, npen, batch, maxIters,
+                                tape, tape_bytes, (cudaStream_t)stream); }
+int proxtv_PD2_TV_batched_vjp_dev_f32(const int* ns, int nds, int npen, const double* dims, int batch, int maxIters, const void* tape,
+                                     const float* gout, float* gY, double* glam, void* stream) {
+    return dev_nd_vjp_batched<float>("proxtv_PD2_TV_batched_vjp_dev_f32", ND_PD2, ns, nds, npen, dims, batch, maxIters, tape, gout, gY, glam, stream); }
+size_t proxtv_PD2_TV_batched_tape_bytes(const int* ns, int nds, int npen, int batch, int maxIters) {
+    return nd_tape_bytes_batched(ND_PD2, ns, nds, npen, batch, maxIters); }
 
 }  // extern "C"

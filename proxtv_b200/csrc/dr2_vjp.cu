@@ -25,7 +25,10 @@
 // result does not depend on timing.
 #include "ptv_internal.h"
 #include "vjp_core.cuh"
+#include <limits.h>
+#include <stdint.h>
 #include <string.h>
+#include <vector>
 
 namespace ptv {
 
@@ -513,7 +516,8 @@ struct PdrTapeHeader {
     int32_t ns[PDR_TAPE_MAX_DIMS];
     uint8_t axis[64];                                                       // 0-based axis of each term
     int32_t cap;                                                            // PD_TV / PD2_TV: the capacity in iterations; PDR_TV: 0
-    uint8_t pad[256 - 8 - 16 - 4 * PDR_TAPE_MAX_DIMS - 64 - 4];
+    int32_t batch;                                                          // the batched tapes (section 16): the items; else 0
+    uint8_t pad[256 - 8 - 16 - 4 * PDR_TAPE_MAX_DIMS - 64 - 4 - 4];
 };
 static_assert(sizeof(PdrTapeHeader) == 256, "tape header is 256 bytes");
 
@@ -525,6 +529,11 @@ static const NdTapeKind ND_TAPE[3] = {
     {0x3150415452524450ull, "not a PDR_TV tape", MAX_ITERS_DR},             // "PDRRTAP1"
 };
 // the capacity in iterations
+// the batched PD2_TV / PD_TV tapes (section 16), by NdSolver
+static const NdTapeKind ND_TAPE_B[2] = {
+    {0x3150415442324450ull, "not a batched PD2_TV tape", MAX_ITERS_PD},     // "PD2BTAP1"
+    {0x3150415442544450ull, "not a batched PD_TV tape", MAX_ITERS_PD},      // "PDTBTAP1"
+};
 static int nd_cap(NdSolver s, int maxIters) { return maxIters <= 0 ? ND_TAPE[s].default_iters : maxIters; }
 // the iterations the recorded passes come from: PDR_TV runs its capacity, PD_TV and PD2_TV what their stop rule let run
 static int nd_K(NdSolver s, int maxIters, int iters) { return s == ND_PDR ? nd_cap(s, maxIters) : iters; }
@@ -538,20 +547,27 @@ static unsigned long long nd_passes(NdSolver s, int npen, int K) {
     }
 }
 
-// 256 + passes x two bitsets of n-element passes, in 64-bit arithmetic; 0 when that does not fit in size_t
-size_t nd_tape_bytes(NdSolver s, const int* ns, int nds, int npen, int maxIters) {
+size_t nd_tape_head_bytes(int batch) { return 256 + (batch > 0 ? al256((size_t)batch * sizeof(int32_t)) : 0); }
+
+// head + passes x two bitsets of n-element passes (batch >= 1: n batch elements), in 64-bit arithmetic; 0 when that does not fit in size_t
+size_t nd_tape_bytes(NdSolver s, const int* ns, int nds, int npen, int maxIters, int batch) {
     NdTerms t;
     nd_terms(ns, nds, 0, nullptr, &t);
+    if (batch > 0 && t.n > LLONG_MAX / batch) return 0;
     const unsigned long long passes = nd_passes(s, npen, nd_cap(s, maxIters));
-    const unsigned long long set2 = 2ull * (unsigned long long)ptvv::vjp_tape_set_bytes(t.n);
-    if (set2 && passes > (SIZE_MAX - 256) / set2) return 0;
-    return 256 + (size_t)(passes * set2);
+    const unsigned long long set2 = 2ull * (unsigned long long)ptvv::vjp_tape_set_bytes(t.n * (batch > 0 ? batch : 1));
+    const size_t head = nd_tape_head_bytes(batch);
+    if (set2 && passes > (SIZE_MAX - head) / set2) return 0;
+    return head + (size_t)(passes * set2);
 }
 
-template <typename T> cudaError_t pdr_tape_pass(void* tape, long long n, long long p, const T* y, FiberGeom g, T lam, cudaStream_t st) {
-    const size_t sb = ptvv::vjp_tape_set_bytes(n);
-    uint32_t* F = (uint32_t*)((char*)tape + 256 + (size_t)p * 2 * sb);
+template <typename T> cudaError_t nd_tape_pass(void* passes, long long cap_n, long long p, const T* y, FiberGeom g, T lam, cudaStream_t st) {
+    const size_t sb = ptvv::vjp_tape_set_bytes(cap_n);
+    uint32_t* F = (uint32_t*)((char*)passes + (size_t)p * 2 * sb);
     return ptvv::fiber_tape<T>(y, g.nf, g.len, g.inc, lam, nullptr, F, F + sb / 4, st);
+}
+template <typename T> cudaError_t pdr_tape_pass(void* tape, long long n, long long p, const T* y, FiberGeom g, T lam, cudaStream_t st) {
+    return nd_tape_pass<T>((char*)tape + 256, n, p, y, g, lam, st);
 }
 
 // K: the iterations recorded; cap: the capacity (PDR_TV, whose K is its capacity: 0)
@@ -588,22 +604,73 @@ const char* nd_tape_check(NdSolver s, const void* tape, size_t elem, const int* 
     return nullptr;
 }
 
+// The batched tape (section 16): the header with the batched magic, K = the largest item K and `batch`, then the K table
+static PdrTapeHeader nd_header_batched(NdSolver s, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters, int batch,
+                                       int Kmax) {
+    PdrTapeHeader h = nd_header(s, elem, ns, nds, npen, dims, maxIters, Kmax);
+    h.magic = ND_TAPE_B[s].magic;
+    h.batch = batch;
+    return h;
+}
+
+cudaError_t nd_tape_header_batched(NdSolver s, void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters,
+                                   int batch, const double* info, cudaStream_t st) {
+    std::vector<char> head(nd_tape_head_bytes(batch), 0);
+    int32_t* K = (int32_t*)(head.data() + 256);
+    int Kmax = 0;
+    for (int b = 0; b < batch; b++) { K[b] = (int32_t)info[3 * (size_t)b + INFO_ITERS]; if (K[b] > Kmax) Kmax = K[b]; }
+    const PdrTapeHeader h = nd_header_batched(s, elem, ns, nds, npen, dims, maxIters, batch, Kmax);
+    memcpy(head.data(), &h, sizeof(h));
+    // pageable source: the copy is staged before the call returns
+    return cudaMemcpyAsync(tape, head.data(), head.size(), cudaMemcpyHostToDevice, st);
+}
+
+// magic, dtype, shape, terms, capacity, batch, then the K table (every K in 1..cap, the largest the header's K), read back together
+const char* nd_tape_check_batched(NdSolver s, const void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims,
+                                  int maxIters, int batch, int* K, cudaStream_t st) {
+    std::vector<char> head(nd_tape_head_bytes(batch));
+    if (cudaMemcpyAsync(head.data(), tape, head.size(), cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) {
+        cudaGetLastError(); return "cannot read the tape header";
+    }
+    PdrTapeHeader h;
+    memcpy(&h, head.data(), sizeof(h));
+    const PdrTapeHeader w = nd_header_batched(s, elem, ns, nds, npen, dims, maxIters, batch, h.K);
+    if (h.magic != w.magic) return ND_TAPE_B[s].not_ours;
+    if (h.elem != w.elem) return "tape recorded with another dtype";
+    if (h.nds != w.nds || memcmp(h.ns, w.ns, sizeof(h.ns)) != 0) return "tape recorded for another shape";
+    if (h.npen != w.npen || memcmp(h.axis, w.axis, sizeof(h.axis)) != 0) return "tape recorded with other penalty terms";
+    if (h.cap != w.cap) return "tape recorded with another maxIters";
+    if (h.batch != w.batch) return "tape recorded for another batch";
+    int Kmax = 0;
+    memcpy(K, head.data() + 256, (size_t)batch * sizeof(int32_t));
+    for (int b = 0; b < batch; b++) {
+        if (K[b] < 1 || K[b] > h.cap) return "tape holds an invalid iteration count";
+        if (K[b] > Kmax) Kmax = K[b];
+    }
+    if (Kmax != h.K) return "tape holds an invalid iteration count";
+    return nullptr;
+}
+
 template <typename T> struct PdrvPtrs { T* gz[64]; };
 
 // The backward workspace of the three solvers, in order: npen arrays a.gz (PD2_TV: gp, and gq when npen = 2), Sk (PD_TV: Gk; PD2_TV
 // with npen = 1: gq), h, sc, gw (only when glam is wanted), the VJP scratch of the largest term, the double sums.  Returns its size
 // and, unless ws is nullptr, splits ws into *L.
+// batch >= 1 (section 16): every array holds the whole batch, the double sums one set of REDUCE_BLOCKS per item, then the device copies of
+// the slot table and of the slot map.
 template <typename T> struct NdVjpWs {
     PdrvPtrs<T> a;
     T *Sk, *h, *sc, *gw;
     void* vscr;
     double* scratch;
+    int *dslots, *dmap;
 };
-template <typename T> static size_t nd_vjp_ws(const NdTerms& t, int npen, bool want_glam, char* ws, NdVjpWs<T>* L) {
-    const size_t ab = al256((size_t)t.n * sizeof(T));
+template <typename T> static size_t nd_vjp_ws(const NdTerms& t, int npen, bool want_glam, char* ws, NdVjpWs<T>* L, int batch = 0) {
+    const int nb = batch > 0 ? batch : 1;
+    const size_t ab = al256((size_t)(t.n * nb) * sizeof(T));
     size_t vs = 0;
     for (int i = 0; i < npen; i++) {
-        const size_t b = ptvv::vjp_scratch_bytes(t.g[i].nf, t.g[i].len);
+        const size_t b = ptvv::vjp_scratch_bytes(t.g[i].nf * nb, t.g[i].len);
         if (b > vs) vs = b;
     }
     size_t off = 0;
@@ -614,12 +681,14 @@ template <typename T> static size_t nd_vjp_ws(const NdTerms& t, int npen, bool w
     L->sc = (T*)take(ab);
     L->gw = want_glam ? (T*)take(ab) : nullptr;
     L->vscr = take(al256(vs));
-    L->scratch = (double*)take(DR2V_SCRATCH);
+    L->scratch = (double*)take(batch > 0 ? al256((size_t)batch * REDUCE_BLOCKS * sizeof(double)) : DR2V_SCRATCH);
+    L->dslots = batch > 0 ? (int*)take(al256((size_t)batch * sizeof(int))) : nullptr;
+    L->dmap = batch > 0 ? (int*)take(al256((size_t)batch * sizeof(int))) : nullptr;
     return off;
 }
-template <typename T> size_t ws_bytes_nd_vjp(const NdTerms& t, int npen, bool want_glam) {
+template <typename T> size_t ws_bytes_nd_vjp(const NdTerms& t, int npen, bool want_glam, int batch) {
     NdVjpWs<T> L;
-    return nd_vjp_ws<T>(t, npen, want_glam, nullptr, &L);
+    return nd_vjp_ws<T>(t, npen, want_glam, nullptr, &L, batch);
 }
 
 // start: v = G / kk, every gz_l = v.  Else the step after term i's VJP pass (result sc): gz_i = (gz_i - sk) + sc, then h = 2 sk - gz_{i+1}
@@ -721,11 +790,121 @@ __global__ void k_pd2v(int mode, bool more, const T* __restrict__ G, const T* __
     }
 }
 
+// glam[slots[s] npen + i] += the sum of slot s's partials (k_img_final's order and arithmetic, per item)
+__global__ void k_item_final(const double* __restrict__ partial, int nblk, const int* __restrict__ slots, double* __restrict__ glam, int npen,
+                             int i) {
+    double acc = 0.0;
+    for (int q = threadIdx.x; q < nblk; q += blockDim.x) acc += partial[(long long)blockIdx.x * nblk + q];
+    acc = dr2v_block_sum(acc);
+    if (threadIdx.x == 0) {
+        double* g = glam + (long long)slots[blockIdx.x] * npen + i;
+        *g = *g + 1.0 * acc;
+    }
+}
+__global__ void k_scale(double* __restrict__ a, long long n, double f) { GRID_STRIDE(q, n) a[q] = a[q] * f; }
+
+// Batched PD_TV / PD2_TV (section 16): the recurrences above per item, item b over its own K_b = Kb[b].  The adjoint arrays keep the
+// forward's slot order (nd_slots); going down from the largest K, the items with K_b = j + 1 join at iteration j with the start values
+// (PD_TV: a_i = 0, gk = G_b / kk, h = gk - 0; PD2_TV: gp = gq = 0, h = G_b - 0), the others moving to their new slots through sc.  Each
+// pass's edge gradients are summed per item with the single-item call's blocks; glam[b npen + i] of the penalties as given.
 template <typename T>
-cudaError_t nd_vjp_device(NdSolver s, const NdTerms& t, int npen, int maxIters, int iters, const void* tape, const T* gout, T* gY,
-                          double* glam, void* ws, cudaStream_t st) {
+static cudaError_t nd_vjp_items(NdSolver s, const NdTerms& t, int npen, int batch, const int* Kb, const void* tape, const T* gout, T* gY,
+                                double* glam, const NdVjpWs<T>& L, cudaStream_t st) {
 #define RTRY(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) return e__; } while (0)
     const long long n = t.n;
+    const size_t sb = ptvv::vjp_tape_set_bytes(n * batch);
+    const char* tb = (const char*)tape + nd_tape_head_bytes(batch);
+    const T kk = (T)npen;
+    int Kmax = 0;
+    for (int b = 0; b < batch; b++) if (Kb[b] > Kmax) Kmax = Kb[b];
+    // the carried state and how a joining item starts it
+    T* arr[66]; int init[66]; int narr = 0;
+    T* gp = L.a.gz[0];
+    T* gq = npen >= 2 ? L.a.gz[1] : L.Sk;
+    if (s == ND_PD) {
+        for (int i = 0; i < npen; i++) { arr[narr] = L.a.gz[i]; init[narr++] = 0; }
+        arr[narr] = L.Sk; init[narr++] = 1;
+        arr[narr] = L.h; init[narr++] = 2;
+    } else {
+        arr[narr] = gp; init[narr++] = 0;
+        arr[narr] = gq; init[narr++] = 0;
+        arr[narr] = L.h; init[narr++] = 3;
+    }
+    std::vector<int> slots(batch), prev(batch), map(batch);
+    int m = 0;
+    long long nm = 0;
+    auto pass = [&](long long p, int i) -> cudaError_t {
+        const FiberGeom& g = t.g[i];
+        const uint32_t* F = (const uint32_t*)(tb + (size_t)p * 2 * sb);
+        RTRY(ptvv::vjp_fibers_tape<T>(F, F + sb / 4, L.h, L.sc, L.gw, g.nf * m, g.len, g.inc, L.vscr, st));
+        const long long per = g.nf * (long long)(g.len - 1);
+        if (glam && per > 0) {
+            int nblk = (int)((per + 2047) / 2048);
+            if (nblk > REDUCE_BLOCKS) nblk = REDUCE_BLOCKS;
+            KernelSpan span(KC_ELEMENTWISE, 1 + (m + 65534) / 65535, st);
+            for (int s0 = 0; s0 < m; s0 += 65535) {
+                const int ny = m - s0 < 65535 ? m - s0 : 65535;
+                k_img_partial<T><<<dim3(nblk, ny), 256, 0, st>>>(L.gw + (long long)s0 * per, per, L.scratch + (long long)s0 * nblk);
+            }
+            k_item_final<<<m, 256, 0, st>>>(L.scratch, nblk, L.dslots, glam, npen, i);
+            RTRY(cudaGetLastError());
+        }
+        return cudaSuccess;
+    };
+    for (int j = Kmax - 1; j >= 0; j--) {
+        const int m2 = nd_slots(Kb, batch, j, slots.data());
+        if (m2 != m) {                                   // items join: every array to its new slots, the joining items' start values
+            for (int s2 = 0, q = 0; s2 < m2; s2++) map[s2] = (q < m && prev[q] == slots[s2]) ? q++ : -1 - slots[s2];
+            RTRY(cudaMemcpyAsync(L.dmap, map.data(), (size_t)m2 * sizeof(int), cudaMemcpyHostToDevice, st));
+            RTRY(cudaMemcpyAsync(L.dslots, slots.data(), (size_t)m2 * sizeof(int), cudaMemcpyHostToDevice, st));
+            for (int a = 0; a < narr; a++) {
+                RTRY(ew_slot_gather<T>(arr[a], L.sc, L.dmap, m2, n, init[a], gout, kk, st));
+                RTRY(cudaMemcpyAsync(arr[a], L.sc, (size_t)m2 * n * sizeof(T), cudaMemcpyDeviceToDevice, st));
+            }
+            m = m2; nm = n * m; prev.swap(slots);
+        }
+        const unsigned ge = ew_grid(nm);
+        if (s == ND_PD) {
+            for (int i = 0; i < npen; i++) {
+                RTRY(pass((long long)j * npen + i, i));
+                KernelSpan sp(KC_ELEMENTWISE, 1, st);
+                k_pdv<T><<<ge, 256, 0, st>>>(L.a, npen, i, false, j > 0, gout, L.sc, L.Sk, L.h, gY, nm);
+                RTRY(cudaGetLastError());
+            }
+        } else {
+            if (npen >= 2) {
+                RTRY(pass(2LL * j + 1, 1));
+                KernelSpan sp(KC_ELEMENTWISE, 1, st);
+                k_pd2v<T><<<ge, 256, 0, st>>>(1, true, gout, L.sc, gp, gq, L.h, gY, nm);
+                RTRY(cudaGetLastError());
+            }
+            RTRY(pass(npen >= 2 ? 2LL * j : 0, 0));
+            KernelSpan sp(KC_ELEMENTWISE, 1, st);
+            k_pd2v<T><<<ge, 256, 0, st>>>(2, j > 0, gout, L.sc, gp, gq, L.h, gY, nm);
+            RTRY(cudaGetLastError());
+        }
+    }
+    if (glam && s == ND_PD) {                            // d/d of the penalties as given: PD_TV solved with npen lam_i
+        KernelSpan sp(KC_ELEMENTWISE, 1, st);
+        k_scale<<<ew_grid((long long)batch * npen), 256, 0, st>>>(glam, (long long)batch * npen, (double)npen);
+        RTRY(cudaGetLastError());
+    }
+    return cudaSuccess;
+#undef RTRY
+}
+
+template <typename T>
+cudaError_t nd_vjp_device(NdSolver s, const NdTerms& t, int npen, int maxIters, int iters, const void* tape, const T* gout, T* gY,
+                          double* glam, void* ws, cudaStream_t st, int batch, const int* Kb) {
+#define RTRY(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) return e__; } while (0)
+    const long long n = t.n;
+    if (batch > 0) {
+        if (glam) RTRY(cudaMemsetAsync(glam, 0, (size_t)batch * npen * sizeof(double), st));
+        if (n == 0) return cudaSuccess;
+        NdVjpWs<T> L;
+        nd_vjp_ws<T>(t, npen, glam != nullptr, (char*)ws, &L, batch);
+        return nd_vjp_items<T>(s, t, npen, batch, Kb, tape, gout, gY, glam, L, st);
+    }
     const int K = nd_K(s, maxIters, iters);
     if (glam) RTRY(cudaMemsetAsync(glam, 0, (size_t)npen * sizeof(double), st));
     if (n == 0 || K <= 0) return cudaSuccess;
@@ -791,8 +970,10 @@ cudaError_t nd_vjp_device(NdSolver s, const NdTerms& t, int npen, int maxIters, 
 
 #define INST(T) \
     template cudaError_t pdr_tape_pass<T>(void*, long long, long long, const T*, FiberGeom, T, cudaStream_t); \
-    template size_t ws_bytes_nd_vjp<T>(const NdTerms&, int, bool); \
-    template cudaError_t nd_vjp_device<T>(NdSolver, const NdTerms&, int, int, int, const void*, const T*, T*, double*, void*, cudaStream_t); \
+    template cudaError_t nd_tape_pass<T>(void*, long long, long long, const T*, FiberGeom, T, cudaStream_t); \
+    template size_t ws_bytes_nd_vjp<T>(const NdTerms&, int, bool, int); \
+    template cudaError_t nd_vjp_device<T>(NdSolver, const NdTerms&, int, int, int, const void*, const T*, T*, double*, void*, cudaStream_t, \
+                                          int, const int*); \
     template size_t ws_bytes_dr2_record<T>(size_t, size_t, int); \
     template size_t ws_bytes_dr2_vjp<T>(size_t, size_t, int); \
     template cudaError_t dr2_record_device<T>(size_t, size_t, int, int, const T*, T, T, T*, int, void*, void*, Engine, cudaStream_t); \

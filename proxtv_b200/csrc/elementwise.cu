@@ -239,6 +239,182 @@ template <typename T> cudaError_t ew_pd_combine(T* const* dp, T* const* dz, T* c
     return cudaGetLastError();
 }
 
+// ---- the per-item forms of the two stop reductions (batched PD_TV / PD2_TV, DESIGN.md section 16) ----
+// A 2D grid: blockIdx.y = slot s0 + y of the running items, each item n elements at s * n; blockIdx.x = one of the nblk reduction blocks
+// the single-item call uses for n elements, with the same element-to-thread assignment inside the item (element indices, not
+// addresses: a slot that is not 16-byte aligned sums in the order of the aligned single-item call).  partial[s * nblk + x].
+constexpr int MAX_GRID_Y = 65535;
+
+// PD_TV's combine: K 1..4, the vector kernel's assignment (V = 16 / sizeof(T) consecutive elements per thread step, the trailing n % V by
+// block 0's thread 0 after its loop); VLD: the slots are 16-byte aligned, so the V elements load as one vector.  k_pd_combine_items_gen:
+// the generic kernel's assignment (one element per step), k terms, the pointer tables in device memory.
+template <typename T>
+__global__ void k_pd_combine_items_gen(T* const* __restrict__ p, T* const* __restrict__ z, int k, T* __restrict__ x, long long n, int s0,
+                                       double* __restrict__ partial) {
+    const long long base = (long long)(s0 + blockIdx.y) * n;
+    double acc = 0;
+    const T kk = (T)k;
+    for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
+        const long long e = base + q;
+        T xo = x[e], xn = T(0);
+        for (int i = 0; i < k; i++) xn += p[i][e] / kk;
+        for (int i = 0; i < k; i++) z[i][e] += xn - p[i][e];
+        x[e] = xn;
+        acc += fabs((double)xn - (double)xo);
+    }
+    acc = block_sum(acc);
+    if (threadIdx.x == 0) partial[(long long)(s0 + blockIdx.y) * gridDim.x + blockIdx.x] = acc;
+}
+template <typename T, int K, bool VLD>
+__global__ void __launch_bounds__(256, 1) k_pd_combine_items(PdPtrs<T, K> a, T* __restrict__ x, long long n, int s0, double* __restrict__ partial) {
+    const long long base = (long long)(s0 + blockIdx.y) * n;
+    double acc = 0;
+    {
+        constexpr int V = 16 / (int)sizeof(T);
+        struct alignas(16) Vec { T v[V]; };
+        const T kk = (T)K;
+        const long long nv = n / V;
+        for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < nv; q += (long long)gridDim.x * blockDim.x) {
+            const long long e0 = base + q * V;
+            T xo[V], pv[K][V], zv[K][V], xn[V];
+            if constexpr (VLD) {
+                const Vec a0 = *reinterpret_cast<const Vec*>(x + e0);
+#pragma unroll
+                for (int c = 0; c < V; c++) xo[c] = a0.v[c];
+#pragma unroll
+                for (int i = 0; i < K; i++) {
+                    const Vec a1 = *reinterpret_cast<const Vec*>(a.p[i] + e0), a2 = *reinterpret_cast<const Vec*>(a.z[i] + e0);
+#pragma unroll
+                    for (int c = 0; c < V; c++) { pv[i][c] = a1.v[c]; zv[i][c] = a2.v[c]; }
+                }
+            } else {
+#pragma unroll
+                for (int c = 0; c < V; c++) {
+                    xo[c] = x[e0 + c];
+#pragma unroll
+                    for (int i = 0; i < K; i++) { pv[i][c] = a.p[i][e0 + c]; zv[i][c] = a.z[i][e0 + c]; }
+                }
+            }
+#pragma unroll
+            for (int c = 0; c < V; c++) {
+                T s = T(0);
+#pragma unroll
+                for (int i = 0; i < K; i++) s += pv[i][c] / kk;
+#pragma unroll
+                for (int i = 0; i < K; i++) zv[i][c] += s - pv[i][c];
+                xn[c] = s;
+                acc += fabs((double)s - (double)xo[c]);
+            }
+            if constexpr (VLD) {
+#pragma unroll
+                for (int i = 0; i < K; i++) {
+                    Vec o;
+#pragma unroll
+                    for (int c = 0; c < V; c++) o.v[c] = zv[i][c];
+                    *reinterpret_cast<Vec*>(a.z[i] + e0) = o;
+                }
+                Vec o;
+#pragma unroll
+                for (int c = 0; c < V; c++) o.v[c] = xn[c];
+                *reinterpret_cast<Vec*>(x + e0) = o;
+            } else {
+#pragma unroll
+                for (int c = 0; c < V; c++) {
+#pragma unroll
+                    for (int i = 0; i < K; i++) a.z[i][e0 + c] = zv[i][c];
+                    x[e0 + c] = xn[c];
+                }
+            }
+        }
+        if (blockIdx.x == 0 && threadIdx.x == 0)                   // the < V trailing elements of the item
+            for (long long e = base + nv * V; e < base + n; e++) {
+                T xo = x[e], s = T(0);
+                for (int i = 0; i < K; i++) s += a.p[i][e] / kk;
+                for (int i = 0; i < K; i++) a.z[i][e] += s - a.p[i][e];
+                x[e] = s; acc += fabs((double)s - (double)xo);
+            }
+    }
+    acc = block_sum(acc);
+    if (threadIdx.x == 0) partial[(long long)(s0 + blockIdx.y) * gridDim.x + blockIdx.x] = acc;
+}
+// PD2_TV's stop value: k_absdiff_partial per item
+template <typename T> __global__ void k_absdiff_items(const T* __restrict__ a, const T* __restrict__ b, long long n, int s0,
+                                                      double* __restrict__ partial) {
+    const long long base = (long long)(s0 + blockIdx.y) * n;
+    double acc = 0;
+    for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x)
+        acc += fabs((double)a[base + q] - (double)b[base + q]);
+    acc = block_sum(acc);
+    if (threadIdx.x == 0) partial[(long long)(s0 + blockIdx.y) * gridDim.x + blockIdx.x] = acc;
+}
+// k_final_mean per item: block s sums its nblk partials in the single-item order, result[s] = that / n
+__global__ void k_final_mean_items(const double* __restrict__ partial, int nblk, long long n, double* __restrict__ result) {
+    double acc = 0;
+    for (int q = threadIdx.x; q < nblk; q += blockDim.x) acc += partial[(long long)blockIdx.x * nblk + q];
+    acc = block_sum(acc);
+    if (threadIdx.x == 0) result[blockIdx.x] = acc / (double)n;
+}
+
+template <typename T, int K>
+static void launch_pd_items(T* const* hp, T* const* hz, bool vld, T* x, long long n, int s0, int ny, double* scratch, int nblk, cudaStream_t st) {
+    PdPtrs<T, K> a;
+    for (int i = 0; i < K; i++) { a.p[i] = hp[i]; a.z[i] = hz[i]; }
+    if (vld) k_pd_combine_items<T, K, true><<<dim3(nblk, ny), 256, 0, st>>>(a, x, n, s0, scratch);
+    else k_pd_combine_items<T, K, false><<<dim3(nblk, ny), 256, 0, st>>>(a, x, n, s0, scratch);
+}
+template <typename T> cudaError_t ew_pd_combine_items(T* const* dp, T* const* dz, T* const* hp, T* const* hz, int k, T* x, long long n,
+                                                      int items, double* scratch, double* result, cudaStream_t st) {
+    KernelSpan span(KC_ELEMENTWISE, 1 + (items + MAX_GRID_Y - 1) / MAX_GRID_Y, st);
+    // the single-item call's choice for an aligned x and workspace: the vector kernel for 1..4 terms
+    const bool vec = k >= 1 && k <= 4;
+    const bool vld = ((n * (long long)sizeof(T)) & 15) == 0;            // every slot 16-byte aligned (the arrays are)
+    int nblk = vec ? (int)grid_for(n, 256, 16 / (int)sizeof(T) * 2) : (int)grid_for(n, 256, 4);
+    if (nblk > REDUCE_BLOCKS) nblk = REDUCE_BLOCKS;
+    for (int s0 = 0; s0 < items; s0 += MAX_GRID_Y) {
+        const int ny = items - s0 < MAX_GRID_Y ? items - s0 : MAX_GRID_Y;
+        switch (vec ? k : 0) {
+            case 1: launch_pd_items<T, 1>(hp, hz, vld, x, n, s0, ny, scratch, nblk, st); break;
+            case 2: launch_pd_items<T, 2>(hp, hz, vld, x, n, s0, ny, scratch, nblk, st); break;
+            case 3: launch_pd_items<T, 3>(hp, hz, vld, x, n, s0, ny, scratch, nblk, st); break;
+            case 4: launch_pd_items<T, 4>(hp, hz, vld, x, n, s0, ny, scratch, nblk, st); break;
+            default: k_pd_combine_items_gen<T><<<dim3(nblk, ny), 256, 0, st>>>(dp, dz, k, x, n, s0, scratch); break;
+        }
+    }
+    k_final_mean_items<<<items, 256, 0, st>>>(scratch, nblk, n, result);
+    return cudaGetLastError();
+}
+template <typename T> cudaError_t ew_mean_abs_diff_items(const T* a, const T* b, long long n, int items, double* scratch, double* result,
+                                                         cudaStream_t st) {
+    KernelSpan span(KC_ELEMENTWISE, 1 + (items + MAX_GRID_Y - 1) / MAX_GRID_Y, st);
+    int nblk = (int)grid_for(n, 256, 8); if (nblk > REDUCE_BLOCKS) nblk = REDUCE_BLOCKS;
+    for (int s0 = 0; s0 < items; s0 += MAX_GRID_Y) {
+        const int ny = items - s0 < MAX_GRID_Y ? items - s0 : MAX_GRID_Y;
+        k_absdiff_items<T><<<dim3(nblk, ny), 256, 0, st>>>(a, b, n, s0, scratch);
+    }
+    k_final_mean_items<<<items, 256, 0, st>>>(scratch, nblk, n, result);
+    return cudaGetLastError();
+}
+
+// Moves whole n-element slots: dst slot s = src slot map[s] when map[s] >= 0; map[s] = -1 - b: item b joins, with the start value init
+// 0: 0 ; 1: G_b / kk ; 2: G_b / kk - 0 ; 3: G_b - 0 (G_b = G + b n, the expressions of the backward's start steps, dr2_vjp.cu).
+template <typename T> __global__ void k_slot_gather(const T* __restrict__ src, T* __restrict__ dst, const int* __restrict__ map, long long n,
+                                                    long long total, int init, const T* __restrict__ G, T kk) {
+    for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < total; q += (long long)gridDim.x * blockDim.x) {
+        const long long s = q / n, e = q - s * n;
+        const int m = map[s];
+        if (m >= 0) { dst[q] = src[(long long)m * n + e]; continue; }
+        const T g = init ? G[(long long)(-1 - m) * n + e] : T(0);
+        dst[q] = init == 0 ? T(0) : init == 1 ? g / kk : init == 2 ? g / kk - T(0) : g - T(0);
+    }
+}
+template <typename T> cudaError_t ew_slot_gather(const T* src, T* dst, const int* map, int slots, long long n, int init, const T* G, T kk,
+                                                 cudaStream_t st) {
+    KernelSpan span(KC_ELEMENTWISE, 1, st);
+    const long long total = (long long)slots * n;
+    k_slot_gather<T><<<grid_for(total, 256), 256, 0, st>>>(src, dst, map, n, total, init, G, kk);
+    return cudaGetLastError();
+}
+
 // ---- parallel Douglas-Rachford combine (src/TVNDopt.cpp:456-475): q = sum_i p_i/k ; x = sum_i z_i/k (both accumulated term by
 //      term) ; z_i += 2 q - x - p_i ; stop = mean|x - x_old| ----
 template <typename T> __global__ void k_pdr_combine(T* const* __restrict__ p, T* const* __restrict__ z, int k, T* __restrict__ x,
@@ -371,6 +547,9 @@ template <typename T> cudaError_t ew_mean_abs_step(const T* y, long long n, doub
     template cudaError_t ew_mean_abs_diff<T>(const T*, const T*, long long, double*, double*, cudaStream_t); \
     template cudaError_t ew_pd_combine<T>(T* const*, T* const*, T* const*, T* const*, int, T*, long long, double*, double*, cudaStream_t); \
     template cudaError_t ew_pdr_combine<T>(T* const*, T* const*, T* const*, T* const*, int, T*, long long, double*, double*, cudaStream_t); \
+    template cudaError_t ew_pd_combine_items<T>(T* const*, T* const*, T* const*, T* const*, int, T*, long long, int, double*, double*, cudaStream_t); \
+    template cudaError_t ew_mean_abs_diff_items<T>(const T*, const T*, long long, int, double*, double*, cudaStream_t); \
+    template cudaError_t ew_slot_gather<T>(const T*, T*, const int*, int, long long, int, const T*, T, cudaStream_t); \
     template cudaError_t ew_div_scalar<T>(const T*, T*, long long, T, cudaStream_t);
 INST(double)
 INST(float)

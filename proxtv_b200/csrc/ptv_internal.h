@@ -91,6 +91,17 @@ template <typename T> cudaError_t ew_mean_abs_step(const T* y, long long n, doub
 template <typename T> cudaError_t ew_dr_first(const T* Y, const T* t, T* U, T* D, long long n, cudaStream_t st);  // D = t - t ; U = Y - (2 D - t)
 constexpr int REDUCE_BLOCKS = 1184;    // fixed, not the device's SM count (~9 per SM on a 132-SM H100): partial sums are combined in
                                        // the same fixed order on every GPU (deterministic)
+// The per-item stop values of a batched PD_TV / PD2_TV solve (DESIGN.md section 16): `items` running items of n elements in slots 0..items-1
+// of each array; result[s] = the value the single-item call (ew_pd_combine with aligned arrays / ew_mean_abs_diff) computes for slot s,
+// bit for bit.  scratch: items * REDUCE_BLOCKS doubles.
+template <typename T> cudaError_t ew_pd_combine_items(T* const* dp, T* const* dz, T* const* hp, T* const* hz, int k, T* x, long long n,
+                                                      int items, double* scratch, double* result, cudaStream_t st);
+template <typename T> cudaError_t ew_mean_abs_diff_items(const T* a, const T* b, long long n, int items, double* scratch, double* result,
+                                                         cudaStream_t st);
+// dst slot s (n elements) = src slot map[s] (device array), or for map[s] = -1 - b item b's start value (init 0: 0, 1: G_b / kk,
+// 2: G_b / kk - 0, 3: G_b - 0); src and dst must not overlap
+template <typename T> cudaError_t ew_slot_gather(const T* src, T* dst, const int* map, int slots, long long n, int init, const T* G, T kk,
+                                                 cudaStream_t st);
 
 // ---- device-resident solvers (solver.cu).  All arrays are device pointers; `ws` must hold ws_bytes_*() bytes. ----
 template <typename T> size_t ws_bytes_dr2(size_t M, size_t N, int batch);
@@ -126,15 +137,23 @@ struct NdTerms {
 // Fills t: n, then the fibers of term i along its 1-based axis dims[i] (npen = 0: n only).  nullptr when every axis is valid, else the
 // reason: more than 64 terms (no fibers filled) or an axis outside 1..nds.
 const char* nd_terms(const int* ns, int nds, int npen, const double* dims, NdTerms* t);
-// the forward workspace of the three N-D solvers for n elements and npen terms
-template <typename T> size_t ws_bytes_pd(long long n, int npen);
+// the forward workspace of the three N-D solvers for n elements and npen terms; batch >= 1: of the batched PD_TV / PD2_TV solve
+template <typename T> size_t ws_bytes_pd(long long n, int npen, int batch = 0);
+// The slot rule of the batched PD_TV / PD2_TV (DESIGN.md section 16), the one place forward and backward take it from: at iteration j
+// (0-based) the state arrays hold the items {b : K[b] > j}, in increasing b, in slots 0, 1, ...  Writes them to slots (unless nullptr)
+// and returns their count.  The forward runs it with K[b] = INT_MAX for an item that has not stopped yet.
+int nd_slots(const int* K, int batch, int j, int* slots);
 // PD2_TV / PD_TV (proximal Dykstra, stop rule mean|x - x_old| <= STOP_PD).  tape: nullptr, or the recorded forward's buffer (header
-// written by the caller after the call, from info[0]): the segmentation tape of every pass
+// written by the caller after the call, from info[0]): the segmentation tape of every pass.
+// batch = 0: one array (the single-item entry points).  batch >= 1: `batch` items of prod(ns) elements back to back in y and x, each
+// with its own stop rule and info row (info: 3 batch doubles), bit for bit the single-item call on that item under the seq and chunked
+// engines; tape: the batched layout (nd_tape_head_bytes(batch) bytes of header and K table, then passes of batch items each).
 template <typename T> int pd2_device(const T* y, const double* lambdas, const double* dims, T* x, double* info, const int* ns,
-                                     int nds, int npen, int maxIters, void* ws, Engine eng, cudaStream_t st, void* tape = nullptr);
+                                     int nds, int npen, int maxIters, void* ws, Engine eng, cudaStream_t st, void* tape = nullptr,
+                                     int batch = 0);
 template <typename T> int pd_device(const T* y, const double* lambdas_scaled, const double* dims, T* x, double* info,
                                     const int* ns, int nds, int npen, int maxIters, void* ws, Engine eng, cudaStream_t st,
-                                    void* tape = nullptr);
+                                    void* tape = nullptr, int batch = 0);
 // Engine choice under ENGINE_AUTO for data y (device pointer, n elements) and penalty lam: the lane engine keeps every open segment of
 // a fiber inside a 64-row (float64) / 128-row (float32) shared-memory window and sends fibers whose segments outgrow it through a
 // slow exact repair path, so it only pays while segments are short -- lam not larger than about the mean step |y[i+1] - y[i]| of the
@@ -184,21 +203,34 @@ template <typename T> int pdr_device(const T* y, const double* lambdas_scaled, c
 // and PD2_TV stop early, so their tape holds the capacity of maxIters iterations -- maxIters npen passes (PD_TV), 2 maxIters (PD2_TV; 1
 // when npen = 1) -- and the header the iterations run, `iters` (info[0]; ignored for PDR_TV).
 constexpr int PDR_TAPE_MAX_DIMS = 16;                                    // axes the tape header holds
-// header + passes x two bitsets; 0 when the byte count does not fit in size_t
-size_t nd_tape_bytes(NdSolver s, const int* ns, int nds, int npen, int maxIters);
+// header + passes x two bitsets; 0 when the byte count does not fit in size_t.  batch >= 1: the batched PD_TV / PD2_TV tape (section 16),
+// whose passes hold `batch` items each
+size_t nd_tape_bytes(NdSolver s, const int* ns, int nds, int npen, int maxIters, int batch = 0);
+// the bytes before the first pass: the 256-byte header, and for batch >= 1 the K table (batch int32, 256-byte aligned)
+size_t nd_tape_head_bytes(int batch);
 // the tape of pass p (output y over the fibers g, penalty lam) into a tape of n-element passes
 template <typename T> cudaError_t pdr_tape_pass(void* tape, long long n, long long p, const T* y, FiberGeom g, T lam, cudaStream_t st);
+// the same into the passes that start at `passes`, each sized for cap_n elements (y covers the first nf * len of them)
+template <typename T> cudaError_t nd_tape_pass(void* passes, long long cap_n, long long p, const T* y, FiberGeom g, T lam, cudaStream_t st);
 // writes the 256-byte header after the solve (arguments checked by the caller; axes = dims - 1)
 cudaError_t nd_tape_header(NdSolver s, void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters, int iters,
                            cudaStream_t st);
 // validates a tape's header against the arguments (one stream synchronisation): nullptr ok, else the reason
 const char* nd_tape_check(NdSolver s, const void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters,
                           int iters, cudaStream_t st);
-template <typename T> size_t ws_bytes_nd_vjp(const NdTerms& t, int npen, bool want_glam);
+// The batched tape's header and K table (K[b] = info[3 b]), written after the solve; and its check, which also reads the K table into K
+// (batch ints) -- one stream synchronisation for both
+cudaError_t nd_tape_header_batched(NdSolver s, void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters,
+                                   int batch, const double* info, cudaStream_t st);
+const char* nd_tape_check_batched(NdSolver s, const void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims,
+                                  int maxIters, int batch, int* K, cudaStream_t st);
+template <typename T> size_t ws_bytes_nd_vjp(const NdTerms& t, int npen, bool want_glam, int batch = 0);
 // gY, and glam[npen] unless nullptr (PD_TV / PDR_TV: d/d of the scaled penalties; PD2_TV: of the penalties as given), from the tape
-// alone; arguments checked by the caller; workspace ws_bytes_nd_vjp
+// alone; arguments checked by the caller; workspace ws_bytes_nd_vjp.  batch >= 1 (PD_TV / PD2_TV): the batched tape, item b's K = Kb[b]
+// (host), glam[batch][npen] of the penalties as given for both solvers
 template <typename T> cudaError_t nd_vjp_device(NdSolver s, const NdTerms& t, int npen, int maxIters, int iters, const void* tape,
-                                                const T* gout, T* gY, double* glam, void* ws, cudaStream_t st);
+                                                const T* gout, T* gY, double* glam, void* ws, cudaStream_t st, int batch = 0,
+                                                const int* Kb = nullptr);
 
 // ---- CondatChambollePock2_TV (cp2.cu, DESIGN.md section 15): Condat (alg 0), Chambolle-Pock (1) and accelerated Chambolle-Pock (2) ----
 size_t ws_bytes_cp2(size_t M, size_t N, int batch, size_t elem);

@@ -8,7 +8,9 @@
 #include "ptv_internal.h"
 #include "chunk_core.cuh"
 #include <float.h>
+#include <limits.h>
 #include <stdio.h>
+#include <vector>
 
 namespace ptv {
 
@@ -490,11 +492,79 @@ int drw_device(size_t M, size_t N, int batch, int row_major, const T* Y, const T
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-template <typename T> size_t ws_bytes_pd(long long n, int npen) {
+// batch >= 1: the single-item layout for the whole batch, then NdItems' arrays (NdItems::split)
+template <typename T> size_t ws_bytes_pd(long long n, int npen, int batch) {
+    if (batch > 0) return ws_bytes_pd<T>(n * batch, npen, 0) + align256((size_t)(n * batch) * sizeof(T)) +
+                          align256((size_t)batch * REDUCE_BLOCKS * sizeof(double)) + align256((size_t)batch * sizeof(double)) +
+                          align256((size_t)batch * sizeof(int));
     int arrays = 2 * npen + 4;   // PD_TV: p_i, z_i + 3 staging ; PD2_TV (npen <= 2): p, q, z, xl + 3 staging
     if (arrays < 8) arrays = 8;
     return (size_t)arrays * align256((size_t)n * sizeof(T)) + SCRATCH_BYTES + align256(2 * 64 * sizeof(void*));
 }
+
+int nd_slots(const int* K, int batch, int j, int* slots) {
+    int m = 0;
+    for (int b = 0; b < batch; b++)
+        if (K[b] > j) { if (slots) slots[m] = b; m++; }
+    return m;
+}
+
+// The fibers of `items` items of one term's geometry g: an item is the slowest axis, so its fibers are a contiguous range
+static FiberGeom items_geom(const FiberGeom& g, int items) { return FiberGeom{g.nf * items, g.len, g.inc}; }
+
+// The items of a batched PD_TV / PD2_TV solve (DESIGN.md section 16).  K[b] is INT_MAX while item b runs, then the iterations it ran; the
+// running items sit in the slots nd_slots gives them, slots[0..m).  Each iteration's stop values come back in one read-back; an item
+// that stops gets its info row and its x copied to its place in the output, and the others' state arrays move to their new slots through
+// a staging array (the moves of one array overlap, so they cannot be made in place).
+template <typename T> struct NdItems {
+    int batch = 0, m = 0; long long n = 0; T* out = nullptr; double* info = nullptr;
+    std::vector<int> K, slots, next, map; std::vector<double> stop;
+    T* x = nullptr; double* partial = nullptr; double* dstop = nullptr; int* dmap = nullptr;
+    // w: the workspace past the single-item layout of the whole batch (ws_bytes_pd)
+    void split(int b, long long n_, T* out_, double* info_, char* w) {
+        batch = b; m = b; n = n_; out = out_; info = info_;
+        K.assign(b, INT_MAX); slots.resize(b); next.resize(b); map.resize(b); stop.resize(b);
+        nd_slots(K.data(), b, 0, slots.data());
+        if (!w) return;
+        x = (T*)w; w += align256((size_t)(n * b) * sizeof(T));
+        partial = (double*)w; w += align256((size_t)b * REDUCE_BLOCKS * sizeof(double));
+        dstop = (double*)w; w += align256((size_t)b * sizeof(double));
+        dmap = (int*)w;
+    }
+    void row(int b, int iters, double s) {
+        info[3 * (size_t)b + INFO_ITERS] = iters; info[3 * (size_t)b + INFO_GAP] = s;
+        info[3 * (size_t)b + INFO_RC] = iters >= MAX_ITERS_PD ? RC_ITERS : RC_OK;
+    }
+    // after `iters` iterations; go(stop) is the solver's loop condition for one item; arrays[0] is x
+    template <class Go> cudaError_t step(int iters, Go go, T* const* arrays, int narr, T* stage, cudaStream_t st) {
+        cudaError_t e = cudaMemcpyAsync(stop.data(), dstop, (size_t)m * sizeof(double), cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        if (e != cudaSuccess) return e;
+        int gone = 0;
+        for (int s = 0; s < m; s++) {
+            if (go(stop[s])) continue;
+            const int b = slots[s];
+            K[b] = iters; row(b, iters, stop[s]); gone++;
+            e = cudaMemcpyAsync(out + (size_t)b * n, x + (size_t)s * n, (size_t)n * sizeof(T), cudaMemcpyDeviceToDevice, st);
+            if (e != cudaSuccess) return e;
+        }
+        if (!gone) return cudaSuccess;
+        const int m2 = nd_slots(K.data(), batch, iters, next.data());
+        if (m2 > 0) {
+            for (int s2 = 0, s = 0; s2 < m2; s2++) { while (slots[s] != next[s2]) s++; map[s2] = s; }    // both in increasing b
+            e = cudaMemcpyAsync(dmap, map.data(), (size_t)m2 * sizeof(int), cudaMemcpyHostToDevice, st);
+            for (int a = 0; a < narr && e == cudaSuccess; a++) {
+                e = ew_slot_gather<T>(arrays[a], stage, dmap, m2, n, 0, nullptr, T(0), st);
+                if (e == cudaSuccess) e = cudaMemcpyAsync(arrays[a], stage, (size_t)m2 * n * sizeof(T), cudaMemcpyDeviceToDevice, st);
+            }
+            if (e != cudaSuccess) return e;
+        }
+        slots.swap(next); m = m2;
+        return cudaSuccess;
+    }
+    // items that never ran (no elements, no terms): the single-item call's info
+    void rest(int iters) { for (int b = 0; b < batch; b++) if (K[b] == INT_MAX) row(b, iters, DBL_MAX); }
+};
 
 const char* nd_terms(const int* ns, int nds, int npen, const double* dims, NdTerms* t) {
     long long n = 1;
@@ -520,44 +590,60 @@ static int read_stop(const double* dres, double* stop, cudaStream_t st) {
 // tape != nullptr (the recorded forward, dr2_vjp.cu): after each pass the segmentation tape of its output is written -- z as pass
 // 2 iters, x as pass 2 iters + 1 (npen = 1: z as pass 0); nothing else changes.
 template <typename T>
-int pd2_device(const T* y, const double* lambdas, const double* dims, T* x, double* info, const int* ns, int nds, int npen,
-               int maxIters, void* ws, Engine eng, cudaStream_t st, void* tape) {
+int pd2_device(const T* y, const double* lambdas, const double* dims, T* x_out, double* info, const int* ns, int nds, int npen,
+               int maxIters, void* ws, Engine eng, cudaStream_t st, void* tape, int batch) {
     if (npen > 2) { printf("PD2_TV: this algorithm can not work with more than 2 penalties\n");      // :95-96
                     if (info) info[INFO_RC] = RC_ERROR; return 0; }
     NdTerms t;
     const char* why = nd_terms(ns, nds, npen, dims, &t);
     const long long n = t.n;
+    const int nb = batch > 0 ? batch : 1;
     if (maxIters <= 0) maxIters = MAX_ITERS_PD;
-    if (npen >= 1) eng = lane_guard<T>(eng, y, n, npen >= 2 && lambdas[1] > lambdas[0] ? lambdas[1] : lambdas[0], st);
+    if (npen >= 1) eng = lane_guard<T>(eng, y, n * nb, npen >= 2 && lambdas[1] > lambdas[0] ? lambdas[1] : lambdas[0], st);
     if (npen < 1 || why) { printf("PD2_TV: invalid penalty dimensions\n"); if (info) info[INFO_RC] = RC_ERROR; return 0; }
-    const FiberGeom& g0 = t.g[0];
-    const FiberGeom& g1 = t.g[1];                    // npen >= 2 only
     double stop = DBL_MAX; int iters = 0;
+    NdItems<T> I;
     if (n > 0) {
-        char* w = (char*)ws; const size_t ab = align256((size_t)n * sizeof(T));
+        const long long nt = n * nb;
+        char* w = (char*)ws; const size_t ab = align256((size_t)nt * sizeof(T));
         T* p = (T*)w; w += ab; T* q = (T*)w; w += ab; T* z = (T*)w; w += ab; T* xl = (T*)w; w += ab;
         T* scr = (T*)w; w += 3 * ab;                 // staging of strided passes: 2 arrays + per-chunk masks / entering values
         double* scratch = (double*)w; double* dres = scratch + REDUCE_BLOCKS;
-        PTV_TRY(cudaMemcpyAsync(x, y, (size_t)n * sizeof(T), cudaMemcpyDeviceToDevice, st));          // :132-137
-        PTV_TRY(cudaMemsetAsync(p, 0, (size_t)n * sizeof(T), st));
-        PTV_TRY(cudaMemsetAsync(q, 0, (size_t)n * sizeof(T), st));
-        while (stop > STOP_PD && (npen > 1 || !iters) && iters < maxIters) {                           // :157
-            PTV_TRY(cudaMemcpyAsync(xl, x, (size_t)n * sizeof(T), cudaMemcpyDeviceToDevice, st));
-            PTV_TRY(prox_fibers<T>(x, p, IN_A_PLUS_B, z, 0, g0, (T)lambdas[0], nullptr, eng, scr, st, 3 * n));       // :171-208
-            if (tape) PTV_TRY(pdr_tape_pass<T>(tape, n, 2LL * iters, z, g0, (T)lambdas[0], st));
-            PTV_TRY(ew_dual_update<T>(p, x, z, n, st));                                               // :211-213
+        if (batch) I.split(batch, n, x_out, info, (char*)ws + ws_bytes_pd<T>(nt, npen));
+        T* x = batch ? I.x : x_out;                  // a batch iterates in the workspace: an item's x goes out when it stops
+        char* tp = tape ? (char*)tape + nd_tape_head_bytes(batch) : nullptr;
+        T* const state[3] = {x, p, q};
+        PTV_TRY(cudaMemcpyAsync(x, y, (size_t)nt * sizeof(T), cudaMemcpyDeviceToDevice, st));         // :132-137
+        PTV_TRY(cudaMemsetAsync(p, 0, (size_t)nt * sizeof(T), st));
+        PTV_TRY(cudaMemsetAsync(q, 0, (size_t)nt * sizeof(T), st));
+        while (batch ? I.m > 0 : stop > STOP_PD && (npen > 1 || !iters) && iters < maxIters) {        // :157
+            const int m = batch ? I.m : 1;
+            const long long nm = n * m;
+            const FiberGeom g0 = items_geom(t.g[0], m), g1 = npen >= 2 ? items_geom(t.g[1], m) : g0;
+            PTV_TRY(cudaMemcpyAsync(xl, x, (size_t)nm * sizeof(T), cudaMemcpyDeviceToDevice, st));
+            PTV_TRY(prox_fibers<T>(x, p, IN_A_PLUS_B, z, 0, g0, (T)lambdas[0], nullptr, eng, scr, st, 3 * nm));      // :171-208
+            if (tp) PTV_TRY(nd_tape_pass<T>(tp, nt, 2LL * iters, z, g0, (T)lambdas[0], st));
+            PTV_TRY(ew_dual_update<T>(p, x, z, nm, st));                                              // :211-213
             if (npen >= 2) {
-                PTV_TRY(prox_fibers<T>(z, q, IN_A_PLUS_B, x, 0, g1, (T)lambdas[1], nullptr, eng, scr, st, 3 * n));   // :216-258
-                if (tape) PTV_TRY(pdr_tape_pass<T>(tape, n, 2LL * iters + 1, x, g1, (T)lambdas[1], st));
-                PTV_TRY(ew_dual_update<T>(q, z, x, n, st));                                           // :261-263
+                PTV_TRY(prox_fibers<T>(z, q, IN_A_PLUS_B, x, 0, g1, (T)lambdas[1], nullptr, eng, scr, st, 3 * nm));  // :216-258
+                if (tp) PTV_TRY(nd_tape_pass<T>(tp, nt, 2LL * iters + 1, x, g1, (T)lambdas[1], st));
+                PTV_TRY(ew_dual_update<T>(q, z, x, nm, st));                                          // :261-263
             } else {
-                PTV_TRY(cudaMemcpyAsync(x, z, (size_t)n * sizeof(T), cudaMemcpyDeviceToDevice, st));  // :266-269
+                PTV_TRY(cudaMemcpyAsync(x, z, (size_t)nm * sizeof(T), cudaMemcpyDeviceToDevice, st)); // :266-269
+            }
+            if (batch) {                                                                              // :273-277 per item
+                PTV_TRY(ew_mean_abs_diff_items<T>(x, xl, n, m, I.partial, I.dstop, st));
+                iters++;
+                PTV_TRY(I.step(iters, [&](double s) { return s > STOP_PD && npen > 1 && iters < maxIters; }, state, npen >= 2 ? 3 : 2,
+                               scr, st));
+                continue;
             }
             PTV_TRY(ew_mean_abs_diff<T>(x, xl, n, scratch, dres, st));                                // :273-277
             if (!read_stop(dres, &stop, st)) { PTV_TRY(cudaGetLastError()); PTV_TRY(cudaErrorUnknown); }
             iters++;
         }
     }
+    if (batch) { if (!I.batch) I.split(batch, 0, x_out, info, nullptr); I.rest(0); return 1; }
     if (info) { info[INFO_ITERS] = iters; info[INFO_GAP] = stop;
                 info[INFO_RC] = iters >= MAX_ITERS_PD ? RC_ITERS : RC_OK; }                           // :283-295
     return 1;
@@ -567,11 +653,11 @@ int pd2_device(const T* y, const double* lambdas, const double* dims, T* x, doub
 // "<name>: <reason>" on stdout, info[RC] = RC_ERROR, false.
 template <typename T>
 static bool pd_start(const char* name, const T* y, const double* lam, const double* dims, double* info, const int* ns, int nds, int npen,
-                     NdTerms* t, Engine* eng, cudaStream_t st) {
+                     NdTerms* t, Engine* eng, cudaStream_t st, int items = 1) {
     const char* why = nd_terms(ns, nds, npen, dims, t);
     if (npen <= 64) {
         double lmax = 0.0; for (int i = 0; i < npen; i++) if (lam[i] > lmax) lmax = lam[i];
-        *eng = lane_guard<T>(*eng, y, t->n, lmax, st);
+        *eng = lane_guard<T>(*eng, y, t->n * items, lmax, st);
     }
     if (why) { printf("%s: %s\n", name, why); if (info) info[INFO_RC] = RC_ERROR; return false; }
     return true;
@@ -599,30 +685,46 @@ template <typename T> static cudaError_t pd_ws(void* ws, long long n, int npen, 
 // tape != nullptr (the recorded forward, dr2_vjp.cu): after each pass the segmentation tape of its output p_i is written as pass
 // iters * npen + i; nothing else changes.
 template <typename T>
-int pd_device(const T* y, const double* lam, const double* dims, T* x, double* info, const int* ns, int nds, int npen,
-              int maxIters, void* ws, Engine eng, cudaStream_t st, void* tape) {
+int pd_device(const T* y, const double* lam, const double* dims, T* x_out, double* info, const int* ns, int nds, int npen,
+              int maxIters, void* ws, Engine eng, cudaStream_t st, void* tape, int batch) {
     if (maxIters <= 0) maxIters = MAX_ITERS_PD;
+    const int nb = batch > 0 ? batch : 1;
     NdTerms t;
-    if (!pd_start<T>("PD_TV", y, lam, dims, info, ns, nds, npen, &t, &eng, st)) return 0;
-    const long long n = t.n;
+    if (!pd_start<T>("PD_TV", y, lam, dims, info, ns, nds, npen, &t, &eng, st, nb)) return 0;
+    const long long n = t.n, nt = n * nb;
     double stop = DBL_MAX; int iters = 0;
+    NdItems<T> I;
     if (n > 0 && npen > 0) {
         PdWs<T> W;
-        PTV_TRY(pd_ws<T>(ws, n, npen, &W, st));
-        PTV_TRY(cudaMemsetAsync(x, 0, (size_t)n * sizeof(T), st));                                    // :125-130
-        for (int i = 0; i < npen; i++) PTV_TRY(cudaMemcpyAsync(W.hz[i], y, (size_t)n * sizeof(T), cudaMemcpyDeviceToDevice, st));
-        while (stop > STOP_PD && iters < maxIters) {                                                  // :151
+        PTV_TRY(pd_ws<T>(ws, nt, npen, &W, st));
+        if (batch) I.split(batch, n, x_out, info, (char*)ws + ws_bytes_pd<T>(nt, npen));
+        T* x = batch ? I.x : x_out;                  // a batch iterates in the workspace: an item's x goes out when it stops
+        char* tp = tape ? (char*)tape + nd_tape_head_bytes(batch) : nullptr;
+        T* state[65] = {x};
+        for (int i = 0; i < npen; i++) state[1 + i] = W.hz[i];
+        PTV_TRY(cudaMemsetAsync(x, 0, (size_t)nt * sizeof(T), st));                                   // :125-130
+        for (int i = 0; i < npen; i++) PTV_TRY(cudaMemcpyAsync(W.hz[i], y, (size_t)nt * sizeof(T), cudaMemcpyDeviceToDevice, st));
+        while (batch ? I.m > 0 : stop > STOP_PD && iters < maxIters) {                               // :151
+            const int m = batch ? I.m : 1;
             for (int i = 0; i < npen; i++) {
-                PTV_TRY(prox_fibers<T>(W.hz[i], nullptr, IN_A, W.hp[i], 0, t.g[i], (T)lam[i], nullptr, eng, W.scr, st, 3 * n));  // :171-208
-                if (tape) PTV_TRY(pdr_tape_pass<T>(tape, n, (long long)iters * npen + i, W.hp[i], t.g[i], (T)lam[i], st));
+                const FiberGeom g = items_geom(t.g[i], m);
+                PTV_TRY(prox_fibers<T>(W.hz[i], nullptr, IN_A, W.hp[i], 0, g, (T)lam[i], nullptr, eng, W.scr, st, 3 * n * m));  // :171-208
+                if (tp) PTV_TRY(nd_tape_pass<T>(tp, nt, (long long)iters * npen + i, W.hp[i], g, (T)lam[i], st));
+            }
+            if (batch) {                                                                              // :212-227 per item
+                PTV_TRY(ew_pd_combine_items<T>(W.dp, W.dz, W.hp, W.hz, npen, x, n, m, I.partial, I.dstop, st));
+                iters++;
+                PTV_TRY(I.step(iters, [&](double s) { return s > STOP_PD && iters < maxIters; }, state, 1 + npen, W.scr, st));
+                continue;
             }
             PTV_TRY(ew_pd_combine<T>(W.dp, W.dz, W.hp, W.hz, npen, x, n, W.scratch, W.dres, st));             // :212-227
             if (!read_stop(W.dres, &stop, st)) { PTV_TRY(cudaGetLastError()); PTV_TRY(cudaErrorUnknown); }
             iters++;
         }
     } else if (n > 0) {
-        PTV_TRY(cudaMemsetAsync(x, 0, (size_t)n * sizeof(T), st));
+        PTV_TRY(cudaMemsetAsync(x_out, 0, (size_t)nt * sizeof(T), st));
     }
+    if (batch) { if (!I.batch) I.split(batch, 0, x_out, info, nullptr); I.rest(0); return 1; }
     if (info) { info[INFO_ITERS] = iters; info[INFO_GAP] = stop;
                 info[INFO_RC] = iters >= MAX_ITERS_PD ? RC_ITERS : RC_OK; }                           // :233-245
     return 1;
@@ -674,11 +776,11 @@ int pdr_device(const T* y, const double* lam, const double* dims, T* x, double* 
     template int dr2_lane_pick<T>(size_t, size_t, int, int, const T*, const T*, const void*, T, T, Engine, void**); \
     template int drw_device<T>(size_t, size_t, int, int, const T*, const T*, const T*, T*, int, double*, void*, Engine, cudaStream_t); \
     template struct DrwPasses<T>; \
-    template size_t ws_bytes_pd<T>(long long, int); \
+    template size_t ws_bytes_pd<T>(long long, int, int); \
     template int pd2_device<T>(const T*, const double*, const double*, T*, double*, const int*, int, int, int, void*, Engine, cudaStream_t, \
-                               void*); \
+                               void*, int); \
     template int pd_device<T>(const T*, const double*, const double*, T*, double*, const int*, int, int, int, void*, Engine, cudaStream_t, \
-                              void*); \
+                              void*, int); \
     template int pdr_device<T>(const T*, const double*, const double*, T*, double*, const int*, int, int, int, void*, Engine, cudaStream_t, \
                                void*);
 INST(double)
