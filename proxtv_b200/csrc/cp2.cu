@@ -153,9 +153,9 @@ int grid_1d(long long n) { long long b = (n + 255) / 256; return (int)(b < 132 *
 
 // per device: pinned slots for the running-image count of two consecutive checks
 int* pinned_alive() {
-    static int* h[64] = {};
-    int d = 0;
-    if (cudaGetDevice(&d) != cudaSuccess || d < 0 || d >= 64) { cudaGetLastError(); return nullptr; }
+    static int* h[MAX_DEVICES] = {};
+    const int d = device_slot();
+    if (d < 0) return nullptr;
     if (!h[d] && cudaHostAlloc((void**)&h[d], 2 * sizeof(int), cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); h[d] = nullptr; }
     return h[d];
 }

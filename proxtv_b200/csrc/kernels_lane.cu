@@ -714,7 +714,7 @@ void lane_set_tuning(int clen, int halo, int variant) { g_tune.clen = clen; g_tu
 // at group_count + cap_groups) into its arguments, and a regrown buffer may come back at the same address with a larger counter
 // region: `gen` counts the allocations, so that a captured graph can tell a stale layout from the current one (solver.cu: DrGraphKey).
 struct LaneScratch { void* p = nullptr; size_t cap = 0; long long cap_groups = 0; unsigned long long gen = 0; };
-static LaneScratch g_scr[64];
+static LaneScratch g_scr[ptv::MAX_DEVICES];
 static long long lane_scratch_bytes(long long groups_cap, long long nf, int len) {
     const long long nfp = (nf + 31) / 32 * 32 + 32 * 64;
     const long long maxchunks = len / 64 + 2;
@@ -838,8 +838,8 @@ cudaError_t lane_prox(int op, const T* A, const T* B, const T* C, T* X, long lon
     if (a.plan.nmax < 1) a.plan.nmax = 1;
     if (a.plan.nmax > len / 64 + 2) return cudaErrorInvalidConfiguration;
     {
-        int d = 0; cudaGetDevice(&d);
-        if (d < 0 || d >= 64 || scratch != g_scr[d].p || groups > g_scr[d].cap_groups) return cudaErrorInvalidValue;      // not lane_scratch()'s buffer
+        const int d = ptv::device_slot();
+        if (d < 0 || scratch != g_scr[d].p || groups > g_scr[d].cap_groups) return cudaErrorInvalidValue;      // not lane_scratch()'s buffer
         a.stats = (unsigned long long*)scratch;
         a.group_count = (int*)((char*)scratch + 64);
         a.rec = a.group_count + g_scr[d].cap_groups;
@@ -859,7 +859,8 @@ bool lane_shape_ok(long long nf, int len, long long inc, size_t elem, const void
 }
 
 void* lane_scratch(long long nf, int len) {
-    int d = 0; if (cudaGetDevice(&d) != cudaSuccess || d < 0 || d >= 64) return nullptr;
+    const int d = ptv::device_slot();
+    if (d < 0) return nullptr;
     LaneScratch& s = g_scr[d];
     const long long groups = nf + 64;                   // upper bound on the fiber groups of any slicing of nf fibers
     const long long gcap = groups > s.cap_groups ? groups : s.cap_groups;
@@ -872,11 +873,12 @@ void* lane_scratch(long long nf, int len) {
     return s.p;
 }
 unsigned long long lane_scratch_generation() {
-    int d = 0; if (cudaGetDevice(&d) != cudaSuccess || d < 0 || d >= 64) return 0;
-    return g_scr[d].gen;
+    const int d = ptv::device_slot();
+    return d < 0 ? 0 : g_scr[d].gen;
 }
 unsigned long long lane_read_stats(int reset) {
-    int d = 0; if (cudaGetDevice(&d) != cudaSuccess || d < 0 || d >= 64 || !g_scr[d].p) return 0;
+    const int d = ptv::device_slot();
+    if (d < 0 || !g_scr[d].p) return 0;
     unsigned long long v = 0;
     cudaDeviceSynchronize();
     cudaMemcpy(&v, g_scr[d].p, sizeof(v), cudaMemcpyDeviceToHost);

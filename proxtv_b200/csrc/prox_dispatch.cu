@@ -36,10 +36,9 @@ cudaError_t scatter_fibers_sparse(const T* in, const uint32_t* Mk, const T* Cv, 
 long long strided_scratch_elems(long long nf, long long len) { return 2 * nf * len + 2 * nf * ((len + 31) / 32) + 64; }
 
 // outcome of the long-fiber tiles per device, for tests (long_fiber_last in ptv_internal.h); stored + 2, so a slot never written reads -1
-static int g_lf_last_d[64] = {};
-static int lf_slot() { int d = 0; if (cudaGetDevice(&d) != cudaSuccess) { cudaGetLastError(); d = 0; } return (d < 0 || d >= 64) ? 63 : d; }
-void long_fiber_note(int v) { g_lf_last_d[lf_slot()] = v + 2; }
-int long_fiber_last() { const int v = g_lf_last_d[lf_slot()]; return v ? v - 2 : -1; }
+static int g_lf_last_d[MAX_DEVICES] = {};
+void long_fiber_note(int v) { const int d = device_slot(); if (d >= 0) g_lf_last_d[d] = v + 2; }
+int long_fiber_last() { const int d = device_slot(); const int v = d < 0 ? 0 : g_lf_last_d[d]; return v ? v - 2 : -1; }
 
 template <typename T>
 cudaError_t prox_fibers_ex(const T* A, const T* B, const T* C, InOp op, T* X, int out_op, FiberGeom g, T lam, const T* lamv,

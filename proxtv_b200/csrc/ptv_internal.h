@@ -13,6 +13,15 @@ constexpr double STOP_PD = 1e-6;       // src/TVopt.h:71
 constexpr int MAX_ITERS_PD = 35;       // src/TVopt.h:73
 constexpr int MAX_ITERS_DR = 35;       // src/TVopt.h:83
 
+// State kept per device (workspaces, streams, graphs, scratch) lives in tables of MAX_DEVICES slots, indexed by device_slot(): the
+// current device's index, or -1 when there is none or it lies past the table (the caller then refuses, or answers "none").
+constexpr int MAX_DEVICES = 64;
+inline int device_slot() {
+    int d = -1;
+    if (cudaGetDevice(&d) != cudaSuccess) { cudaGetLastError(); return -1; }
+    return d >= 0 && d < MAX_DEVICES ? d : -1;
+}
+
 // The set of 1D fibers of a column-major array along one dimension (src/TVNDopt.cpp:133-138,184-188):
 // fiber j starts at (j / inc) * inc * len + (j % inc) and its elements are `inc` apart.  A leading batch of arrays is
 // simply one more (slowest) dimension.

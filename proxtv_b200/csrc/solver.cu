@@ -69,10 +69,9 @@ struct DrPipe {
     }
 };
 // streams, events and the captured graph belong to one device: one set per device (calls are serialised by the C-ABI mutex)
-static constexpr int MAX_DEV = 64;
-static DrPipe g_pipe_d[MAX_DEV];
-static int cur_dev() { int d = 0; if (cudaGetDevice(&d) != cudaSuccess) { cudaGetLastError(); d = 0; } return (d < 0 || d >= MAX_DEV) ? 0 : d; }
-#define g_pipe (g_pipe_d[cur_dev()])
+static DrPipe g_pipe_d[MAX_DEVICES];
+// the current device's set, ready; nullptr when it cannot be made or the device has no slot (the schedules that need it are then skipped)
+static DrPipe* dev_pipe() { const int d = device_slot(); return d >= 0 && g_pipe_d[d].init() ? &g_pipe_d[d] : nullptr; }
 
 // one iteration (or the final projection pair when `final`): t -> s (cols) -> x (rows); returns false on a CUDA error.
 // Each pass is cut into p.parts pieces issued alternately on two compute streams; the transpose of a piece is queued on
@@ -144,7 +143,7 @@ static int dr2_piped_body(size_t M, size_t N, const T* Y, T w1, T w2, T* out, in
             BTRY(prox_const_fibers<T>(t, (long long)M * N, 1, (int)M, w1, x, st));
             BTRY(ew_dr_reflect_bcast<T>(t, x, s, n, (long long)M * N, gc.len, gc.inc, st));
         }
-        if (!dr_iteration_pipelined<T>(g_pipe, M, N, Y, t, s, final ? out : x, scr, w1, w2, first, final, sparse, st)) {
+        if (!dr_iteration_pipelined<T>(*dev_pipe(), M, N, Y, t, s, final ? out : x, scr, w1, w2, first, final, sparse, st)) {
             BTRY(cudaGetLastError()); return 1; }
         if (!final) { T* tmp = t; t = x; x = tmp; }
     }
@@ -155,12 +154,14 @@ static int dr2_piped_body(size_t M, size_t N, const T* Y, T w1, T w2, T* out, in
 // ------------------------------------------------------------------------------------------------------------------
 // lane_guard (declared in ptv_internal.h): is the lane engine a good choice for this data?
 struct LaneGuardState { const void* y = nullptr; long long n = 0; double lam = 0.0; size_t ts = 0; int ok = -1; double* dev = nullptr; };
-static LaneGuardState g_guard_d[MAX_DEV];
-int lane_guard_last() { return g_guard_d[cur_dev()].ok; }
+static LaneGuardState g_guard_d[MAX_DEVICES];
+int lane_guard_last() { const int d = device_slot(); return d < 0 ? -1 : g_guard_d[d].ok; }
 template <typename T>
 Engine lane_guard(Engine eng, const T* y, long long n, double lam, cudaStream_t st) {
     if (eng != ENGINE_AUTO || n < 2 || !(lam > 0.0)) return eng;
-    LaneGuardState& G = g_guard_d[cur_dev()];
+    const int dev = device_slot();
+    if (dev < 0) return ENGINE_CHUNKED;
+    LaneGuardState& G = g_guard_d[dev];
     {   // evaluated on every call: the same buffer (the C ABI's own staging area, a caller's frame buffer) holds different data each time
         cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
         if (cudaStreamIsCapturing(st, &cap) != cudaSuccess || cap != cudaStreamCaptureStatusNone) { cudaGetLastError(); return eng; }
@@ -279,8 +280,7 @@ struct DrGraphKey {
     }
 };
 struct DrGraph { cudaGraphExec_t exec = nullptr; DrGraphKey key{}; long long launches[KC_COUNT] = {0, 0, 0}; };
-static DrGraph g_dr_graph_d[MAX_DEV];
-#define g_dr_graph (g_dr_graph_d[cur_dev()])
+static DrGraph g_dr_graph_d[MAX_DEVICES];
 
 // ------------------------------------------------------------------------------------------------------------------
 template <typename T> size_t ws_bytes_dr2(size_t M, size_t N, int batch) {
@@ -294,7 +294,7 @@ int dr2_lane_pick(size_t M, size_t N, int batch, int row_major, const T* Y, cons
     *lscr = nullptr;
     const void* lane_ptrs[3] = {Y, out, ws};
     const bool lane_t = eng == ENGINE_LANE_T || row_major;
-    bool lane = (eng == ENGINE_AUTO || eng == ENGINE_LANE || eng == ENGINE_LANE_T) && w1 > T(0) && w2 > T(0) && M >= 2 && N >= 2 && g_pipe.init() &&
+    bool lane = (eng == ENGINE_AUTO || eng == ENGINE_LANE || eng == ENGINE_LANE_T) && w1 > T(0) && w2 > T(0) && M >= 2 && N >= 2 && dev_pipe() &&
                 ptvl::lane_shape_ok((long long)N * batch, (int)M, lane_t ? (long long)N : 1, sizeof(T), lane_ptrs, 3) &&
                 ptvl::lane_shape_ok((long long)M * batch, (int)N, (long long)M, sizeof(T), lane_ptrs, 3) &&
                 (!lane_t || (((long long)M * sizeof(T)) % 16 == 0 && ((long long)N * sizeof(T)) % 16 == 0));
@@ -328,9 +328,9 @@ int dr2_device(size_t M, size_t N, int batch, int row_major, const T* Y, T w1, T
     // The whole solve is captured once into a CUDA graph and replayed while the call's arguments stay the same (no host
     // launch latency); event timing of single launches needs plain launches, so profiling bypasses the graph.
     const bool tpose = eng == ENGINE_TPOSE;
-    const bool tspace = (eng == ENGINE_TSPACE || tpose) && !row_major && M >= 64 && N >= 64 && g_pipe.init();
+    const bool tspace = (eng == ENGINE_TSPACE || tpose) && !row_major && M >= 64 && N >= 64 && dev_pipe();
     const bool piped = (eng == ENGINE_AUTO || eng == ENGINE_PIPELINED) && !row_major && batch == 1 && M >= 1024 && N >= 1024 && M % 2 == 0 && N % 2 == 0 &&
-                       (size_t)((M > N ? M : N) * sizeof(T)) <= 96 * 1024 && g_pipe.init();
+                       (size_t)((M > N ? M : N) * sizeof(T)) <= 96 * 1024 && dev_pipe();
     // lane-per-fiber engine: images whose row pitch suits TMA tiling, positive weights.  Column-major: the staged schedule (column
     // pass over contiguous fibers) or, engine lane-t, the transposed one; row-major: only the transposed schedule applies.
     void* lscr = nullptr;
@@ -347,16 +347,17 @@ int dr2_device(size_t M, size_t N, int batch, int row_major, const T* Y, T w1, T
                        (double)w2, maxit, lane ? lscr : nullptr, lane ? ptvl::lane_scratch_generation() : 0ull};
         int rc = -1;
         if (!profile_is_enabled()) {
-            DrGraph& G = g_dr_graph;
+            DrPipe& P = *dev_pipe();                        // every schedule here took it, so the device has a slot
+            DrGraph& G = g_dr_graph_d[device_slot()];
             if (!(G.exec && G.key == key)) {
                 if (G.exec) { cudaGraphExecDestroy(G.exec); G.exec = nullptr; }
                 long long c0[KC_COUNT], c1[KC_COUNT];
                 profile_counters(c0);
                 cudaGraph_t graph = nullptr;
-                bool okc = cudaStreamBeginCapture(g_pipe.sg, cudaStreamCaptureModeRelaxed) == cudaSuccess;
+                bool okc = cudaStreamBeginCapture(P.sg, cudaStreamCaptureModeRelaxed) == cudaSuccess;
                 if (okc) {
-                    rc = body(g_pipe.sg);
-                    okc = (cudaStreamEndCapture(g_pipe.sg, &graph) == cudaSuccess) && rc == 0 && graph;
+                    rc = body(P.sg);
+                    okc = (cudaStreamEndCapture(P.sg, &graph) == cudaSuccess) && rc == 0 && graph;
                 }
                 if (okc) okc = cudaGraphInstantiate(&G.exec, graph, 0) == cudaSuccess;
                 if (graph) cudaGraphDestroy(graph);
@@ -366,11 +367,11 @@ int dr2_device(size_t M, size_t N, int batch, int row_major, const T* Y, T w1, T
                 if (!okc) { cudaGetLastError(); G.exec = nullptr; } else G.key = key;
             }
             if (G.exec) {
-                PTV_TRY(cudaEventRecord(g_pipe.eIn, st));
-                PTV_TRY(cudaStreamWaitEvent(g_pipe.sg, g_pipe.eIn, 0));
-                PTV_TRY(cudaGraphLaunch(G.exec, g_pipe.sg));
-                PTV_TRY(cudaEventRecord(g_pipe.eOut, g_pipe.sg));
-                PTV_TRY(cudaStreamWaitEvent(st, g_pipe.eOut, 0));
+                PTV_TRY(cudaEventRecord(P.eIn, st));
+                PTV_TRY(cudaStreamWaitEvent(P.sg, P.eIn, 0));
+                PTV_TRY(cudaGraphLaunch(G.exec, P.sg));
+                PTV_TRY(cudaEventRecord(P.eOut, P.sg));
+                PTV_TRY(cudaStreamWaitEvent(st, P.eOut, 0));
                 profile_add(G.launches);
                 if (info) { info[INFO_ITERS] = maxit; info[INFO_RC] = RC_OK; }
                 return 0;
