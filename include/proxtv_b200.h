@@ -206,6 +206,21 @@ int proxtv_CP2_TV_batched_f64(size_t M, size_t N, int batch, int row_major, cons
                               double *info);
 int proxtv_CP2_TV_batched_f32(size_t M, size_t N, int batch, int row_major, const float *Y, double lambda, float *X, int alg, int maxit,
                               double *info);
+/* The weighted form of proxtv_CP2_TV_* (DESIGN.md section 15.1): the same iteration with each dual clipped to its own edge's weight
+ * instead of one lambda -- the converged counterpart of DR2L1W_TV.  W1 weights the edge (i, j)-(i+1, j), W2 the edge (i, j)-(i, j+1);
+ * the maps are back to back per image and laid out like proxtv_DR2L1W_TV_batched_*'s (below), in the images' storage order.  With
+ * every weight equal to lambda the result is proxtv_CP2_TV_*'s bit for bit; a zero weight disconnects its edge.  Weights must be
+ * >= 0 (not checked).  alg 0 (Condat) or 1 (Chambolle-Pock) only: the accelerated rule takes its step sizes from one lambda.
+ * Return values, info rows and the float32 rules as proxtv_CP2_TV_*; also refused (info[2] = 3 for every image): alg 2, W1 NULL
+ * with M > 1, W2 NULL with N > 1. */
+int proxtv_CP2W_TV_dev_f64(size_t M, size_t N, int batch, int row_major, const double *Y, const double *W1, const double *W2,
+                           double *X, int alg, int maxit, double *info, void *stream);
+int proxtv_CP2W_TV_dev_f32(size_t M, size_t N, int batch, int row_major, const float *Y, const float *W1, const float *W2,
+                           float *X, int alg, int maxit, double *info, void *stream);
+int proxtv_CP2W_TV_batched_f64(size_t M, size_t N, int batch, int row_major, const double *Y, const double *W1, const double *W2,
+                               double *X, int alg, int maxit, double *info);
+int proxtv_CP2W_TV_batched_f32(size_t M, size_t N, int batch, int row_major, const float *Y, const float *W1, const float *W2,
+                               float *X, int alg, int maxit, double *info);
 
 /* DR2L1W_TV with device arrays (layouts as above; f32 is an extension the reference lacks). */
 int proxtv_DR2L1W_TV_dev_f64(size_t M, size_t N, const double *Y, const double *W1, const double *W2, double *out, int maxit,

@@ -9,7 +9,7 @@ device the calls raise.
 Extensions the reference lacks (SURVEY.md section 8b): a leading batch dimension (``tv1_1d_batched``,
 ``tv1w_1d_batched``, ``tv1_2d_batched``, ``tv1w_2d_batched``), float32, and torch CUDA tensors as inputs (device-resident path: no PCIe
 traffic, no host transposes -- a C-ordered tensor is handled by swapping the kernels' stride roles).  The batched 1D functions,
-``tv1_2d`` ('dr' and 'pd') / ``tv1_2d_batched`` ('dr'), ``tv1w_2d`` / ``tv1w_2d_batched`` and the N-D ``tvgen`` / ``tvgen_pdr`` are differentiable on torch
+``tv1_2d`` ('dr' and 'pd') / ``tv1_2d_batched`` ('dr'), ``tv1w_2d`` / ``tv1w_2d_batched`` ('dr') and the N-D ``tvgen`` / ``tvgen_pdr`` are differentiable on torch
 tensors (exact backward kernels).
 """
 import ctypes as C
@@ -330,13 +330,19 @@ def tv1_2d(x, w, n_threads=1, max_iters=0, method="dr"):
     return y
 
 
-def tv1w_2d(x, w_col, w_row, max_iters=0, n_threads=1):
+def tv1w_2d(x, w_col, w_row, max_iters=0, n_threads=1, method="dr"):
     r"""2D weighted anisotropic TV-L1 prox by Douglas-Rachford splitting (prox_tv/__init__.py:445-481 -> DR2L1W_TV).
 
     ``w_col``: (M-1, N) weights of the differences along columns, ``w_row``: (M, N-1) along rows.  Same fixed-iteration
     scheme as ``tv1_2d(method='dr')`` (35 iterations unless ``max_iters`` > 0).  ``n_threads`` is ignored.
     numpy input: Fortran-ordered float64 result like the reference.  torch CUDA tensors (float64 / float32, weights of any
     floating dtype on any device): computed on x's device, returns a tensor shaped and typed like ``x``.
+
+    ``method='condat'`` or ``'chambolle-pock'``: the converged weighted prox instead, the primal-dual iteration of
+    ``tv1_2d(method=...)`` with each dual clipped to its own edge's weight, run until X stops changing or ``max_iters`` (0: 2500)
+    (proxtv_CP2W_TV_*, DESIGN.md section 15.1).  With every weight equal to w it is ``tv1_2d(x, w, method=...)`` bit for bit in
+    float64.  torch tensors of either memory order are solved in place of their layout and the result has the solved tensor's
+    layout; these methods have no backward pass.  ``'chambolle-pock-acc'`` is not available: its step rule needs one penalty.
 
     torch: differentiable with respect to ``x``, ``w_col`` and ``w_row``.  With grad mode on and one of them requiring grad, the
     forward records a segmentation tape of every prox pass (2 bits per element per pass, kept on the device until the backward) and
@@ -345,6 +351,8 @@ def tv1w_2d(x, w_col, w_row, max_iters=0, n_threads=1):
     device, and expanded weights (``w.expand(M - 1, N)``), get theirs through ordinary autograd.  The forward result is the same
     either way; double backward is not supported.
     """
+    if _cp2w_method(method):
+        return _cp2w(x, w_col, w_row, max_iters, method, batched=False)
     if _is_torch(x):
         return _drw_torch(x, w_col, w_row, max_iters)
     assert np.all(np.asarray(w_col) >= 0)
@@ -396,7 +404,7 @@ def _drw_solve(Y, W1, W2, geom, tape=None):
     return out
 
 
-def tv1w_2d_batched(x, w_col, w_row, max_iters=0):
+def tv1w_2d_batched(x, w_col, w_row, max_iters=0, method="dr"):
     r"""``tv1w_2d`` on every image of x (B, H, W), with per-image weight maps ``w_col`` (B, H-1, W) (edges along columns) and
     ``w_row`` (B, H, W-1) (edges along rows).  Each image is solved independently with exactly the single-image iteration (its own
     2 * mean start value, 35 iterations unless ``max_iters`` > 0).
@@ -407,7 +415,13 @@ def tv1w_2d_batched(x, w_col, w_row, max_iters=0):
     device are moved to x's device and dtype and laid out like it through ordinary autograd ops.  Differentiable with respect to
     ``x``, ``w_col`` and ``w_row`` like ``tv1w_2d`` (proxtv_DR2L1W_TV_batched_vjp_dev_*, DESIGN.md section 12); an expanded weight
     (``w.expand(B, H - 1, W)``) gets the sum of its per-edge gradients through autograd.
+
+    ``method='condat'`` or ``'chambolle-pock'``: the converged weighted prox of ``tv1w_2d(method=...)`` on every image, each running
+    until its own stop test holds (float32: float32 arithmetic).  Results as above (numpy: C-ordered, x's dtype; torch: the solved
+    tensor's layout); no backward pass.
     """
+    if _cp2w_method(method):
+        return _cp2w(x, w_col, w_row, max_iters, method, batched=True)
     if _is_torch(x):
         return _drw_batched_torch(x, w_col, w_row, max_iters)
     x = np.asarray(x)
@@ -436,15 +450,18 @@ def _drw_batched_torch(x, w_col, w_row, max_iters):
     0: every image's map column-major)."""
     M, N, batch, row_major, xin = _dr2_layout(x, batched=True)
     assert tuple(w_col.shape) == (batch, M - 1, N) and tuple(w_row.shape) == (batch, M, N - 1)
-
-    def lay(w):
-        w = w.to(device=xin.device, dtype=xin.dtype)
-        return w.contiguous() if row_major else w.transpose(1, 2).contiguous().transpose(1, 2)
-    w1, w2 = lay(w_col), lay(w_row)
+    w1, w2 = _drw_lay(w_col, xin, row_major), _drw_lay(w_row, xin, row_major)
     geom = (M, N, batch, row_major, int(max_iters))
     if _needs_grad(x, w_col, w_row):
         return _autograd().DRW.apply(xin, w1, w2, geom)
     return _drw_solve(xin, w1, w2, geom)
+
+
+def _drw_lay(w, xin, row_major):
+    """A weight map (or a batch of them) on xin's device and dtype, laid out like xin's images (row_major = 1: C order; 0: every map
+    column-major), through ordinary autograd ops."""
+    w = w.to(device=xin.device, dtype=xin.dtype)
+    return w.contiguous() if row_major else w.transpose(-2, -1).contiguous().transpose(-2, -1)
 
 
 def _dr2_layout(x, batched):
@@ -559,6 +576,62 @@ def _cp2(x, w, max_iters, method, batched):
         fn = lib.proxtv_CP2_TV_batched_f32 if dt == np.float32 else lib.proxtv_CP2_TV_batched_f64
         ok = fn(H, W, B, 1, _ptr(x), w, _ptr(out), alg, int(max_iters), _ptr(info))
         _check(ok and not np.any(info[2::3] == 3), "CondatChambollePock2_TV (batched)")
+    return out
+
+
+_CP2W_ALGS = {"condat": 0, "chambolle-pock": 1}          # the weighted solver's `alg` (proxtv_CP2W_TV_*)
+
+
+def _cp2w_method(method):
+    """True for the weighted primal-dual methods, False for 'dr'; anything else raises."""
+    if method == "chambolle-pock-acc":
+        raise NotImplementedError("the weighted 2D prox has no 'chambolle-pock-acc': its accelerated step rule takes gamma = 1 / lambda "
+                                  "from one penalty, and per-edge weights give none; use 'condat' or 'chambolle-pock'")
+    assert method == "dr" or method in _CP2W_ALGS, "method must be 'dr', 'condat' or 'chambolle-pock'"
+    return method != "dr"
+
+
+def _cp2w(x, w_col, w_row, max_iters, method, batched):
+    """The weighted primal-dual prox for tv1w_2d / tv1w_2d_batched (proxtv_CP2W_TV_*).  numpy 2D: a Fortran-ordered float64 copy (result
+    Fortran-ordered float64); numpy 3D: the C-ordered (B, H, W) array in x's dtype; torch: either memory order (_dr2_layout), the weight
+    maps laid out to match, result in the solved tensor's layout."""
+    alg = _CP2W_ALGS[method]
+    if _is_torch(x):
+        if _needs_grad(x, w_col, w_row):
+            raise NotImplementedError("tv1w_2d method %r has no backward pass; use method='dr' for gradients, or call it under "
+                                      "torch.no_grad() / on detached tensors" % method)
+        import torch
+        M, N, batch, row_major, xin = _dr2_layout(x, batched)
+        lead = (batch,) if batched else ()
+        assert tuple(w_col.shape) == lead + (M - 1, N) and tuple(w_row.shape) == lead + (M, N - 1)
+        w1, w2 = _drw_lay(w_col, xin, row_major), _drw_lay(w_row, xin, row_major)
+        out = torch.empty_strided(xin.shape, xin.stride(), dtype=xin.dtype, device=xin.device)
+        info = np.zeros(_N_INFO * batch)
+        _dev_call("CP2W_TV_dev", xin, M, N, batch, row_major, xin, w1, w2, out, alg, int(max_iters), info, info=info)
+        return out
+    x = np.asarray(x)
+    assert x.ndim == (3 if batched else 2)
+    assert np.all(np.asarray(w_col) >= 0)
+    assert np.all(np.asarray(w_row) >= 0)
+    if batched:
+        B, M, N = x.shape
+        dt, order, row_major = (np.float32 if x.dtype == np.float32 else np.float64), "C", 1
+    else:
+        B, (M, N) = 1, x.shape
+        dt, order, row_major = np.float64, "F", 0
+    lead = (B,) if batched else ()
+    assert np.shape(w_col) == lead + (M - 1, N)
+    assert np.shape(w_row) == lead + (M, N - 1)
+    x = np.require(x, dt, [order])
+    w1 = np.require(np.asarray(w_col), dt, [order])
+    w2 = np.require(np.asarray(w_row), dt, [order])
+    out = _pool.empty(x.shape, dt, order)
+    if x.size:
+        info = np.zeros(_N_INFO * B)
+        lib = require_device()
+        fn = lib.proxtv_CP2W_TV_batched_f32 if dt == np.float32 else lib.proxtv_CP2W_TV_batched_f64
+        ok = fn(M, N, B, row_major, _ptr(x), _ptr(w1), _ptr(w2), _ptr(out), alg, int(max_iters), _ptr(info))
+        _check(ok and not np.any(info[2::3] == 3), "proxtv_CP2W_TV_batched")
     return out
 
 

@@ -202,16 +202,18 @@ int run_drw(const char* fn, bool host_io, size_t M, size_t N, int batch, int row
 
 // CondatChambollePock2_TV with host (host_io) or device arrays: `batch` images back to back, column-major (row_major = 0) or C order
 // (1); info: host, 3 doubles per image, or NULL.  Returns 1 on success, 0 on failure (src/TV2Dopt.cpp:600-602, :750-756).  A
-// refusal marks every image's row (the first one when batch < 1).
+// refusal marks every image's row (the first one when batch < 1).  weighted (DESIGN.md section 15.1): per-edge maps W1, W2 laid out
+// like run_drw's instead of lambda, alg 0 or 1.
 template <typename T>
-int run_cp2(const char* fn, bool host_io, size_t M, size_t N, int batch, int row_major, const T* Y, double lambda, T* X, int alg, int maxit,
-            double* info, cudaStream_t st) {
+int run_cp2(const char* fn, bool host_io, size_t M, size_t N, int batch, int row_major, const T* Y, double lambda, bool weighted,
+            const T* W1, const T* W2, T* X, int alg, int maxit, double* info, cudaStream_t st) {
     const Refuse no{fn, info, batch > 1 ? batch : 1};
+    if (weighted && alg == 2) return no("the weighted solver has no accelerated variant (alg 2); use alg 0 or 1");
     if (alg != 0 && alg != 1 && alg != 2) return no("Algorithm parameter has an invalid value");
     if (batch < 0) return no("invalid shape (need batch >= 0)");
     if (batch == 0) return 1;
     if (M < 1 || N < 1 || M > 0x7fffffff || N > 0x7fffffff) return no("invalid shape (need 1 <= M, N < 2^31)");
-    if (!Y || !X) return no("NULL array");
+    if (!Y || !X || (weighted && ((M > 1 && !W1) || (N > 1 && !W2)))) return no("NULL array");
     if (!no.have_device()) return 0;
     WsGuard guard(st);
     const size_t n = M * N * (size_t)batch;
@@ -219,11 +221,14 @@ int run_cp2(const char* fn, bool host_io, size_t M, size_t N, int batch, int row
     if (!ws) return no("out of memory");
     HostIO<T> io(no, st);
     if (host_io) {
-        io.in(Y, n); io.out(X, n);
+        io.in(Y, n);
+        if (weighted) { io.in(W1, (M - 1) * N * (size_t)batch); io.in(W2, M * (N - 1) * (size_t)batch); }
+        io.out(X, n);
         if (!io.stage()) return 0;
     }
     std::vector<int> iters(info ? batch : 0);
-    if (!no.cuda_ok(cp2_device<T>(M, N, batch, row_major, Y, lambda, X, alg, maxit, info ? iters.data() : nullptr, ws, st))) return 0;
+    if (!no.cuda_ok(cp2_device<T>(M, N, batch, row_major, Y, lambda, weighted, W1, W2, X, alg, maxit, info ? iters.data() : nullptr, ws, st)))
+        return 0;
     if (!io.finish()) return 0;
     if (info) for (int b = 0; b < batch; b++) { info[3 * (size_t)b + INFO_ITERS] = iters[b]; info[3 * (size_t)b + INFO_RC] = RC_OK; }
     return 1;
@@ -627,7 +632,7 @@ int DR2L1W_TV(size_t M, size_t N, double* unary, double* W1, double* W2, double*
     return run_drw<double>("DR2L1W_TV", true, M, N, 1, 0, unary, W1, W2, s, maxit, info, 0);
 }
 int CondatChambollePock2_TV(size_t M, size_t N, double* Y, double lambda, double* X, short alg, int maxit, double* info) {
-    return run_cp2<double>("Condat2_TV", true, M, N, 1, 0, Y, lambda, X, alg, maxit, info, 0);
+    return run_cp2<double>("Condat2_TV", true, M, N, 1, 0, Y, lambda, false, nullptr, nullptr, X, alg, maxit, info, 0);
 }
 int PD2_TV(double* y, double* lambdas, double* norms, double* dims, double* x, double* info, int* ns, int nds, int npen, int,
            int maxIters) {
@@ -705,16 +710,31 @@ int proxtv_DR2_TV_batched_f32(size_t M, size_t N, int batch, const float* Y, flo
 
 int proxtv_CP2_TV_dev_f64(size_t M, size_t N, int batch, int row_major, const double* Y, double lambda, double* X, int alg, int maxit,
                           double* info, void* stream) {
-    return run_cp2<double>("proxtv_CP2_TV_dev_f64", false, M, N, batch, row_major, Y, lambda, X, alg, maxit, info, (cudaStream_t)stream); }
+    return run_cp2<double>("proxtv_CP2_TV_dev_f64", false, M, N, batch, row_major, Y, lambda, false, nullptr, nullptr,
+                           X, alg, maxit, info, (cudaStream_t)stream); }
 int proxtv_CP2_TV_dev_f32(size_t M, size_t N, int batch, int row_major, const float* Y, double lambda, float* X, int alg, int maxit,
                           double* info, void* stream) {
-    return run_cp2<float>("proxtv_CP2_TV_dev_f32", false, M, N, batch, row_major, Y, lambda, X, alg, maxit, info, (cudaStream_t)stream); }
+    return run_cp2<float>("proxtv_CP2_TV_dev_f32", false, M, N, batch, row_major, Y, lambda, false, nullptr, nullptr,
+                           X, alg, maxit, info, (cudaStream_t)stream); }
 int proxtv_CP2_TV_batched_f64(size_t M, size_t N, int batch, int row_major, const double* Y, double lambda, double* X, int alg, int maxit,
                               double* info) {
-    return run_cp2<double>("proxtv_CP2_TV_batched_f64", true, M, N, batch, row_major, Y, lambda, X, alg, maxit, info, 0); }
+    return run_cp2<double>("proxtv_CP2_TV_batched_f64", true, M, N, batch, row_major, Y, lambda, false, nullptr, nullptr, X, alg, maxit, info, 0); }
 int proxtv_CP2_TV_batched_f32(size_t M, size_t N, int batch, int row_major, const float* Y, double lambda, float* X, int alg, int maxit,
                               double* info) {
-    return run_cp2<float>("proxtv_CP2_TV_batched_f32", true, M, N, batch, row_major, Y, lambda, X, alg, maxit, info, 0); }
+    return run_cp2<float>("proxtv_CP2_TV_batched_f32", true, M, N, batch, row_major, Y, lambda, false, nullptr, nullptr, X, alg, maxit, info, 0); }
+
+int proxtv_CP2W_TV_dev_f64(size_t M, size_t N, int batch, int row_major, const double* Y, const double* W1, const double* W2, double* X,
+                           int alg, int maxit, double* info, void* stream) {
+    return run_cp2<double>("proxtv_CP2W_TV_dev_f64", false, M, N, batch, row_major, Y, 0., true, W1, W2, X, alg, maxit, info, (cudaStream_t)stream); }
+int proxtv_CP2W_TV_dev_f32(size_t M, size_t N, int batch, int row_major, const float* Y, const float* W1, const float* W2, float* X,
+                           int alg, int maxit, double* info, void* stream) {
+    return run_cp2<float>("proxtv_CP2W_TV_dev_f32", false, M, N, batch, row_major, Y, 0., true, W1, W2, X, alg, maxit, info, (cudaStream_t)stream); }
+int proxtv_CP2W_TV_batched_f64(size_t M, size_t N, int batch, int row_major, const double* Y, const double* W1, const double* W2,
+                               double* X, int alg, int maxit, double* info) {
+    return run_cp2<double>("proxtv_CP2W_TV_batched_f64", true, M, N, batch, row_major, Y, 0., true, W1, W2, X, alg, maxit, info, 0); }
+int proxtv_CP2W_TV_batched_f32(size_t M, size_t N, int batch, int row_major, const float* Y, const float* W1, const float* W2, float* X,
+                               int alg, int maxit, double* info) {
+    return run_cp2<float>("proxtv_CP2W_TV_batched_f32", true, M, N, batch, row_major, Y, 0., true, W1, W2, X, alg, maxit, info, 0); }
 
 int proxtv_DR2L1W_TV_dev_f64(size_t M, size_t N, const double* Y, const double* W1, const double* W2, double* out, int maxit, double* info, void* stream) {
     return run_drw<double>("proxtv_DR2L1W_TV_dev_f64", false, M, N, 1, 0, Y, W1, W2, out, maxit, info, (cudaStream_t)stream); }

@@ -13,6 +13,11 @@
 // Storage: both memory orders of an M x N image are an F x S array with the F axis contiguous (column-major: F = M, S = N;
 // row-major: F = N, S = M); only the roles of the two difference terms swap, and D = a + b is commutative in IEEE arithmetic, so
 // both orders give the same bits.  The duals are stored padded to F x S (the last row of Uf, the last column of Us unused).
+//
+// Weighted (DESIGN.md section 15.1, alg 0 and 1 only): each dual is clipped to its own edge's weight instead of lambda.  The caller's
+// maps are read in place: in F x S terms they are an (F-1) x S map Wf of the edges along F and an F x (S-1) map Ws of the edges
+// along S, both F-contiguous (column-major: Wf = W1, Ws = W2; C order: Wf = W2, Ws = W1), so the weight of the dual at q = b F S +
+// f + F s is Wf[q - (b S + s)] and Ws[q - b F].
 #include "ptv_internal.h"
 #include <math.h>
 #include <stdio.h>
@@ -49,10 +54,12 @@ __device__ __forceinline__ bool keeps_running(const double* sums, int batch, int
     return sqrt(num / den) > 0;
 }
 
-template <typename T>
+// WTD: clip each dual to its edge's weight in Wf / Ws (lam unused); else to lam (Wf, Ws unused)
+template <typename T, bool WTD>
 __global__ void __launch_bounds__(THREADS, 3) k_cp2_iter(Geom g, const T* __restrict__ Y, const T* __restrict__ X,
                                                          const T* __restrict__ Uf, const T* __restrict__ Us, T* __restrict__ Xn,
-                                                         T* __restrict__ Ufn, T* __restrict__ Usn, int* stopped, double* sums, int it, int alg, T tau, T c, T theta, T sigma, T lam) {
+                                                         T* __restrict__ Ufn, T* __restrict__ Usn, int* stopped, double* sums, int it, int alg, T tau, T c, T theta, T sigma, T lam,
+                                                         const T* __restrict__ Wf, const T* __restrict__ Ws) {
     __shared__ T zs[CELLS];
     __shared__ double red[THREADS / 32][2];
     const int tid = threadIdx.x;
@@ -98,8 +105,8 @@ __global__ void __launch_bounds__(THREADS, 3) k_cp2_iter(Geom g, const T* __rest
             const int lf = p % HF, ls = p / HF, f = f0 + lf, s = s0 + ls;
             if (p >= CELLS || lf >= TF || ls >= TS || f >= F || s >= S) continue;
             const long long q = base + f + (long long)F * s;
-            if (f < F - 1) Ufn[q] = clip<T>(ufv[k] + sigma * (zs[p + 1] - zv[k]), lam);
-            if (s < S - 1) Usn[q] = clip<T>(usv[k] + sigma * (zs[p + HF] - zv[k]), lam);
+            if (f < F - 1) Ufn[q] = clip<T>(ufv[k] + sigma * (zs[p + 1] - zv[k]), WTD ? Wf[q - ((long long)b * S + s)] : lam);
+            if (s < S - 1) Usn[q] = clip<T>(usv[k] + sigma * (zs[p + HF] - zv[k]), WTD ? Ws[q - (long long)b * F] : lam);
         }
         for (int o = 16; o > 0; o >>= 1) { num += __shfl_down_sync(0xffffffffu, num, o); den += __shfl_down_sync(0xffffffffu, den, o); }
         if ((tid & 31) == 0) { red[tid >> 5][0] = num; red[tid >> 5][1] = den; }
@@ -168,8 +175,8 @@ size_t ws_bytes_cp2(size_t M, size_t N, int batch, size_t elem) {
 }
 
 template <typename T>
-cudaError_t cp2_device(size_t M, size_t N, int batch, int row_major, const T* Y, double lambda, T* out, int alg, int maxit, int* iters,
-                       void* ws, cudaStream_t st) {
+cudaError_t cp2_device(size_t M, size_t N, int batch, int row_major, const T* Y, double lambda, bool weighted, const T* W1, const T* W2,
+                       T* out, int alg, int maxit, int* iters, void* ws, cudaStream_t st) {
     Geom g;
     g.F = (int)(row_major ? N : M); g.S = (int)(row_major ? M : N);
     g.img = (long long)M * (long long)N; g.batch = batch;
@@ -183,6 +190,8 @@ cudaError_t cp2_device(size_t M, size_t N, int batch, int row_major, const T* Y,
     int* stopped = (int*)w; w += align256((size_t)batch * sizeof(int));
     double* sums = (double*)w; w += align256(3 * (size_t)batch * SLOTS * 2 * sizeof(double));
     int* d_alive = (int*)w;
+    const T* Wf = row_major ? W2 : W1;
+    const T* Ws = row_major ? W1 : W2;
     int* h_alive = pinned_alive();
     if (!h_alive) return cudaErrorMemoryAllocation;
     cudaEvent_t ev[2];
@@ -207,8 +216,12 @@ cudaError_t cp2_device(size_t M, size_t N, int batch, int row_major, const T* Y,
                 const double cc = 1. / (1. + tau), tau_i = tau, theta_i = theta;
                 if (alg == 2) { tau *= theta; sigma /= theta; theta = 1. / sqrt(1 + 2 * gamma * tau); }
                 const int r = (it - 1) & 1, wr = it & 1;
-                k_cp2_iter<T><<<grid, THREADS, 0, st>>>(g, Y, Xb[r], Ufb[r], Usb[r], Xb[wr], Ufb[wr], Usb[wr], stopped, sums, it, alg,
-                                                        (T)tau_i, (T)cc, (T)theta_i, (T)sigma, (T)lambda);
+                if (weighted)
+                    k_cp2_iter<T, true><<<grid, THREADS, 0, st>>>(g, Y, Xb[r], Ufb[r], Usb[r], Xb[wr], Ufb[wr], Usb[wr], stopped, sums, it, alg,
+                                                                  (T)tau_i, (T)cc, (T)theta_i, (T)sigma, T(0), Wf, Ws);
+                else
+                    k_cp2_iter<T, false><<<grid, THREADS, 0, st>>>(g, Y, Xb[r], Ufb[r], Usb[r], Xb[wr], Ufb[wr], Usb[wr], stopped, sums, it, alg,
+                                                                   (T)tau_i, (T)cc, (T)theta_i, (T)sigma, (T)lambda, nullptr, nullptr);
                 CP2_TRY(cudaGetLastError());
             }
             if (it > maxit) break;
@@ -237,7 +250,9 @@ done:
     return err;
 }
 
-template cudaError_t cp2_device<double>(size_t, size_t, int, int, const double*, double, double*, int, int, int*, void*, cudaStream_t);
-template cudaError_t cp2_device<float>(size_t, size_t, int, int, const float*, double, float*, int, int, int*, void*, cudaStream_t);
+template cudaError_t cp2_device<double>(size_t, size_t, int, int, const double*, double, bool, const double*, const double*, double*, int,
+                                        int, int*, void*, cudaStream_t);
+template cudaError_t cp2_device<float>(size_t, size_t, int, int, const float*, double, bool, const float*, const float*, float*, int, int,
+                                       int*, void*, cudaStream_t);
 
 }  // namespace ptv

@@ -245,10 +245,12 @@ template <typename T> cudaError_t nd_vjp_device(NdSolver s, const NdTerms& t, in
 size_t ws_bytes_cp2(size_t M, size_t N, int batch, size_t elem);
 // `batch` M x N images back to back, column-major (row_major = 0) or C order (1); alg in 0..2 (checked by the caller); maxit <= 0:
 // 2500.  iters: nullptr, or host memory for each image's final `it` (iterations run + 1; the call then synchronises the stream).
-// Reads the running-image count back every 64 iterations (one stream synchronisation each).
+// Reads the running-image count back every 64 iterations (one stream synchronisation each).  weighted (section 15.1; alg 0 or 1,
+// lambda unused): each dual is clipped to its edge's weight in W1 ((M-1) x N per image) / W2 (M x (N-1)), device maps laid out like
+// proxtv_DR2L1W_TV_batched_*'s; W1 may be nullptr when M == 1, W2 when N == 1.  The workspace is the same either way.
 template <typename T>
-cudaError_t cp2_device(size_t M, size_t N, int batch, int row_major, const T* Y, double lambda, T* out, int alg, int maxit, int* iters,
-                       void* ws, cudaStream_t st);
+cudaError_t cp2_device(size_t M, size_t N, int batch, int row_major, const T* Y, double lambda, bool weighted, const T* W1, const T* W2,
+                       T* out, int alg, int maxit, int* iters, void* ws, cudaStream_t st);
 
 }  // namespace ptv
 
