@@ -221,6 +221,41 @@ int proxtv_CP2W_TV_batched_f64(size_t M, size_t N, int batch, int row_major, con
                                double *X, int alg, int maxit, double *info);
 int proxtv_CP2W_TV_batched_f32(size_t M, size_t N, int batch, int row_major, const float *Y, const float *W1, const float *W2,
                                float *X, int alg, int maxit, double *info);
+/* Backward pass of the converged solves proxtv_CP2_TV_* / proxtv_CP2W_TV_* (DESIGN.md section 15.2), alg 0 and 1.  It is not the
+ * derivative of the iterations computed but the Jacobian of the prox itself at the partition the forward reached, so it is right
+ * when the forward has converged.  An edge e = (i, j), j the successor of i along its axis, is FUSED iff its weight w_e (lambda, or its
+ * entry of W1 / W2) is > 0 and either |U_e| < w_e for the final dual U_e of the image's last iteration or X_i == X_j as stored; a NaN
+ * never fuses.  Clusters are the 4-connected components of the fused edges, per image.
+ * record: the _dev_ call, bit for bit the same X and info, then a fused-edge tape into the device buffer `tape` (at least
+ * proxtv_CP2_TV_tape_bytes() bytes, the same size for both forms): a 256-byte header (dtype, M, N, batch, row_major, weighted) and
+ * two bitsets in storage order (bit q: q fused with its successor along the contiguous axis; along the strided axis), each laid out
+ * like proxtv_fiber_tape_dev_*'s.  Returns 1 ok / 0 error (info[2] = 3 for every image); refused without writing anything else: alg
+ * 2, an invalid alg, M, N or batch < 1, M N >= 2^31, Y, X, tape (or a needed weight map) NULL, a negative lambda, tape_bytes too
+ * small.
+ * vjp: from the tape, the recorded result X and the upstream gradient gout (both laid out like X): gY = the cluster means of gout,
+ * gY_i = (T)(S_C / |C|) with S_C the sum of (double) gout over i's cluster C; per-edge gW1 / gW2 (weighted form, laid out like W1 / W2,
+ * each may be NULL) = (T)(sgn(X_j - X_i) ((double) gY_i - (double) gY_j)) on cut edges and +0 on fused ones; unless glam is NULL,
+ * glam = 2 * batch doubles, per image [sum of those edge gradients along axis 0, along axis 1] (the gradient of lambda per axis).
+ * Deterministic: S_C is summed exactly in fixed point and rounded once, glam in a fixed order; the same bits in both storage orders.
+ * Synchronises the stream once (reads the tape's header).  Returns 1 ok / 0 error; refused without writing anything: M, N or batch <
+ * 1, M N >= 2^31, tape, X, gout or gY NULL, a header that does not match the arguments (dtype, shape, batch, row_major, weighted). */
+size_t proxtv_CP2_TV_tape_bytes(size_t M, size_t N, int batch);
+int proxtv_CP2_TV_record_dev_f64(size_t M, size_t N, int batch, int row_major, const double *Y, double lambda, double *X, int alg,
+                                 int maxit, double *info, void *tape, size_t tape_bytes, void *stream);
+int proxtv_CP2_TV_record_dev_f32(size_t M, size_t N, int batch, int row_major, const float *Y, double lambda, float *X, int alg,
+                                 int maxit, double *info, void *tape, size_t tape_bytes, void *stream);
+int proxtv_CP2W_TV_record_dev_f64(size_t M, size_t N, int batch, int row_major, const double *Y, const double *W1, const double *W2,
+                                  double *X, int alg, int maxit, double *info, void *tape, size_t tape_bytes, void *stream);
+int proxtv_CP2W_TV_record_dev_f32(size_t M, size_t N, int batch, int row_major, const float *Y, const float *W1, const float *W2,
+                                  float *X, int alg, int maxit, double *info, void *tape, size_t tape_bytes, void *stream);
+int proxtv_CP2_TV_vjp_dev_f64(size_t M, size_t N, int batch, int row_major, const void *tape, const double *X, const double *gout,
+                              double *gY, double *glam, void *stream);
+int proxtv_CP2_TV_vjp_dev_f32(size_t M, size_t N, int batch, int row_major, const void *tape, const float *X, const float *gout,
+                              float *gY, double *glam, void *stream);
+int proxtv_CP2W_TV_vjp_dev_f64(size_t M, size_t N, int batch, int row_major, const void *tape, const double *X, const double *gout,
+                               double *gY, double *gW1, double *gW2, double *glam, void *stream);
+int proxtv_CP2W_TV_vjp_dev_f32(size_t M, size_t N, int batch, int row_major, const void *tape, const float *X, const float *gout,
+                               float *gY, float *gW1, float *gW2, double *glam, void *stream);
 
 /* DR2L1W_TV with device arrays (layouts as above; f32 is an extension the reference lacks). */
 int proxtv_DR2L1W_TV_dev_f64(size_t M, size_t N, const double *Y, const double *W1, const double *W2, double *out, int maxit,

@@ -10,7 +10,8 @@ Extensions the reference lacks (SURVEY.md section 8b): a leading batch dimension
 ``tv1w_1d_batched``, ``tv1_2d_batched``, ``tv1w_2d_batched``), float32, and torch CUDA tensors as inputs (device-resident path: no PCIe
 traffic, no host transposes -- a C-ordered tensor is handled by swapping the kernels' stride roles).  The batched 1D functions,
 ``tv1_2d`` ('dr' and 'pd') / ``tv1_2d_batched`` ('dr'), ``tv1w_2d`` / ``tv1w_2d_batched`` ('dr') and the N-D ``tvgen`` / ``tvgen_pdr`` are differentiable on torch
-tensors (exact backward kernels).
+tensors (exact backward kernels); the converged 2D solvers ('condat', 'chambolle-pock') are too with ``backward='converged'``, through
+the Jacobian of the prox at the partition the forward reached.
 """
 import ctypes as C
 import functools
@@ -281,14 +282,14 @@ _CP2_ALGS = {"condat": 0, "chambolle-pock": 1, "chambolle-pock-acc": 2}         
 _TV1_2D_GPU_METHODS = ("dr", "pd") + tuple(_CP2_ALGS)
 
 
-def tv1_2d(x, w, n_threads=1, max_iters=0, method="dr"):
+def tv1_2d(x, w, n_threads=1, max_iters=0, method="dr", backward=None):
     r"""2D anisotropic TV-L1 prox (prox_tv/__init__.py:355-416).
 
     ``method='dr'`` (default) reproduces the reference's DR2_TV iteration exactly (35 fixed iterations unless
     ``max_iters`` > 0 -- NOT a converged solve, see SURVEY.md section 0.3); ``'pd'`` reproduces PD2_TV.  ``'condat'``,
     ``'chambolle-pock'`` and ``'chambolle-pock-acc'`` reproduce CondatChambollePock2_TV bit for bit (float64): primal-dual
-    iterations run until X stops changing or ``max_iters`` (0: 2500) -- the converged prox (DESIGN.md section 15); they have no
-    backward pass.  ``'yang'`` and ``'kolmogorov'`` are not provided.  ``n_threads`` is ignored.
+    iterations run until X stops changing or ``max_iters`` (0: 2500) -- the converged prox (DESIGN.md section 15); by default they
+    have no backward pass (see ``backward``).  ``'yang'`` and ``'kolmogorov'`` are not provided.  ``n_threads`` is ignored.
     numpy input: returns a Fortran-ordered float64 array like the reference.  torch CUDA tensor input (2D, float64 or
     float32): stays on the device and returns a tensor of the same dtype/layout.
 
@@ -298,13 +299,23 @@ def tv1_2d(x, w, n_threads=1, max_iters=0, method="dr"):
     (proxtv_DR2_TV_vjp_dev_*, DESIGN.md section 11), run on the current CUDA stream; double backward is not supported.
     ``method='pd'`` on a tensor is ``tvgen(x, [w, w], [1, 2], [1, 1], max_iters=max_iters)`` on it (PD2_TV, same code, same
     gradients; the gradient of ``w`` is the sum of both terms' penalty gradients, in float64).
+
+    ``backward='converged'`` (``'condat'`` and ``'chambolle-pock'`` only, opt-in): torch tensors become differentiable with respect to
+    ``x`` and ``w`` given as a 0-dim tensor through the Jacobian of the prox itself, not of the iterations computed: the result is
+    constant on clusters of pixels joined by fused edges (DESIGN.md section 15.2), the gradient of ``x`` is the upstream gradient
+    averaged over each cluster and that of ``w`` sums sgn(y_j - y_i) (gx_i - gx_j) over the cut edges.  The forward records a fused-edge
+    tape (2 bits per element) after its last iteration and returns the same bits as an unrecorded solve.  This gradient is right only
+    when the forward has converged (it stopped before ``max_iters``, or at least reached the prox's partition of fused edges); the
+    accelerated ``'chambolle-pock-acc'`` does not reach it and is refused, as are ``'dr'`` and ``'pd'``, which have their own exact
+    backward.  Double backward is not supported; numpy input is unaffected.
     """
     assert w >= 0
     assert method in _TV1_2D_METHODS
     if method not in _TV1_2D_GPU_METHODS:
         raise NotImplementedError("proxtv_b200 implements the 2D solvers %s; got %r" % (", ".join(map(repr, _TV1_2D_GPU_METHODS)), method))
+    _converged_backward(method, backward)
     if method in _CP2_ALGS:
-        return _cp2(x, w, max_iters, method, batched=False)
+        return _cp2(x, w, max_iters, method, batched=False, backward=backward)
     if _is_torch(x):
         if method == "pd":
             assert x.dim() == 2
@@ -330,7 +341,7 @@ def tv1_2d(x, w, n_threads=1, max_iters=0, method="dr"):
     return y
 
 
-def tv1w_2d(x, w_col, w_row, max_iters=0, n_threads=1, method="dr"):
+def tv1w_2d(x, w_col, w_row, max_iters=0, n_threads=1, method="dr", backward=None):
     r"""2D weighted anisotropic TV-L1 prox by Douglas-Rachford splitting (prox_tv/__init__.py:445-481 -> DR2L1W_TV).
 
     ``w_col``: (M-1, N) weights of the differences along columns, ``w_row``: (M, N-1) along rows.  Same fixed-iteration
@@ -342,7 +353,11 @@ def tv1w_2d(x, w_col, w_row, max_iters=0, n_threads=1, method="dr"):
     ``tv1_2d(method=...)`` with each dual clipped to its own edge's weight, run until X stops changing or ``max_iters`` (0: 2500)
     (proxtv_CP2W_TV_*, DESIGN.md section 15.1).  With every weight equal to w it is ``tv1_2d(x, w, method=...)`` bit for bit in
     float64.  torch tensors of either memory order are solved in place of their layout and the result has the solved tensor's
-    layout; these methods have no backward pass.  ``'chambolle-pock-acc'`` is not available: its step rule needs one penalty.
+    layout; by default these methods have no backward pass.  ``'chambolle-pock-acc'`` is not available: its step rule needs one penalty.
+    ``backward='converged'`` (opt-in, these two methods only) makes them differentiable on torch tensors with respect to ``x``,
+    ``w_col`` and ``w_row`` through the Jacobian of the prox at the partition the forward reached, as ``tv1_2d(backward='converged')``
+    describes: each edge weight gets sgn(y_j - y_i) (gx_i - gx_j) on a cut edge and 0 on a fused one.  Right only when the forward has
+    converged; weights of another dtype or device, and expanded weights, get their gradients through ordinary autograd.
 
     torch: differentiable with respect to ``x``, ``w_col`` and ``w_row``.  With grad mode on and one of them requiring grad, the
     forward records a segmentation tape of every prox pass (2 bits per element per pass, kept on the device until the backward) and
@@ -351,8 +366,9 @@ def tv1w_2d(x, w_col, w_row, max_iters=0, n_threads=1, method="dr"):
     device, and expanded weights (``w.expand(M - 1, N)``), get theirs through ordinary autograd.  The forward result is the same
     either way; double backward is not supported.
     """
+    _converged_backward(method, backward)
     if _cp2w_method(method):
-        return _cp2w(x, w_col, w_row, max_iters, method, batched=False)
+        return _cp2w(x, w_col, w_row, max_iters, method, batched=False, backward=backward)
     if _is_torch(x):
         return _drw_torch(x, w_col, w_row, max_iters)
     assert np.all(np.asarray(w_col) >= 0)
@@ -404,7 +420,7 @@ def _drw_solve(Y, W1, W2, geom, tape=None):
     return out
 
 
-def tv1w_2d_batched(x, w_col, w_row, max_iters=0, method="dr"):
+def tv1w_2d_batched(x, w_col, w_row, max_iters=0, method="dr", backward=None):
     r"""``tv1w_2d`` on every image of x (B, H, W), with per-image weight maps ``w_col`` (B, H-1, W) (edges along columns) and
     ``w_row`` (B, H, W-1) (edges along rows).  Each image is solved independently with exactly the single-image iteration (its own
     2 * mean start value, 35 iterations unless ``max_iters`` > 0).
@@ -418,10 +434,11 @@ def tv1w_2d_batched(x, w_col, w_row, max_iters=0, method="dr"):
 
     ``method='condat'`` or ``'chambolle-pock'``: the converged weighted prox of ``tv1w_2d(method=...)`` on every image, each running
     until its own stop test holds (float32: float32 arithmetic).  Results as above (numpy: C-ordered, x's dtype; torch: the solved
-    tensor's layout); no backward pass.
+    tensor's layout); no backward pass unless ``backward='converged'``, the opt-in gradient of ``tv1w_2d``, per image.
     """
+    _converged_backward(method, backward)
     if _cp2w_method(method):
-        return _cp2w(x, w_col, w_row, max_iters, method, batched=True)
+        return _cp2w(x, w_col, w_row, max_iters, method, batched=True, backward=backward)
     if _is_torch(x):
         return _drw_batched_torch(x, w_col, w_row, max_iters)
     x = np.asarray(x)
@@ -509,18 +526,21 @@ def _dr2_solve(xin, w, geom, tape=None):
     return out
 
 
-def tv1_2d_batched(x, w, max_iters=0, method="dr"):
+def tv1_2d_batched(x, w, max_iters=0, method="dr", backward=None):
     """``tv1_2d(method=method)`` on every image of x (B, H, W)  -- BASELINE config 5 with the default ``method='dr'``.
 
     numpy: float64 or float32, C-ordered (B, H, W); torch: CUDA tensor (B, H, W).  Each image is solved independently with
     exactly the single-image iteration (its own 2*mean initialisation).  torch: differentiable like ``tv1_2d``.
     ``method`` 'condat', 'chambolle-pock' or 'chambolle-pock-acc': each image runs until its own stop test holds (float32: float32
-    arithmetic); numpy results are C-ordered arrays of x's dtype, tensors keep their layout; no backward pass.
+    arithmetic); numpy results are C-ordered arrays of x's dtype, tensors keep their layout; no backward pass unless
+    ``backward='converged'`` ('condat' and 'chambolle-pock'), the opt-in gradient of ``tv1_2d``, per image (the gradient of a 0-dim
+    ``w`` sums every image's).
     """
     assert w >= 0
     assert method == "dr" or method in _CP2_ALGS, "method must be 'dr', 'condat', 'chambolle-pock' or 'chambolle-pock-acc'"
+    _converged_backward(method, backward)
     if method in _CP2_ALGS:
-        return _cp2(x, w, max_iters, method, batched=True)
+        return _cp2(x, w, max_iters, method, batched=True, backward=backward)
     if _is_torch(x):
         return _dr2_torch(x, w, max_iters, batched=True)
     x = np.asarray(x)
@@ -538,22 +558,33 @@ def tv1_2d_batched(x, w, max_iters=0, method="dr"):
     return np.transpose(out, (0, 2, 1))
 
 
-def _cp2(x, w, max_iters, method, batched):
+def _converged_backward(method, backward):
+    """Validates the ``backward`` keyword of the 2D solvers: None, or 'converged' with 'condat' / 'chambolle-pock'."""
+    assert backward in (None, "converged"), "backward must be None or 'converged'"
+    if backward == "converged" and method not in _CP2W_ALGS:
+        why = ("does not reach the prox's partition of fused edges in its iterations" if method == "chambolle-pock-acc"
+               else "is a fixed splitting with its own exact backward (omit backward=)")
+        raise NotImplementedError("backward='converged' is the Jacobian of the converged prox, for method 'condat' or 'chambolle-pock'; "
+                                  "method %r %s" % (method, why))
+
+
+def _cp2(x, w, max_iters, method, batched, backward=None):
     """CondatChambollePock2_TV for tv1_2d / tv1_2d_batched.  numpy 2D: the reference's entry point on a Fortran-ordered float64 copy;
     numpy 3D: proxtv_CP2_TV_batched_* on the C-ordered (B, H, W) array; torch: proxtv_CP2_TV_dev_* on either memory order
     (_dr2_layout), result in the solved tensor's layout."""
     alg = _CP2_ALGS[method]
     if _is_torch(x):
-        if _needs_grad(x, w):
-            raise NotImplementedError("tv1_2d method %r has no backward pass; use method='dr' or 'pd' for gradients, or call it "
-                                      "under torch.no_grad() / on a detached tensor" % method)
-        import torch
-        wf = float(w.detach()) if _is_torch(w) else float(w)
+        grad = _needs_grad(x, w)
+        if grad and backward is None:
+            raise NotImplementedError("tv1_2d method %r has no backward pass by default; pass backward='converged' for the Jacobian of "
+                                      "the converged prox, use method='dr' or 'pd' for gradients, or call it under torch.no_grad() / "
+                                      "on a detached tensor" % method)
+        wf, w_t = _w_float(w)
         M, N, batch, row_major, xin = _dr2_layout(x, batched)
-        out = torch.empty_strided(xin.shape, xin.stride(), dtype=xin.dtype, device=xin.device)
-        info = np.zeros(_N_INFO * batch)
-        _dev_call("CP2_TV_dev", xin, M, N, batch, row_major, xin, wf, out, alg, int(max_iters), info, info=info)
-        return out
+        geom = (M, N, batch, row_major, alg, int(max_iters))
+        if grad:
+            return _autograd().CP2.apply(xin, None, None, wf, w_t, geom)
+        return _cp2_solve(xin, None, None, wf, geom)
     w = force_float_scalar(w)
     if not batched:
         x = np.asfortranarray(x, dtype="float64")
@@ -591,24 +622,42 @@ def _cp2w_method(method):
     return method != "dr"
 
 
-def _cp2w(x, w_col, w_row, max_iters, method, batched):
+def _cp2_solve(xin, W1, W2, w, geom, tape=None):
+    """proxtv_CP2_TV_dev_* (W1 None: penalty w) or proxtv_CP2W_TV_dev_* (weight maps W1, W2 laid out like xin) on xin, geom = (M, N,
+    batch, row_major, alg, max_iters); given a tape (a uint8 CUDA tensor, proxtv_CP2_TV_tape_bytes() long) the _record_dev_ form, the
+    same solve followed by its fused-edge tape.  The result has xin's layout."""
+    import torch
+    M, N, batch, row_major, alg, max_iters = geom
+    out = torch.empty_strided(xin.shape, xin.stride(), dtype=xin.dtype, device=xin.device)
+    info = np.zeros(_N_INFO * batch)
+    entry, pen = ("CP2W_TV", (W1, W2)) if W1 is not None else ("CP2_TV", (w,))
+    args = (M, N, batch, row_major, xin, *pen, out, alg, max_iters, info)
+    if tape is None:
+        _dev_call(entry + "_dev", xin, *args, info=info)
+    else:
+        _dev_call(entry + "_record_dev", xin, *args, tape, tape.numel(), info=info)
+    return out
+
+
+def _cp2w(x, w_col, w_row, max_iters, method, batched, backward=None):
     """The weighted primal-dual prox for tv1w_2d / tv1w_2d_batched (proxtv_CP2W_TV_*).  numpy 2D: a Fortran-ordered float64 copy (result
     Fortran-ordered float64); numpy 3D: the C-ordered (B, H, W) array in x's dtype; torch: either memory order (_dr2_layout), the weight
     maps laid out to match, result in the solved tensor's layout."""
     alg = _CP2W_ALGS[method]
     if _is_torch(x):
-        if _needs_grad(x, w_col, w_row):
-            raise NotImplementedError("tv1w_2d method %r has no backward pass; use method='dr' for gradients, or call it under "
-                                      "torch.no_grad() / on detached tensors" % method)
-        import torch
+        grad = _needs_grad(x, w_col, w_row)
+        if grad and backward is None:
+            raise NotImplementedError("tv1w_2d method %r has no backward pass by default; pass backward='converged' for the Jacobian of "
+                                      "the converged prox, use method='dr' for gradients, or call it under torch.no_grad() / on "
+                                      "detached tensors" % method)
         M, N, batch, row_major, xin = _dr2_layout(x, batched)
         lead = (batch,) if batched else ()
         assert tuple(w_col.shape) == lead + (M - 1, N) and tuple(w_row.shape) == lead + (M, N - 1)
         w1, w2 = _drw_lay(w_col, xin, row_major), _drw_lay(w_row, xin, row_major)
-        out = torch.empty_strided(xin.shape, xin.stride(), dtype=xin.dtype, device=xin.device)
-        info = np.zeros(_N_INFO * batch)
-        _dev_call("CP2W_TV_dev", xin, M, N, batch, row_major, xin, w1, w2, out, alg, int(max_iters), info, info=info)
-        return out
+        geom = (M, N, batch, row_major, alg, int(max_iters))
+        if grad:
+            return _autograd().CP2.apply(xin, w1, w2, 0.0, None, geom)
+        return _cp2_solve(xin, w1, w2, 0.0, geom)
     x = np.asarray(x)
     assert x.ndim == (3 if batched else 2)
     assert np.all(np.asarray(w_col) >= 0)
@@ -1037,4 +1086,42 @@ def _autograd():
             g_ws = _penalty_grad(glam if solver == "PD2_TV" else glam * float(npen), ctx.ws_like) if need_ws else None
             return (gY if need_x else None), g_ws, *rest
 
-    return types.SimpleNamespace(ProxRows=ProxRows, DRW=DRW, DR2=DR2, ND=ND)
+    class CP2(torch.autograd.Function):
+        """apply(xin, W1, W2, w, w_t, geom) of _cp2_solve (W1 None: the penalty w, read from w_t when that is a tensor).  backward:
+        proxtv_CP2_TV_vjp_dev_* / proxtv_CP2W_TV_vjp_dev_*, the Jacobian of the converged prox at the recorded partition -- gx = the
+        cluster means of the upstream gradient, per-edge weight gradients (NULL for a map that needs none), glam per image and axis."""
+        @staticmethod
+        def forward(ctx, xin, W1, W2, w, w_t, geom):
+            M, N, batch = geom[:3]
+            tape = torch.empty(int(require_device().proxtv_CP2_TV_tape_bytes(M, N, batch)), dtype=torch.uint8, device=xin.device)
+            out = _cp2_solve(xin, W1, W2, w, geom, tape)
+            ctx.save_for_backward(tape, out)
+            ctx.geom = geom
+            ctx.layouts = [(t.shape, t.stride(), t.dtype) if t is not None else None for t in (out, W1, W2)]
+            ctx.w_like = (w_t.dtype, w_t.device, ()) if w_t is not None else None
+            return out
+
+        @staticmethod
+        @once_differentiable
+        def backward(ctx, gout):
+            tape, out = ctx.saved_tensors
+            M, N, batch, row_major = ctx.geom[:4]
+            need_x, need_w1, need_w2, _, need_w_t, _ = ctx.needs_input_grad
+
+            def like(i):
+                shape, stride, dt = ctx.layouts[i]
+                return torch.empty_strided(shape, stride, dtype=dt, device=tape.device)
+            g = like(0)                                   # the upstream gradient in the output's layout
+            g.copy_(gout)
+            gY = like(0)
+            if ctx.layouts[1] is not None:
+                gW1 = like(1) if need_w1 else None
+                gW2 = like(2) if need_w2 else None
+                _dev_call("CP2W_TV_vjp_dev", g, M, N, batch, row_major, tape, out, g, gY, gW1, gW2, None)
+                return (gY if need_x else None), gW1, gW2, None, None, None
+            glam = torch.empty(2 * batch, dtype=torch.float64, device=tape.device) if need_w_t else None
+            _dev_call("CP2_TV_vjp_dev", g, M, N, batch, row_major, tape, out, g, gY, glam)
+            g_w = _penalty_grad(glam, ctx.w_like) if need_w_t else None
+            return (gY if need_x else None), None, None, None, g_w, None
+
+    return types.SimpleNamespace(ProxRows=ProxRows, DRW=DRW, DR2=DR2, ND=ND, CP2=CP2)

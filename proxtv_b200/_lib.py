@@ -63,6 +63,19 @@ SIGNATURES = {
     "proxtv_CP2W_TV_dev_f32": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, C.c_int, _vp, _vp, _vp, _vp, C.c_int, C.c_int, _vp, _vp]),
     "proxtv_CP2W_TV_batched_f64": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, C.c_int, _vp, _vp, _vp, _vp, C.c_int, C.c_int, _vp]),
     "proxtv_CP2W_TV_batched_f32": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, C.c_int, _vp, _vp, _vp, _vp, C.c_int, C.c_int, _vp]),
+    "proxtv_CP2_TV_tape_bytes": (C.c_size_t, [C.c_size_t, C.c_size_t, C.c_int]),
+    "proxtv_CP2_TV_record_dev_f64": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, C.c_int, _vp, C.c_double, _vp, C.c_int, C.c_int, _vp, _vp,
+                                               C.c_size_t, _vp]),
+    "proxtv_CP2_TV_record_dev_f32": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, C.c_int, _vp, C.c_double, _vp, C.c_int, C.c_int, _vp, _vp,
+                                               C.c_size_t, _vp]),
+    "proxtv_CP2W_TV_record_dev_f64": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, C.c_int, _vp, _vp, _vp, _vp, C.c_int, C.c_int, _vp, _vp,
+                                                C.c_size_t, _vp]),
+    "proxtv_CP2W_TV_record_dev_f32": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, C.c_int, _vp, _vp, _vp, _vp, C.c_int, C.c_int, _vp, _vp,
+                                                C.c_size_t, _vp]),
+    "proxtv_CP2_TV_vjp_dev_f64": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "proxtv_CP2_TV_vjp_dev_f32": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "proxtv_CP2W_TV_vjp_dev_f64": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "proxtv_CP2W_TV_vjp_dev_f32": (C.c_int, [C.c_size_t, C.c_size_t, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "proxtv_DR2L1W_TV_dev_f64": (C.c_int, [C.c_size_t, C.c_size_t, _vp, _vp, _vp, _vp, C.c_int, _vp, _vp]),
     "proxtv_DR2L1W_TV_dev_f32": (C.c_int, [C.c_size_t, C.c_size_t, _vp, _vp, _vp, _vp, C.c_int, _vp, _vp]),
     "proxtv_DR2L1W_TV_tape_bytes": (C.c_size_t, [C.c_size_t, C.c_size_t, C.c_int]),

@@ -6,6 +6,7 @@
 // return 0 (src/TV2Dopt.cpp:78-82,368-372).
 #include "../../include/proxtv_b200.h"
 #include "ptv_internal.h"
+#include <limits.h>
 #include <mutex>
 #include <stdio.h>
 #include <string.h>
@@ -206,7 +207,7 @@ int run_drw(const char* fn, bool host_io, size_t M, size_t N, int batch, int row
 // like run_drw's instead of lambda, alg 0 or 1.
 template <typename T>
 int run_cp2(const char* fn, bool host_io, size_t M, size_t N, int batch, int row_major, const T* Y, double lambda, bool weighted,
-            const T* W1, const T* W2, T* X, int alg, int maxit, double* info, cudaStream_t st) {
+            const T* W1, const T* W2, T* X, int alg, int maxit, double* info, cudaStream_t st, void* tape = nullptr) {
     const Refuse no{fn, info, batch > 1 ? batch : 1};
     if (weighted && alg == 2) return no("the weighted solver has no accelerated variant (alg 2); use alg 0 or 1");
     if (alg != 0 && alg != 1 && alg != 2) return no("Algorithm parameter has an invalid value");
@@ -227,11 +228,42 @@ int run_cp2(const char* fn, bool host_io, size_t M, size_t N, int batch, int row
         if (!io.stage()) return 0;
     }
     std::vector<int> iters(info ? batch : 0);
-    if (!no.cuda_ok(cp2_device<T>(M, N, batch, row_major, Y, lambda, weighted, W1, W2, X, alg, maxit, info ? iters.data() : nullptr, ws, st)))
+    if (!no.cuda_ok(cp2_device<T>(M, N, batch, row_major, Y, lambda, weighted, W1, W2, X, alg, maxit, info ? iters.data() : nullptr, ws, st,
+                                  tape)))
         return 0;
     if (!io.finish()) return 0;
     if (info) for (int b = 0; b < batch; b++) { info[3 * (size_t)b + INFO_ITERS] = iters[b]; info[3 * (size_t)b + INFO_RC] = RC_OK; }
     return 1;
+}
+
+// The recorded converged solve: run_cp2's device call, then the fused-edge tape (DESIGN.md section 15.2).  Its own refusals come first.
+template <typename T>
+static int dev_cp2_record(const char* fn, size_t M, size_t N, int batch, int row_major, const T* Y, double lambda, bool weighted, const T* W1,
+                          const T* W2, T* X, int alg, int maxit, double* info, void* tape, size_t tape_bytes, void* stream) {
+    const Refuse no{fn, info, batch > 1 ? batch : 1};
+    if (alg == 2) return no("the accelerated solver (alg 2) has no converged backward: it does not reach the prox's partition; record with alg 0 or 1");
+    if (alg != 0 && alg != 1) return no("Algorithm parameter has an invalid value");
+    if (M < 1 || N < 1 || batch < 1 || M > (size_t)INT_MAX || N > (size_t)INT_MAX || M * N > (size_t)INT_MAX)
+        return no("invalid shape (need M, N, batch >= 1 and M N < 2^31)");
+    if (!Y || !X || !tape || (weighted && ((M > 1 && !W1) || (N > 1 && !W2)))) return no("NULL array");
+    if (!weighted && !(lambda >= 0)) return no("negative penalty");
+    if (tape_bytes < cp2_tape_bytes(M, N, batch)) return no("tape_bytes smaller than proxtv_CP2_TV_tape_bytes()");
+    return run_cp2<T>(fn, false, M, N, batch, row_major, Y, lambda, weighted, W1, W2, X, alg, maxit, info, (cudaStream_t)stream, tape);
+}
+
+template <typename T>
+static int dev_cp2_vjp(const char* fn, bool weighted, size_t M, size_t N, int batch, int row_major, const void* tape, const T* X, const T* gout,
+                       T* gY, T* gW1, T* gW2, double* glam, void* stream) {
+    const Refuse no{fn};
+    if (M < 1 || N < 1 || batch < 1 || M > (size_t)INT_MAX || N > (size_t)INT_MAX || M * N > (size_t)INT_MAX)
+        return no("invalid shape (need M, N, batch >= 1 and M N < 2^31)");
+    if (!tape || !X || !gout || !gY) return no("NULL array");
+    if (!no.have_device()) return 0;
+    WsGuard guard((cudaStream_t)stream);
+    if (const char* why = cp2_tape_check(tape, sizeof(T), M, N, batch, row_major, weighted, (cudaStream_t)stream)) return no(why);
+    void* ws = ws_get(ws_bytes_cp2_vjp(M, N, batch));
+    if (!ws) return no("out of memory");
+    return no.cuda_ok(cp2_vjp_device<T>(M, N, batch, row_major, tape, X, gout, gY, gW1, gW2, glam, ws, (cudaStream_t)stream));
 }
 
 // PD_TV and PDR_TV multiply the caller's penalties by the number of terms, in place (TVNDopt.cpp:100-101, :339-340); PD2_TV takes
@@ -735,6 +767,36 @@ int proxtv_CP2W_TV_batched_f64(size_t M, size_t N, int batch, int row_major, con
 int proxtv_CP2W_TV_batched_f32(size_t M, size_t N, int batch, int row_major, const float* Y, const float* W1, const float* W2, float* X,
                                int alg, int maxit, double* info) {
     return run_cp2<float>("proxtv_CP2W_TV_batched_f32", true, M, N, batch, row_major, Y, 0., true, W1, W2, X, alg, maxit, info, 0); }
+
+size_t proxtv_CP2_TV_tape_bytes(size_t M, size_t N, int batch) { return batch < 1 ? 0 : cp2_tape_bytes(M, N, batch); }
+int proxtv_CP2_TV_record_dev_f64(size_t M, size_t N, int batch, int row_major, const double* Y, double lambda, double* X, int alg, int maxit,
+                                 double* info, void* tape, size_t tape_bytes, void* stream) {
+    return dev_cp2_record<double>("proxtv_CP2_TV_record_dev_f64", M, N, batch, row_major, Y, lambda, false, nullptr, nullptr, X, alg, maxit, info,
+                                  tape, tape_bytes, stream); }
+int proxtv_CP2_TV_record_dev_f32(size_t M, size_t N, int batch, int row_major, const float* Y, double lambda, float* X, int alg, int maxit,
+                                 double* info, void* tape, size_t tape_bytes, void* stream) {
+    return dev_cp2_record<float>("proxtv_CP2_TV_record_dev_f32", M, N, batch, row_major, Y, lambda, false, nullptr, nullptr, X, alg, maxit, info,
+                                 tape, tape_bytes, stream); }
+int proxtv_CP2W_TV_record_dev_f64(size_t M, size_t N, int batch, int row_major, const double* Y, const double* W1, const double* W2, double* X,
+                                  int alg, int maxit, double* info, void* tape, size_t tape_bytes, void* stream) {
+    return dev_cp2_record<double>("proxtv_CP2W_TV_record_dev_f64", M, N, batch, row_major, Y, 0., true, W1, W2, X, alg, maxit, info, tape,
+                                  tape_bytes, stream); }
+int proxtv_CP2W_TV_record_dev_f32(size_t M, size_t N, int batch, int row_major, const float* Y, const float* W1, const float* W2, float* X,
+                                  int alg, int maxit, double* info, void* tape, size_t tape_bytes, void* stream) {
+    return dev_cp2_record<float>("proxtv_CP2W_TV_record_dev_f32", M, N, batch, row_major, Y, 0., true, W1, W2, X, alg, maxit, info, tape,
+                                 tape_bytes, stream); }
+int proxtv_CP2_TV_vjp_dev_f64(size_t M, size_t N, int batch, int row_major, const void* tape, const double* X, const double* gout, double* gY,
+                              double* glam, void* stream) {
+    return dev_cp2_vjp<double>("proxtv_CP2_TV_vjp_dev_f64", false, M, N, batch, row_major, tape, X, gout, gY, nullptr, nullptr, glam, stream); }
+int proxtv_CP2_TV_vjp_dev_f32(size_t M, size_t N, int batch, int row_major, const void* tape, const float* X, const float* gout, float* gY,
+                              double* glam, void* stream) {
+    return dev_cp2_vjp<float>("proxtv_CP2_TV_vjp_dev_f32", false, M, N, batch, row_major, tape, X, gout, gY, nullptr, nullptr, glam, stream); }
+int proxtv_CP2W_TV_vjp_dev_f64(size_t M, size_t N, int batch, int row_major, const void* tape, const double* X, const double* gout, double* gY,
+                               double* gW1, double* gW2, double* glam, void* stream) {
+    return dev_cp2_vjp<double>("proxtv_CP2W_TV_vjp_dev_f64", true, M, N, batch, row_major, tape, X, gout, gY, gW1, gW2, glam, stream); }
+int proxtv_CP2W_TV_vjp_dev_f32(size_t M, size_t N, int batch, int row_major, const void* tape, const float* X, const float* gout, float* gY,
+                               float* gW1, float* gW2, double* glam, void* stream) {
+    return dev_cp2_vjp<float>("proxtv_CP2W_TV_vjp_dev_f32", true, M, N, batch, row_major, tape, X, gout, gY, gW1, gW2, glam, stream); }
 
 int proxtv_DR2L1W_TV_dev_f64(size_t M, size_t N, const double* Y, const double* W1, const double* W2, double* out, int maxit, double* info, void* stream) {
     return run_drw<double>("proxtv_DR2L1W_TV_dev_f64", false, M, N, 1, 0, Y, W1, W2, out, maxit, info, (cudaStream_t)stream); }

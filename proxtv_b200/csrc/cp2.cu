@@ -18,6 +18,9 @@
 // maps are read in place: in F x S terms they are an (F-1) x S map Wf of the edges along F and an F x (S-1) map Ws of the edges
 // along S, both F-contiguous (column-major: Wf = W1, Ws = W2; C order: Wf = W2, Ws = W1), so the weight of the dual at q = b F S +
 // f + F s is Wf[q - (b S + s)] and Ws[q - b F].
+//
+// Recorded (DESIGN.md section 15.2): given a tape, one more launch after k_cp2_out writes the fused-edge tape of the backward
+// (cp2_vjp.cu) from the final duals; every launch before it is the same.
 #include "ptv_internal.h"
 #include <math.h>
 #include <stdio.h>
@@ -176,7 +179,7 @@ size_t ws_bytes_cp2(size_t M, size_t N, int batch, size_t elem) {
 
 template <typename T>
 cudaError_t cp2_device(size_t M, size_t N, int batch, int row_major, const T* Y, double lambda, bool weighted, const T* W1, const T* W2,
-                       T* out, int alg, int maxit, int* iters, void* ws, cudaStream_t st) {
+                       T* out, int alg, int maxit, int* iters, void* ws, cudaStream_t st, void* tape) {
     Geom g;
     g.F = (int)(row_major ? N : M); g.S = (int)(row_major ? M : N);
     g.img = (long long)M * (long long)N; g.batch = batch;
@@ -238,6 +241,7 @@ cudaError_t cp2_device(size_t M, size_t N, int batch, int row_major, const T* Y,
         }
         k_cp2_out<T><<<grid_1d(n), 256, 0, st>>>(g, Xb[0], Xb[1], stopped, it, out);
         CP2_TRY(cudaGetLastError());
+        if (tape) CP2_TRY(cp2_tape_tail<T>(M, N, batch, row_major, out, Ufb, Usb, stopped, it, lambda, weighted, Wf, Ws, tape, st));
         if (iters) {
             CP2_TRY(cudaMemcpyAsync(iters, stopped, (size_t)batch * sizeof(int), cudaMemcpyDeviceToHost, st));
             CP2_TRY(cudaStreamSynchronize(st));
@@ -251,8 +255,8 @@ done:
 }
 
 template cudaError_t cp2_device<double>(size_t, size_t, int, int, const double*, double, bool, const double*, const double*, double*, int,
-                                        int, int*, void*, cudaStream_t);
+                                        int, int*, void*, cudaStream_t, void*);
 template cudaError_t cp2_device<float>(size_t, size_t, int, int, const float*, double, bool, const float*, const float*, float*, int, int,
-                                       int*, void*, cudaStream_t);
+                                       int*, void*, cudaStream_t, void*);
 
 }  // namespace ptv

@@ -247,10 +247,26 @@ size_t ws_bytes_cp2(size_t M, size_t N, int batch, size_t elem);
 // 2500.  iters: nullptr, or host memory for each image's final `it` (iterations run + 1; the call then synchronises the stream).
 // Reads the running-image count back every 64 iterations (one stream synchronisation each).  weighted (section 15.1; alg 0 or 1,
 // lambda unused): each dual is clipped to its edge's weight in W1 ((M-1) x N per image) / W2 (M x (N-1)), device maps laid out like
-// proxtv_DR2L1W_TV_batched_*'s; W1 may be nullptr when M == 1, W2 when N == 1.  The workspace is the same either way.
+// proxtv_DR2L1W_TV_batched_*'s; W1 may be nullptr when M == 1, W2 when N == 1.  The workspace is the same either way.  tape: nullptr, or
+// a buffer of cp2_tape_bytes() bytes (alg 0 or 1, M N < 2^31; checked by the caller) that cp2_tape_tail fills after the solve.
 template <typename T>
 cudaError_t cp2_device(size_t M, size_t N, int batch, int row_major, const T* Y, double lambda, bool weighted, const T* W1, const T* W2,
-                       T* out, int alg, int maxit, int* iters, void* ws, cudaStream_t st);
+                       T* out, int alg, int maxit, int* iters, void* ws, cudaStream_t st, void* tape = nullptr);
+// ---- backward pass of the converged solve (cp2_vjp.cu, DESIGN.md section 15.2) ----
+size_t cp2_tape_bytes(size_t M, size_t N, int batch);                   // 256-byte header + two bitsets (fused along F, along S)
+size_t ws_bytes_cp2_vjp(size_t M, size_t N, int batch);
+// The fused-edge tape of a finished solve: X its result, Uf / Us the two buffers of each dual, image b's final ones those of iteration
+// (stopped[b] ? stopped[b] : it_end) - 1; Wf / Ws the weight maps in storage terms (weighted), else lambda.
+template <typename T>
+cudaError_t cp2_tape_tail(size_t M, size_t N, int batch, int row_major, const T* X, const T* const Uf[2], const T* const Us[2], const int* stopped,
+                          int it_end, double lambda, bool weighted, const T* Wf, const T* Ws, void* tape, cudaStream_t st);
+// Validates a tape's header against the arguments (one stream synchronisation): nullptr ok, else the reason.
+const char* cp2_tape_check(const void* tape, size_t elem, size_t M, size_t N, int batch, int row_major, bool weighted, cudaStream_t st);
+// gY (laid out like X), per-edge gW1 / gW2 (like W1 / W2) unless nullptr, glam[2 batch] unless nullptr, from the tape, the forward's
+// result X and the upstream gradient gout; workspace ws_bytes_cp2_vjp().  Arguments checked by the caller.
+template <typename T>
+cudaError_t cp2_vjp_device(size_t M, size_t N, int batch, int row_major, const void* tape, const T* X, const T* gout, T* gY, T* gW1, T* gW2,
+                           double* glam, void* ws, cudaStream_t st);
 
 }  // namespace ptv
 
