@@ -12,6 +12,12 @@ traffic, no host transposes -- a C-ordered tensor is handled by swapping the ker
 ``tv1_2d`` ('dr' and 'pd') / ``tv1_2d_batched`` ('dr'), ``tv1w_2d`` / ``tv1w_2d_batched`` ('dr') and the N-D ``tvgen`` / ``tvgen_pdr`` are differentiable on torch
 tensors (exact backward kernels); the converged 2D solvers ('condat', 'chambolle-pock') are too with ``backward='converged'``, through
 the Jacobian of the prox at the partition the forward reached.
+
+Every call into the library goes through ``_host_call`` (numpy: host arrays) or ``_dev_call`` (torch: device pointers on the tensor's
+current stream), which share one failure rule (``_check``).  Each 2D family has one numpy body (``_tv2_numpy``, ``_tv2w_numpy``) on the
+``proxtv_*_batched_*`` host symbols, a single image being a column-major batch of one; the taped 2D solvers share one autograd Function
+(``TV2``) and one table of what differs between them (``_TAPED``); the N-D solvers share one front (``_tvgen_front``), one tensor layout
+(``_nd_layout``) and one Function (``ND``).
 """
 import ctypes as C
 import functools
@@ -60,23 +66,33 @@ def _is_torch(x):
     return type(x).__module__.startswith("torch") and hasattr(x, "data_ptr")
 
 
-def _check(ok, what):
-    if not ok:
-        raise ProxTVError("%s failed: %s" % (what, _lib.last_error()))
+def _check(ok, name, rc=True, info=None):
+    """The one failure rule of the entry points: a zero return where the entry returns 1 on success (rc), or RC = 3 in any row of the
+    info array the call filled.  Raises ProxTVError naming the C symbol."""
+    if (rc and not ok) or (info is not None and np.any(info[2::_N_INFO] == 3)):
+        raise ProxTVError("%s failed: %s" % (name, _lib.last_error()))
+
+
+def _host_call(entry, ref, *args, rc=True, info=None):
+    """Call proxtv_<entry>_f32 / _f64 (by the numpy array ref's dtype), or with ref None the symbol named entry as it is; ndarrays in
+    args go as host pointers, None as NULL.  Raises ProxTVError naming the symbol when the call fails (_check)."""
+    name = entry if ref is None else "proxtv_%s_%s" % (entry, "f32" if ref.dtype == np.float32 else "f64")
+    fn = getattr(require_device(), name)
+    _check(fn(*[_ptr(a) if isinstance(a, np.ndarray) else a for a in args]), name, rc, info)
 
 
 # ---- torch CUDA tensors: device calls and autograd ----
 def _dev_call(entry, ref, *args, rc=True, info=None):
     """Call proxtv_<entry>_f32 / _f64 (by ref's dtype) on ref's device, with ref's current CUDA stream appended to args; torch
     tensors in args go as device pointers, numpy arrays as host pointers, None as NULL.  Raises ProxTVError naming the entry point
-    when the call fails: on a zero return (unless not rc) or, given the info array the call fills, on info[2] == 3."""
+    when the call fails (_check)."""
     import torch
     name = "proxtv_%s_%s" % (entry, "f32" if ref.dtype == torch.float32 else "f64")
     fn = getattr(require_device(), name)
     args = [C.c_void_p(a.data_ptr()) if isinstance(a, torch.Tensor) else _ptr(a) if isinstance(a, np.ndarray) else a for a in args]
     with torch.cuda.device(ref.device):
         ok = fn(*args, C.c_void_p(torch.cuda.current_stream(ref.device).cuda_stream))
-    _check((ok or not rc) and (info is None or info[2] != 3), name)
+    _check(ok, name, rc, info)
 
 
 def _needs_grad(*objs):
@@ -182,9 +198,8 @@ def tv1_1d(x, w, method="hybridtautstring", sigma=0.05, maxbacktracks=None):
     x = force_float_matrix(x)
     y = np.zeros(np.size(x))
     if x.size:
-        lib = require_device()
         xin = x if x.flags.c_contiguous or x.flags.f_contiguous else np.ascontiguousarray(x)
-        _check(lib.proxtv_prox_fibers_f64(_ptr(xin), _ptr(y), 1, int(np.size(x)), 1, w, None), "tv1_1d")
+        _host_call("prox_fibers", y, xin, y, 1, int(np.size(x)), 1, w, None)
     return y
 
 
@@ -203,9 +218,7 @@ def tv1w_1d(x, w, method="tautstring", sigma=0.05):
     if n == 1:
         y[0] = x.ravel()[0]
     elif n > 1:
-        lib = require_device()
-        _check(lib.proxtv_prox_fibers_f64(_ptr(np.ascontiguousarray(x)), _ptr(y), 1, n, 1, 0.0,
-                                          _ptr(np.ascontiguousarray(w))), "tv1w_1d")
+        _host_call("prox_fibers", y, np.ascontiguousarray(x), y, 1, n, 1, 0.0, np.ascontiguousarray(w))
     return y
 
 
@@ -247,9 +260,7 @@ def _batched_1d(x, w, weights):
         assert wv.shape == (B, L - 1)
         assert np.all(wv >= 0)
     if x.size:
-        lib = require_device()
-        fn = lib.proxtv_prox_fibers_f32 if f32 else lib.proxtv_prox_fibers_f64
-        _check(fn(_ptr(x), _ptr(out), B, L, 1, float(w), _ptr(wv) if wv is not None else None), "batched 1D prox")
+        _host_call("prox_fibers", x, x, out, B, L, 1, float(w), wv)
     return out
 
 
@@ -279,6 +290,7 @@ def tv1w_1d_batched(x, w):
 # ======================================================================================================================
 _TV1_2D_METHODS = ("yang", "dr", "pd", "kolmogorov", "condat", "chambolle-pock", "chambolle-pock-acc")  # :391-399
 _CP2_ALGS = {"condat": 0, "chambolle-pock": 1, "chambolle-pock-acc": 2}                          # the `alg` of CondatChambollePock2_TV
+_CP2W_ALGS = {"condat": 0, "chambolle-pock": 1}          # the weighted solver's `alg` (proxtv_CP2W_TV_*)
 _TV1_2D_GPU_METHODS = ("dr", "pd") + tuple(_CP2_ALGS)
 
 
@@ -314,31 +326,21 @@ def tv1_2d(x, w, n_threads=1, max_iters=0, method="dr", backward=None):
     if method not in _TV1_2D_GPU_METHODS:
         raise NotImplementedError("proxtv_b200 implements the 2D solvers %s; got %r" % (", ".join(map(repr, _TV1_2D_GPU_METHODS)), method))
     _converged_backward(method, backward)
-    if method in _CP2_ALGS:
-        return _cp2(x, w, max_iters, method, batched=False, backward=backward)
-    if _is_torch(x):
-        if method == "pd":
+    if method == "pd":
+        if _is_torch(x):
             assert x.dim() == 2
             assert not _is_torch(w) or w.dim() == 0, "w must be a number or a 0-dim tensor"
             wf, w_t = _w_float(w)
-            return _nd_torch("PD2_TV", x, [wf, wf], w_t, [1, 2], max_iters)
-        return _dr2_torch(x, w, max_iters, batched=False)
-    x = np.asfortranarray(x, dtype="float64")
-    assert x.ndim == 2
-    w = force_float_scalar(w)
-    lib = require_device()
-    y = _pool.empty(x.shape, np.float64, "F")
-    info = np.zeros(_N_INFO)
-    if method == "dr":
-        lib.DR2_TV(x.shape[0], x.shape[1], _ptr(x), w, w, 1.0, 1.0, _ptr(y), int(n_threads), int(max_iters), _ptr(info))
-        _check(info[2] != 3, "DR2_TV")
-    else:
-        lam = np.array([w, w]); norms = np.array([1.0, 1.0]); dims = np.array([1.0, 2.0])
-        ns = np.array(x.shape, dtype=np.int32)
-        ok = lib.PD2_TV(_ptr(x), _ptr(lam), _ptr(norms), _ptr(dims), _ptr(y), _ptr(info), _ptr(ns), 2, 2,
-                        int(n_threads), int(max_iters))
-        _check(ok and info[2] != 3, "PD2_TV")
-    return y
+            return _nd_torch("PD2_TV", tvgen, x, [wf, wf], w_t, [1, 2], max_iters)
+        x = np.asfortranarray(x, dtype="float64")
+        assert x.ndim == 2
+        w = force_float_scalar(w)
+        y = _pool.empty(x.shape, np.float64, "F")
+        info = np.zeros(_N_INFO)
+        _host_call("PD2_TV", None, x, np.array([w, w]), np.array([1.0, 1.0]), np.array([1.0, 2.0]), y, info,
+                   np.array(x.shape, dtype=np.int32), 2, 2, int(n_threads), int(max_iters), info=info)
+        return y
+    return _tv2(x, w, max_iters, method, batched=False, backward=backward)
 
 
 def tv1w_2d(x, w_col, w_row, max_iters=0, n_threads=1, method="dr", backward=None):
@@ -367,29 +369,23 @@ def tv1w_2d(x, w_col, w_row, max_iters=0, n_threads=1, method="dr", backward=Non
     either way; double backward is not supported.
     """
     _converged_backward(method, backward)
-    if _cp2w_method(method):
-        return _cp2w(x, w_col, w_row, max_iters, method, batched=False, backward=backward)
+    _w2_method(method)
+    if method != "dr":
+        return _tv2w(x, w_col, w_row, max_iters, method, batched=False, backward=backward)
     if _is_torch(x):
         return _drw_torch(x, w_col, w_row, max_iters)
-    assert np.all(np.asarray(w_col) >= 0)
+    assert np.all(np.asarray(w_col) >= 0)             # the reference's checks in its order: an x that is not 2D raises ValueError
     assert np.all(np.asarray(w_row) >= 0)
     M, N = np.shape(x)
     assert np.shape(w_col) == (M - 1, N)
     assert np.shape(w_row) == (M, N - 1)
-    x = np.asfortranarray(x, dtype="float64")
-    y = _pool.empty(x.shape, np.float64, "F")
-    w_col = np.asfortranarray(w_col, dtype="float64")
-    w_row = np.asfortranarray(w_row, dtype="float64")
-    info = np.zeros(_N_INFO)
-    lib = require_device()
-    lib.DR2L1W_TV(M, N, _ptr(x), _ptr(w_col), _ptr(w_row), _ptr(y), int(n_threads), int(max_iters), _ptr(info))
-    _check(info[2] != 3, "DR2L1W_TV")
-    return y
+    return _tv2w_numpy(x, w_col, w_row, max_iters, None, batched=False)
 
 
 def _drw_torch(x, w_col, w_row, max_iters):
-    """The torch path of tv1w_2d; recorded by the Function when grad mode is on and x, w_col or w_row requires grad.  The solver works
-    on column-major arrays, the row-major storage of the transposes: the transposes and casts to them are ordinary autograd ops."""
+    """The torch path of tv1w_2d(method='dr'); recorded by the Function when grad mode is on and x, w_col or w_row requires grad.  The
+    solver works on column-major arrays, the row-major storage of the transposes: the transposes and casts to them are ordinary autograd
+    ops."""
     import torch
     assert x.is_cuda and x.dtype in (torch.float64, torch.float32) and x.dim() == 2
     M, N = int(x.shape[0]), int(x.shape[1])
@@ -397,27 +393,10 @@ def _drw_torch(x, w_col, w_row, max_iters):
     xt = x.t().contiguous()
     w1 = w_col.to(device=x.device, dtype=x.dtype).t().contiguous()
     w2 = w_row.to(device=x.device, dtype=x.dtype).t().contiguous()
-    geom = (M, N, 1, 0, int(max_iters))
+    geom = (M, N, 1, 0, None, int(max_iters))
     if _needs_grad(x, w_col, w_row):
-        return _autograd().DRW.apply(xt, w1, w2, geom).t()
-    return _drw_solve(xt, w1, w2, geom).t()
-
-
-def _drw_solve(Y, W1, W2, geom, tape=None):
-    """DR2L1W_TV on the solver's buffers, geom = (M, N, batch, row_major, max_iters): Y and the weight maps W1, W2 laid out as
-    proxtv_DR2L1W_TV_batched_dev_* takes them (their memory, whatever the tensors' shapes): proxtv_DR2L1W_TV_batched_dev_*, or given a
-    tape (a uint8 CUDA tensor, proxtv_DR2L1W_TV_batched_tape_bytes() long) proxtv_DR2L1W_TV_batched_record_dev_*, the same solve
-    recording every prox pass's segmentation.  The result has Y's layout."""
-    import torch
-    out = torch.empty_strided(Y.shape, Y.stride(), dtype=Y.dtype, device=Y.device)
-    info = np.zeros(_N_INFO)
-    M, N, batch, row_major, max_iters = geom
-    args = (M, N, batch, row_major, Y, W1, W2, out, max_iters)
-    if tape is None:       # returns 0 on success, like the reference's DR2L1W_TV: only info[2] == 3 signals a failure
-        _dev_call("DR2L1W_TV_batched_dev", Y, *args, info, rc=False, info=info)
-    else:
-        _dev_call("DR2L1W_TV_batched_record_dev", Y, *args, tape, tape.numel(), info)
-    return out
+        return _autograd().TV2.apply(xt, w1, w2, 0.0, None, "DR2L1W_TV_batched", geom).t()
+    return _tv2_solve("DR2L1W_TV_batched", xt, w1, w2, 0.0, geom).t()
 
 
 def tv1w_2d_batched(x, w_col, w_row, max_iters=0, method="dr", backward=None):
@@ -437,41 +416,8 @@ def tv1w_2d_batched(x, w_col, w_row, max_iters=0, method="dr", backward=None):
     tensor's layout); no backward pass unless ``backward='converged'``, the opt-in gradient of ``tv1w_2d``, per image.
     """
     _converged_backward(method, backward)
-    if _cp2w_method(method):
-        return _cp2w(x, w_col, w_row, max_iters, method, batched=True, backward=backward)
-    if _is_torch(x):
-        return _drw_batched_torch(x, w_col, w_row, max_iters)
-    x = np.asarray(x)
-    assert x.ndim == 3
-    B, H, W = x.shape
-    assert np.shape(w_col) == (B, H - 1, W)
-    assert np.shape(w_row) == (B, H, W - 1)
-    assert np.all(np.asarray(w_col) >= 0)
-    assert np.all(np.asarray(w_row) >= 0)
-    dt = np.float32 if x.dtype == np.float32 else np.float64
-    x = np.ascontiguousarray(x, dtype=dt)
-    w1 = np.ascontiguousarray(w_col, dtype=dt)
-    w2 = np.ascontiguousarray(w_row, dtype=dt)
-    out = _pool.empty(x.shape, dt, "C")
-    if x.size:
-        info = np.zeros(_N_INFO)
-        lib = require_device()
-        fn = lib.proxtv_DR2L1W_TV_batched_f32 if dt == np.float32 else lib.proxtv_DR2L1W_TV_batched_f64
-        fn(H, W, B, 1, _ptr(x), _ptr(w1), _ptr(w2), _ptr(out), int(max_iters), _ptr(info))
-        _check(info[2] != 3, "DR2L1W_TV (batched)")
-    return out
-
-
-def _drw_batched_torch(x, w_col, w_row, max_iters):
-    """The torch path of tv1w_2d_batched: the layout of _dr2_layout, the weight maps laid out to match (row_major = 1: C order;
-    0: every image's map column-major)."""
-    M, N, batch, row_major, xin = _dr2_layout(x, batched=True)
-    assert tuple(w_col.shape) == (batch, M - 1, N) and tuple(w_row.shape) == (batch, M, N - 1)
-    w1, w2 = _drw_lay(w_col, xin, row_major), _drw_lay(w_row, xin, row_major)
-    geom = (M, N, batch, row_major, int(max_iters))
-    if _needs_grad(x, w_col, w_row):
-        return _autograd().DRW.apply(xin, w1, w2, geom)
-    return _drw_solve(xin, w1, w2, geom)
+    _w2_method(method)
+    return _tv2w(x, w_col, w_row, max_iters, method, batched=True, backward=backward)
 
 
 def _drw_lay(w, xin, row_major):
@@ -499,33 +445,6 @@ def _dr2_layout(x, batched):
     return M, N, batch, row_major, xin
 
 
-def _dr2_torch(x, w, max_iters, batched):
-    """The torch path of tv1_2d / tv1_2d_batched; recorded by the Function when grad mode is on and x, or w given as a 0-dim tensor,
-    requires grad."""
-    wf, w_t = _w_float(w)
-    M, N, batch, row_major, xin = _dr2_layout(x, batched)
-    geom = (M, N, batch, row_major, int(max_iters))
-    if _needs_grad(x, w_t):
-        return _autograd().DR2.apply(xin, wf, w_t, geom)
-    return _dr2_solve(xin, wf, geom)
-
-
-def _dr2_solve(xin, w, geom, tape=None):
-    """DR2_TV on xin, geom = (M, N, batch, row_major, max_iters) of _dr2_layout: proxtv_DR2_TV_dev_*, or given a tape (a uint8 CUDA
-    tensor, proxtv_DR2_TV_tape_bytes() long) proxtv_DR2_TV_record_dev_*, the lane engine's schedule in plain passes recording every
-    prox pass's segmentation.  The result has xin's layout."""
-    import torch
-    out = torch.empty_strided(xin.shape, xin.stride(), dtype=xin.dtype, device=xin.device)
-    info = np.zeros(_N_INFO)
-    M, N, batch, row_major, max_iters = geom
-    args = (M, N, batch, row_major, xin, w, w, out, max_iters)
-    if tape is None:       # returns 0 on success, like the reference's DR2_TV: only info[2] == 3 signals a failure
-        _dev_call("DR2_TV_dev", xin, *args, info, rc=False, info=info)
-    else:
-        _dev_call("DR2_TV_record_dev", xin, *args, tape, tape.numel(), info)
-    return out
-
-
 def tv1_2d_batched(x, w, max_iters=0, method="dr", backward=None):
     """``tv1_2d(method=method)`` on every image of x (B, H, W)  -- BASELINE config 5 with the default ``method='dr'``.
 
@@ -539,23 +458,7 @@ def tv1_2d_batched(x, w, max_iters=0, method="dr", backward=None):
     assert w >= 0
     assert method == "dr" or method in _CP2_ALGS, "method must be 'dr', 'condat', 'chambolle-pock' or 'chambolle-pock-acc'"
     _converged_backward(method, backward)
-    if method in _CP2_ALGS:
-        return _cp2(x, w, max_iters, method, batched=True, backward=backward)
-    if _is_torch(x):
-        return _dr2_torch(x, w, max_iters, batched=True)
-    x = np.asarray(x)
-    assert x.ndim == 3
-    f32 = x.dtype == np.float32
-    B, H, W = x.shape
-    # device layout: column-major images back to back == C-ordered (B, W, H) array of transposed images
-    xt = np.ascontiguousarray(np.transpose(x, (0, 2, 1)), dtype=np.float32 if f32 else np.float64)
-    out = _pool.empty(xt.shape, xt.dtype, "C")
-    info = np.zeros(_N_INFO)
-    lib = require_device()
-    fn = lib.proxtv_DR2_TV_batched_f32 if f32 else lib.proxtv_DR2_TV_batched_f64
-    fn(H, W, B, _ptr(xt), float(w), float(w), _ptr(out), int(max_iters), _ptr(info))
-    _check(info[2] != 3, "DR2_TV (batched)")
-    return np.transpose(out, (0, 2, 1))
+    return _tv2(x, w, max_iters, method, batched=True, backward=backward)
 
 
 def _converged_backward(method, backward):
@@ -568,119 +471,137 @@ def _converged_backward(method, backward):
                                   "method %r %s" % (method, why))
 
 
-def _cp2(x, w, max_iters, method, batched, backward=None):
-    """CondatChambollePock2_TV for tv1_2d / tv1_2d_batched.  numpy 2D: the reference's entry point on a Fortran-ordered float64 copy;
-    numpy 3D: proxtv_CP2_TV_batched_* on the C-ordered (B, H, W) array; torch: proxtv_CP2_TV_dev_* on either memory order
-    (_dr2_layout), result in the solved tensor's layout."""
-    alg = _CP2_ALGS[method]
-    if _is_torch(x):
-        grad = _needs_grad(x, w)
-        if grad and backward is None:
-            raise NotImplementedError("tv1_2d method %r has no backward pass by default; pass backward='converged' for the Jacobian of "
-                                      "the converged prox, use method='dr' or 'pd' for gradients, or call it under torch.no_grad() / "
-                                      "on a detached tensor" % method)
-        wf, w_t = _w_float(w)
-        M, N, batch, row_major, xin = _dr2_layout(x, batched)
-        geom = (M, N, batch, row_major, alg, int(max_iters))
-        if grad:
-            return _autograd().CP2.apply(xin, None, None, wf, w_t, geom)
-        return _cp2_solve(xin, None, None, wf, geom)
-    w = force_float_scalar(w)
-    if not batched:
-        x = np.asfortranarray(x, dtype="float64")
-        assert x.ndim == 2
-        lib = require_device()
-        y = _pool.empty(x.shape, np.float64, "F")
-        info = np.zeros(_N_INFO)
-        ok = lib.CondatChambollePock2_TV(x.shape[0], x.shape[1], _ptr(x), w, _ptr(y), alg, int(max_iters), _ptr(info))
-        _check(ok and info[2] != 3, "CondatChambollePock2_TV")
-        return y
-    x = np.asarray(x)
-    assert x.ndim == 3
-    dt = np.float32 if x.dtype == np.float32 else np.float64
-    x = np.ascontiguousarray(x, dtype=dt)
-    B, H, W = x.shape
-    out = _pool.empty(x.shape, dt, "C")
-    if x.size:
-        info = np.zeros(_N_INFO * B)
-        lib = require_device()
-        fn = lib.proxtv_CP2_TV_batched_f32 if dt == np.float32 else lib.proxtv_CP2_TV_batched_f64
-        ok = fn(H, W, B, 1, _ptr(x), w, _ptr(out), alg, int(max_iters), _ptr(info))
-        _check(ok and not np.any(info[2::3] == 3), "CondatChambollePock2_TV (batched)")
-    return out
-
-
-_CP2W_ALGS = {"condat": 0, "chambolle-pock": 1}          # the weighted solver's `alg` (proxtv_CP2W_TV_*)
-
-
-def _cp2w_method(method):
-    """True for the weighted primal-dual methods, False for 'dr'; anything else raises."""
+def _w2_method(method):
+    """Validates the method of the weighted 2D prox: 'dr', 'condat' or 'chambolle-pock'."""
     if method == "chambolle-pock-acc":
         raise NotImplementedError("the weighted 2D prox has no 'chambolle-pock-acc': its accelerated step rule takes gamma = 1 / lambda "
                                   "from one penalty, and per-edge weights give none; use 'condat' or 'chambolle-pock'")
     assert method == "dr" or method in _CP2W_ALGS, "method must be 'dr', 'condat' or 'chambolle-pock'"
-    return method != "dr"
 
 
-def _cp2_solve(xin, W1, W2, w, geom, tape=None):
-    """proxtv_CP2_TV_dev_* (W1 None: penalty w) or proxtv_CP2W_TV_dev_* (weight maps W1, W2 laid out like xin) on xin, geom = (M, N,
-    batch, row_major, alg, max_iters); given a tape (a uint8 CUDA tensor, proxtv_CP2_TV_tape_bytes() long) the _record_dev_ form, the
-    same solve followed by its fused-edge tape.  The result has xin's layout."""
-    import torch
-    M, N, batch, row_major, alg, max_iters = geom
-    out = torch.empty_strided(xin.shape, xin.stride(), dtype=xin.dtype, device=xin.device)
-    info = np.zeros(_N_INFO * batch)
-    entry, pen = ("CP2W_TV", (W1, W2)) if W1 is not None else ("CP2_TV", (w,))
-    args = (M, N, batch, row_major, xin, *pen, out, alg, max_iters, info)
-    if tape is None:
-        _dev_call(entry + "_dev", xin, *args, info=info)
-    else:
-        _dev_call(entry + "_record_dev", xin, *args, tape, tape.numel(), info=info)
+def _tv2(x, w, max_iters, method, batched, backward=None):
+    """tv1_2d / tv1_2d_batched with method 'dr' (DR2_TV) or a primal-dual one (CP2_TV, alg _CP2_ALGS[method]).  numpy: _tv2_numpy;
+    torch: either memory order (_dr2_layout), result in the solved tensor's layout."""
+    alg = _CP2_ALGS.get(method)
+    if not _is_torch(x):
+        return _tv2_numpy(x, w, max_iters, alg, batched)
+    if alg is not None and _needs_grad(x, w) and backward is None:
+        raise NotImplementedError("tv1_2d method %r has no backward pass by default; pass backward='converged' for the Jacobian of "
+                                  "the converged prox, use method='dr' or 'pd' for gradients, or call it under torch.no_grad() / "
+                                  "on a detached tensor" % method)
+    entry = "DR2_TV" if alg is None else "CP2_TV"
+    wf, w_t = _w_float(w)
+    M, N, batch, row_major, xin = _dr2_layout(x, batched)
+    geom = (M, N, batch, row_major, alg, int(max_iters))
+    if _needs_grad(x, w_t):
+        return _autograd().TV2.apply(xin, None, None, wf, w_t, entry, geom)
+    return _tv2_solve(entry, xin, None, None, wf, geom)
+
+
+def _tv2w(x, w_col, w_row, max_iters, method, batched, backward=None):
+    """tv1w_2d_batched, and tv1w_2d's primal-dual methods: 'dr' (DR2L1W_TV) or a primal-dual method (CP2W_TV, alg _CP2W_ALGS[method]).
+    numpy: _tv2w_numpy; torch: either memory order (_dr2_layout), the weight maps laid out to match, result in the solved tensor's
+    layout."""
+    alg = _CP2W_ALGS.get(method)
+    cp = alg is not None
+    if not _is_torch(x):
+        x = np.asarray(x)
+        assert x.ndim == (3 if batched else 2)
+        assert np.all(np.asarray(w_col) >= 0)
+        assert np.all(np.asarray(w_row) >= 0)
+        lead, (M, N) = x.shape[:-2], x.shape[-2:]
+        assert np.shape(w_col) == lead + (M - 1, N)
+        assert np.shape(w_row) == lead + (M, N - 1)
+        return _tv2w_numpy(x, w_col, w_row, max_iters, alg, batched)
+    if cp and _needs_grad(x, w_col, w_row) and backward is None:
+        raise NotImplementedError("tv1w_2d method %r has no backward pass by default; pass backward='converged' for the Jacobian of "
+                                  "the converged prox, use method='dr' for gradients, or call it under torch.no_grad() / on "
+                                  "detached tensors" % method)
+    entry = "CP2W_TV" if cp else "DR2L1W_TV_batched"
+    M, N, batch, row_major, xin = _dr2_layout(x, batched)
+    lead = (batch,) if batched else ()
+    assert tuple(w_col.shape) == lead + (M - 1, N) and tuple(w_row.shape) == lead + (M, N - 1)
+    w1, w2 = _drw_lay(w_col, xin, row_major), _drw_lay(w_row, xin, row_major)
+    geom = (M, N, batch, row_major, alg, int(max_iters))
+    if _needs_grad(x, w_col, w_row):
+        return _autograd().TV2.apply(xin, w1, w2, 0.0, None, entry, geom)
+    return _tv2_solve(entry, xin, w1, w2, 0.0, geom)
+
+
+def _host_images(x, batched, transposed=False):
+    """(x, out, M, N, batch, row_major): a numpy image or batch of images laid out as the host 2D entry points take it, and a result
+    array from the pool in the same layout.  One image: a Fortran-ordered float64 copy, a column-major batch of one (row_major = 0).  A
+    batch (B, M, N): float32 kept, anything else float64, C-ordered (row_major = 1) -- or, transposed, the C-ordered (B, N, M) array of
+    its transposes, which is the column-major images back to back (row_major = 0)."""
+    if not batched:
+        x = np.asfortranarray(x, dtype="float64")
+        assert x.ndim == 2
+        return (x, _pool.empty(x.shape, np.float64, "F")) + x.shape + (1, 0)
+    x = np.asarray(x)
+    assert x.ndim == 3
+    dt = np.float32 if x.dtype == np.float32 else np.float64
+    B, M, N = x.shape
+    x = np.ascontiguousarray(np.transpose(x, (0, 2, 1)) if transposed else x, dtype=dt)
+    return x, _pool.empty(x.shape, dt, "C"), M, N, B, 0 if transposed else 1
+
+
+def _tv2_numpy(x, w, max_iters, alg, batched):
+    """The numpy solve of tv1_2d / tv1_2d_batched: 'dr' (alg None) through proxtv_DR2_TV_batched_*, which returns 0 on success and takes
+    column-major images only (a batch is solved as its transposes and the result transposed back); the primal-dual methods through
+    proxtv_CP2_TV_batched_*, which an empty batch does not reach.  One image: Fortran-ordered float64 result; a batch: x's dtype."""
+    w = force_float_scalar(w)
+    x, out, M, N, B, row_major = _host_images(x, batched, transposed=alg is None)
+    info = np.zeros(_N_INFO * max(B, 1))
+    if alg is None:
+        _host_call("DR2_TV_batched", x, M, N, B, x, w, w, out, int(max_iters), info, rc=False, info=info)
+        return np.transpose(out, (0, 2, 1)) if batched else out
+    if x.size or not batched:
+        _host_call("CP2_TV_batched", x, M, N, B, row_major, x, w, out, alg, int(max_iters), info, info=info)
     return out
 
 
-def _cp2w(x, w_col, w_row, max_iters, method, batched, backward=None):
-    """The weighted primal-dual prox for tv1w_2d / tv1w_2d_batched (proxtv_CP2W_TV_*).  numpy 2D: a Fortran-ordered float64 copy (result
-    Fortran-ordered float64); numpy 3D: the C-ordered (B, H, W) array in x's dtype; torch: either memory order (_dr2_layout), the weight
-    maps laid out to match, result in the solved tensor's layout."""
-    alg = _CP2W_ALGS[method]
-    if _is_torch(x):
-        grad = _needs_grad(x, w_col, w_row)
-        if grad and backward is None:
-            raise NotImplementedError("tv1w_2d method %r has no backward pass by default; pass backward='converged' for the Jacobian of "
-                                      "the converged prox, use method='dr' for gradients, or call it under torch.no_grad() / on "
-                                      "detached tensors" % method)
-        M, N, batch, row_major, xin = _dr2_layout(x, batched)
-        lead = (batch,) if batched else ()
-        assert tuple(w_col.shape) == lead + (M - 1, N) and tuple(w_row.shape) == lead + (M, N - 1)
-        w1, w2 = _drw_lay(w_col, xin, row_major), _drw_lay(w_row, xin, row_major)
-        geom = (M, N, batch, row_major, alg, int(max_iters))
-        if grad:
-            return _autograd().CP2.apply(xin, w1, w2, 0.0, None, geom)
-        return _cp2_solve(xin, w1, w2, 0.0, geom)
-    x = np.asarray(x)
-    assert x.ndim == (3 if batched else 2)
-    assert np.all(np.asarray(w_col) >= 0)
-    assert np.all(np.asarray(w_row) >= 0)
-    if batched:
-        B, M, N = x.shape
-        dt, order, row_major = (np.float32 if x.dtype == np.float32 else np.float64), "C", 1
-    else:
-        B, (M, N) = 1, x.shape
-        dt, order, row_major = np.float64, "F", 0
-    lead = (B,) if batched else ()
-    assert np.shape(w_col) == lead + (M - 1, N)
-    assert np.shape(w_row) == lead + (M, N - 1)
-    x = np.require(x, dt, [order])
-    w1 = np.require(np.asarray(w_col), dt, [order])
-    w2 = np.require(np.asarray(w_row), dt, [order])
-    out = _pool.empty(x.shape, dt, order)
+def _tv2w_numpy(x, w_col, w_row, max_iters, alg, batched):
+    """The numpy solve of tv1w_2d / tv1w_2d_batched on checked input: 'dr' (alg None) through proxtv_DR2L1W_TV_batched_*, which returns 0
+    on success, the primal-dual methods through proxtv_CP2W_TV_batched_*; the weight maps laid out like the images (_host_images), and
+    an empty batch reaches neither.  One image: Fortran-ordered float64 result; a batch: C-ordered, x's dtype."""
+    x, out, M, N, B, row_major = _host_images(x, batched)
+    order = "C" if row_major else "F"
+    w1, w2 = (np.require(np.asarray(w), x.dtype, [order]) for w in (w_col, w_row))
     if x.size:
         info = np.zeros(_N_INFO * B)
-        lib = require_device()
-        fn = lib.proxtv_CP2W_TV_batched_f32 if dt == np.float32 else lib.proxtv_CP2W_TV_batched_f64
-        ok = fn(M, N, B, row_major, _ptr(x), _ptr(w1), _ptr(w2), _ptr(out), alg, int(max_iters), _ptr(info))
-        _check(ok and not np.any(info[2::3] == 3), "proxtv_CP2W_TV_batched")
+        entry, alg_ = ("DR2L1W_TV_batched", ()) if alg is None else ("CP2W_TV_batched", (alg,))
+        _host_call(entry, x, M, N, B, row_major, x, w1, w2, out, *alg_, int(max_iters), info, rc=alg is not None, info=info)
+    return out
+
+
+# The taped 2D solvers, by entry point (proxtv_<entry>_dev_* / _record_dev_* / _vjp_dev_*): the tape size, and whether the entry is a
+# Douglas-Rachford one.  Those take the tape before info when recording and (maxit, tape) in the backward, and their unrecorded solve
+# returns 0 on success like the reference's; the primal-dual ones take an alg, the tape after info and (tape, X) in the backward -- so
+# their result is saved for it -- and return 1.
+_TAPED = {
+    "DR2_TV": (lambda lib, M, N, batch, maxit: lib.proxtv_DR2_TV_tape_bytes(M, N, batch, maxit), True),
+    "DR2L1W_TV_batched": (lambda lib, M, N, batch, maxit: lib.proxtv_DR2L1W_TV_batched_tape_bytes(M, N, batch, maxit), True),
+    "CP2_TV": (lambda lib, M, N, batch, maxit: lib.proxtv_CP2_TV_tape_bytes(M, N, batch), False),
+    "CP2W_TV": (lambda lib, M, N, batch, maxit: lib.proxtv_CP2_TV_tape_bytes(M, N, batch), False),
+}
+
+
+def _tv2_solve(entry, xin, W1, W2, w, geom, tape=None):
+    """proxtv_<entry>_dev_* (a _TAPED entry) on xin, geom = (M, N, batch, row_major, alg, max_iters), alg None for the Douglas-Rachford
+    entries: with the weight maps W1, W2 laid out like xin, else the penalty w; given a tape (a uint8 CUDA tensor of the entry's tape
+    size) the _record_dev_ form, the same solve recording its tape.  The result has xin's layout."""
+    import torch
+    M, N, batch, row_major, alg, max_iters = geom
+    dr = _TAPED[entry][1]
+    out = torch.empty_strided(xin.shape, xin.stride(), dtype=xin.dtype, device=xin.device)
+    info = np.zeros(_N_INFO * max(batch, 1))
+    pen = (W1, W2) if W1 is not None else (w, w) if dr else (w,)
+    args = (M, N, batch, row_major, xin, *pen, out) + (() if dr else (alg,)) + (max_iters,)
+    if tape is None:
+        _dev_call(entry + "_dev", xin, *args, info, rc=not dr, info=info)
+    else:
+        rec = (tape, tape.numel(), info) if dr else (info, tape, tape.numel())
+        _dev_call(entry + "_record_dev", xin, *args, *rec, info=info)
     return out
 
 
@@ -713,41 +634,54 @@ def tvgen(x, ws, ds, ps, n_threads=1, max_iters=0):
     512 x 512 x 256 volume with 3 terms at 35 iterations is 105 passes x 16 MiB, about 1.64 GiB.  Double backward is not
     supported.  The forward result is the same either way.
     """
+    return _tvgen_front(tvgen, False, x, ws, ds, ps, n_threads, max_iters)
+
+
+tvgen.last_info = None
+
+
+def _nd_checks(ws, ds, ps, max_iters, n_threads=1):
     assert len(ws) == len(ds)
     assert len(ws) == len(ps)
     assert n_threads >= 1
     assert max_iters >= 0
+
+
+def _p1(ps):
+    if np.any(force_float_matrix(ps) != 1):
+        raise NotImplementedError("proxtv_b200 implements TV-L1 (p = 1) penalty terms only")
+
+
+def _nd_solver(npen, pdr=False):
+    """The solver of tvgen (two terms: PD2_TV, any other count: PD_TV) or, pdr, tvgen_pdr's PDR_TV."""
+    return "PDR_TV" if pdr else "PD2_TV" if npen == 2 else "PD_TV"
+
+
+def _tvgen_front(owner, pdr, x, ws, ds, ps, n_threads, max_iters):
+    """tvgen (owner tvgen: the proximal Dykstra solvers) and tvgen_pdr (owner tvgen_pdr, pdr: PDR_TV).  numpy: the reference's symbol on
+    a Fortran-ordered float64 copy -- float32 only where PD_TV has its own route, proxtv_PD_TV_f32 -- given ws itself when it is a
+    float64 ndarray (PD_TV and PDR_TV scale it in place); sets owner.last_info.  torch: _nd_torch."""
+    _nd_checks(ws, ds, ps, max_iters, n_threads)
     if _is_torch(x):
-        if np.any(force_float_matrix(ps) != 1):
-            raise NotImplementedError("proxtv_b200 implements TV-L1 (p = 1) penalty terms only")
+        _p1(ps)
         lam, ws_t = _ws_floats(ws)
-        return _nd_torch("PD2_TV" if len(lam) == 2 else "PD_TV", x, lam, ws_t, ds, max_iters)
-    info = np.zeros(_N_INFO)
-    f32 = isinstance(x, np.ndarray) and x.dtype == np.float32 and len(ws) != 2
+        return _nd_torch(_nd_solver(len(lam), pdr), owner, x, lam, ws_t, ds, max_iters)
+    solver = _nd_solver(len(ws), pdr)
+    f32 = solver == "PD_TV" and isinstance(x, np.ndarray) and x.dtype == np.float32
     x = np.asfortranarray(x, dtype="float32" if f32 else "float64")
     ws = force_float_matrix(ws)
     ps = force_float_matrix(ps)
+    _p1(ps)
     y = _pool.empty(np.shape(x), x.dtype, "F")
-    if np.any(ps != 1):
-        raise NotImplementedError("proxtv_b200 implements TV-L1 (p = 1) penalty terms only")
-    lib = require_device()
+    info = np.zeros(_N_INFO)
     dsa = np.array(ds, dtype=np.float64)
     ns = np.array(x.shape, dtype=np.int32)
-    if len(ws) == 2:
-        ok = lib.PD2_TV(_ptr(x), _ptr(ws), _ptr(ps), _ptr(dsa), _ptr(y), _ptr(info), _ptr(ns), x.ndim, 2,
-                        int(n_threads), int(max_iters))
-    elif f32:
-        ok = lib.proxtv_PD_TV_f32(_ptr(x), _ptr(ws), _ptr(dsa), _ptr(y), _ptr(info), _ptr(ns), x.ndim, len(ws),
-                                  int(max_iters))
+    if f32:
+        _host_call("PD_TV", x, x, ws, dsa, y, info, ns, x.ndim, len(ws), int(max_iters), info=info)
     else:
-        ok = lib.PD_TV(_ptr(x), _ptr(ws), _ptr(ps), _ptr(dsa), _ptr(y), _ptr(info), _ptr(ns), x.ndim, len(ws),
-                       int(n_threads), int(max_iters))
-    _check(ok and info[2] != 3, "tvgen")
-    tvgen.last_info = info
+        _host_call(solver, None, x, ws, ps, dsa, y, info, ns, x.ndim, len(ws), int(n_threads), int(max_iters), info=info)
+    owner.last_info = info
     return y
-
-
-tvgen.last_info = None
 
 
 def _f_contiguous(x):
@@ -760,16 +694,17 @@ def _f_contiguous(x):
     return True
 
 
-def _pdr_layout(x, ds):
-    """(ns, dims, xin) of an N-D CUDA tensor for the column-major solver: a Fortran-ordered x is taken as it is, with its shape and
-    axes; anything else is a C-ordered array (copied to C order unless it is one already), which is the column-major array of the
-    reversed shape, so axis a becomes nds + 1 - a and no transpose is made."""
+def _nd_layout(x, ds, batched=False):
+    """(ns, dims, xin) of an N-D CUDA tensor for the column-major solvers; batched: a batch of items along its first axis, ns and dims
+    those of an item.  Items that are column-major and back to back (the batch axis slowest) are taken as they are, with their shape
+    and axes; anything else is a C-ordered array (copied to C order unless it is one already), each item of which is the column-major
+    array of its reversed shape (_pdr_c_order), so no transpose is made."""
     import torch
-    assert x.is_cuda and x.dtype in (torch.float64, torch.float32) and x.dim() >= 1
-    if _f_contiguous(x) and not x.is_contiguous():
-        return [int(n) for n in x.shape], [float(d) for d in ds], x
+    assert x.is_cuda and x.dtype in (torch.float64, torch.float32) and x.dim() >= (2 if batched else 1)
+    if not x.is_contiguous() and _f_contiguous(x.movedim(0, -1) if batched else x):
+        return [int(n) for n in x.shape[batched:]], [float(d) for d in ds], x
     xin = x.contiguous()
-    return _pdr_c_order(xin.shape, ds) + (xin,)
+    return _pdr_c_order(xin.shape[batched:], ds) + (xin,)
 
 
 def _pdr_c_order(shape, ds):
@@ -780,32 +715,38 @@ def _pdr_c_order(shape, ds):
 
 def _ws_floats(ws):
     """(the penalties as a list of floats, ws when it is a tensor else None) of a list, ndarray or 1-D tensor; ws is not written."""
-    import torch
     if _is_torch(ws):
+        import torch
         assert ws.dim() == 1, "ws must be a 1-D tensor of one penalty per term"
         return [float(v) for v in ws.detach().to(device="cpu", dtype=torch.float64).numpy()], ws
     return [float(v) for v in np.asarray(ws, dtype=np.float64).ravel()], None
 
 
-def _nd_torch(solver, x, lam, ws_t, ds, max_iters):
-    """The torch path of tvgen_pdr, tvgen and tv1_2d(method='pd'); recorded by the Function when grad mode is on and x, or the
-    penalty tensor ws_t, requires grad.  lam: the penalties as floats; ws_t: None, a 1-D tensor of them, or a 0-dim tensor shared by
-    every term.  Nothing the caller passed is written: the solve gets a float64 copy of lam, which PDR_TV and PD_TV scale in place."""
+def _nd_torch(solver, owner, x, lam, ws_t, ds, max_iters, batched=False):
+    """The torch path of tvgen_pdr, tvgen, tv1_2d(method='pd') and (batched) tvgen_batched; recorded by the Function when grad mode is
+    on and x, or the penalty tensor ws_t, requires grad.  lam: the penalties as floats; ws_t: None, a 1-D tensor of them, or a 0-dim
+    tensor shared by every term.  Nothing the caller passed is written: the solve gets a float64 copy of lam, which PDR_TV and PD_TV
+    scale in place.  Sets owner.last_info."""
+    import torch
     assert len(lam) == len(ds)
     assert ws_t is None or tuple(ws_t.shape) in ((), (len(lam),)), "ws must be one penalty per term, or one 0-dim penalty for all"
-    ns, dims, xin = _pdr_layout(x, ds)
-    args = (solver, np.array(ns, dtype=np.int32), np.array(dims, dtype=np.float64), np.array(lam, dtype=np.float64), int(max_iters))
+    ns, dims, xin = _nd_layout(x, ds, batched)
+    batch = int(x.shape[0]) if batched else 0
+    if batched and batch == 0:
+        owner.last_info = np.zeros((0, _N_INFO))
+        return torch.empty_like(x)
+    args = (solver, np.array(ns, dtype=np.int32), np.array(dims, dtype=np.float64), np.array(lam, dtype=np.float64), int(max_iters),
+            owner, batch)
     if _needs_grad(x, ws_t):
         return _autograd().ND.apply(xin, ws_t, *args)
     return _nd_solve(xin, *args)[0]
 
 
-def _nd_solve(xin, solver, nsa, dsa, lama, max_iters, tape=None, batch=0):
-    """proxtv_<solver>_dev_* (solver: "PDR_TV", "PD_TV" or "PD2_TV") on xin, column-major over nsa (see _pdr_layout), or given a tape
+def _nd_solve(xin, solver, nsa, dsa, lama, max_iters, owner, batch=0, tape=None):
+    """proxtv_<solver>_dev_* (solver: "PDR_TV", "PD_TV" or "PD2_TV") on xin, column-major over nsa (see _nd_layout), or given a tape
     (a uint8 CUDA tensor, proxtv_<solver>_tape_bytes() long) proxtv_<solver>_record_dev_*, the same solve recording every prox pass's
     segmentation.  batch >= 1 (PD_TV / PD2_TV): xin holds `batch` items over nsa back to back, solved by proxtv_<solver>_batched_dev_* /
-    _batched_record_dev_*, and info is (batch, 3).  Sets the last_info of the public function that runs the solver; returns (result in
-    xin's layout, info)."""
+    _batched_record_dev_*, and info is (batch, 3).  Sets owner.last_info; returns (result in xin's layout, info)."""
     import torch
     out = torch.empty_strided(xin.shape, xin.stride(), dtype=xin.dtype, device=xin.device)
     info = np.zeros(_N_INFO * max(batch, 1))
@@ -818,9 +759,7 @@ def _nd_solve(xin, solver, nsa, dsa, lama, max_iters, tape=None, batch=0):
         _dev_call(solver + kind + "_record_dev", xin, *args, tape, tape.numel(), info=info)
     if batch:
         info = info.reshape(batch, _N_INFO)
-        tvgen_batched.last_info = info
-    else:
-        (tvgen_pdr if solver == "PDR_TV" else tvgen).last_info = info
+    owner.last_info = info
     return out, info
 
 
@@ -850,31 +789,13 @@ def tvgen_batched(x, ws, ds, ps, max_iters=0):
     perturbation changes it the map jumps.  The tape is allocated for ``max_iters`` iterations of the whole batch, B times the single
     capacity: PD_TV with 3 terms at 35 iterations takes about 1.64 GiB per 512 x 512 x 256 item.  Double backward is not supported.
     """
-    assert len(ws) == len(ds)
-    assert len(ws) == len(ps)
-    assert max_iters >= 0
-    if np.any(force_float_matrix(ps) != 1):
-        raise NotImplementedError("proxtv_b200 implements TV-L1 (p = 1) penalty terms only")
+    _nd_checks(ws, ds, ps, max_iters)
+    _p1(ps)
     lam, ws_t = _ws_floats(ws)
     assert ws_t is None or tuple(ws_t.shape) in ((), (len(lam),)), "ws must be one penalty per term, or one 0-dim penalty for all"
-    solver = "PD2_TV" if len(lam) == 2 else "PD_TV"
-    lama = np.array(lam, dtype=np.float64)
+    solver = _nd_solver(len(lam))
     if _is_torch(x):
-        import torch
-        assert x.is_cuda and x.dtype in (torch.float64, torch.float32) and x.dim() >= 2
-        B, s = int(x.shape[0]), [int(n) for n in x.shape[1:]]
-        if B == 0:
-            tvgen_batched.last_info = np.zeros((0, _N_INFO))
-            return torch.empty_like(x)
-        if not x.is_contiguous() and _f_contiguous(x[0]) and (B == 1 or x.stride(0) == int(np.prod(s))):
-            xin, ns, dims = x, s, [float(d) for d in ds]              # items column-major, back to back
-        else:
-            xin = x.contiguous()
-            ns, dims = _pdr_c_order(s, ds)
-        args = (solver, np.array(ns, dtype=np.int32), np.array(dims, dtype=np.float64), lama, int(max_iters))
-        if _needs_grad(x, ws_t):
-            return _autograd().ND.apply(xin, ws_t, *args, B)
-        return _nd_solve(xin, *args, None, B)[0]
+        return _nd_torch(solver, tvgen_batched, x, lam, ws_t, ds, max_iters, batched=True)
     x = np.asarray(x)
     f32 = x.dtype == np.float32
     assert x.ndim >= 2
@@ -887,10 +808,9 @@ def tvgen_batched(x, ws, ds, ps, max_iters=0):
     out = np.empty_like(xt)
     info = np.zeros(_N_INFO * B)
     ns = np.array(x.shape[1:], dtype=np.int32)
-    dsa = np.array(ds, dtype=np.float64)
-    fn = getattr(require_device(), "proxtv_%s_batched_%s" % (solver, "f32" if f32 else "f64"))
-    ok = fn(_ptr(xt), _ptr(lama), _ptr(dsa), _ptr(out), _ptr(info), _ptr(ns), len(ns), len(lama), B, int(max_iters))
-    _check(ok and not np.any(info[2::3] == 3), "tvgen_batched")
+    lama = np.array(lam, dtype=np.float64)
+    _host_call(solver + "_batched", xt, xt, lama, np.array(ds, dtype=np.float64), out, info, ns, len(ns), len(lama), B, int(max_iters),
+               info=info)
     tvgen_batched.last_info = info.reshape(B, _N_INFO)
     return np.transpose(out, rev)
 
@@ -916,29 +836,7 @@ def tvgen_pdr(x, ws, ds, ps, n_threads=1, max_iters=0):
     exact vector-Jacobian product of the fixed-iteration splitting that is computed (proxtv_PDR_TV_vjp_dev_*, DESIGN.md section 13),
     run on the current CUDA stream; double backward is not supported.  The forward result is the same either way.
     """
-    assert len(ws) == len(ds)
-    assert len(ws) == len(ps)
-    assert n_threads >= 1
-    assert max_iters >= 0
-    if _is_torch(x):
-        if np.any(force_float_matrix(ps) != 1):
-            raise NotImplementedError("proxtv_b200 implements TV-L1 (p = 1) penalty terms only")
-        lam, ws_t = _ws_floats(ws)
-        return _nd_torch("PDR_TV", x, lam, ws_t, ds, max_iters)
-    info = np.zeros(_N_INFO)
-    x = np.asfortranarray(x, dtype="float64")
-    ws = force_float_matrix(ws)
-    ps = force_float_matrix(ps)
-    if np.any(ps != 1):
-        raise NotImplementedError("proxtv_b200 implements TV-L1 (p = 1) penalty terms only")
-    y = _pool.empty(np.shape(x), x.dtype, "F")
-    lib = require_device()
-    dsa = np.array(ds, dtype=np.float64)
-    ns = np.array(x.shape, dtype=np.int32)
-    ok = lib.PDR_TV(_ptr(x), _ptr(ws), _ptr(ps), _ptr(dsa), _ptr(y), _ptr(info), _ptr(ns), x.ndim, len(ws), int(n_threads), int(max_iters))
-    _check(ok and info[2] != 3, "tvgen_pdr")
-    tvgen_pdr.last_info = info
-    return y
+    return _tvgen_front(tvgen_pdr, True, x, ws, ds, ps, n_threads, max_iters)
 
 
 tvgen_pdr.last_info = None
@@ -982,26 +880,31 @@ def _autograd():
             g_w = _penalty_grad(gw, ctx.w_like) if need_w_t else None
             return (gx if need_x else None), None, g_w, (gw if need_wt else None)
 
-    class DRW(torch.autograd.Function):
-        """apply(Y, W1, W2, geom) of _drw_solve.  backward: proxtv_DR2L1W_TV_batched_vjp_dev_*, with NULL for a weight map whose input
-        does not need its gradient; the upstream gradient is taken in the output's layout, the gradients come in their inputs'."""
+    class TV2(torch.autograd.Function):
+        """apply(xin, W1, W2, w, w_t, entry, geom) of _tv2_solve (W1 None: the penalty w, read from w_t when that is a tensor).
+        backward: proxtv_<entry>_vjp_dev_* -- the exact vector-Jacobian product of the unrolled splitting (DR2_TV, DR2L1W_TV) or the
+        Jacobian of the converged prox at the recorded partition (CP2_TV, CP2W_TV) -- with per-edge weight gradients (NULL for a map that
+        needs none) or glam per image and axis; the upstream gradient is taken in the output's layout, the gradients come in their
+        inputs'."""
         @staticmethod
-        def forward(ctx, Y, W1, W2, geom):
-            M, N, batch, _, max_iters = geom
-            nb = int(require_device().proxtv_DR2L1W_TV_batched_tape_bytes(M, N, batch, max_iters))
-            tape = torch.empty(nb, dtype=torch.uint8, device=Y.device)
-            out = _drw_solve(Y, W1, W2, geom, tape)
-            ctx.save_for_backward(tape)
-            ctx.geom = geom
-            ctx.layouts = [(t.shape, t.stride(), t.dtype) for t in (out, W1, W2)]
+        def forward(ctx, xin, W1, W2, w, w_t, entry, geom):
+            M, N, batch, _, _, max_iters = geom
+            tape_bytes, dr = _TAPED[entry]
+            tape = torch.empty(int(tape_bytes(require_device(), M, N, batch, max_iters)), dtype=torch.uint8, device=xin.device)
+            out = _tv2_solve(entry, xin, W1, W2, w, geom, tape)
+            ctx.save_for_backward(tape, None if dr else out)
+            ctx.entry, ctx.geom = entry, geom
+            ctx.layouts = [(t.shape, t.stride(), t.dtype) if t is not None else None for t in (out, W1, W2)]
+            ctx.w_like = (w_t.dtype, w_t.device, ()) if w_t is not None else None
             return out
 
         @staticmethod
         @once_differentiable
         def backward(ctx, gout):
-            (tape,) = ctx.saved_tensors
-            M, N, batch, row_major, max_iters = ctx.geom
-            need_y, need_w1, need_w2, _ = ctx.needs_input_grad
+            tape, out = ctx.saved_tensors
+            M, N, batch, row_major, _, max_iters = ctx.geom
+            dr = _TAPED[ctx.entry][1]
+            need_x, need_w1, need_w2, _, need_w_t, _, _ = ctx.needs_input_grad
 
             def like(i):
                 shape, stride, dt = ctx.layouts[i]
@@ -1009,46 +912,24 @@ def _autograd():
             g = like(0)                                   # the upstream gradient in the output's layout
             g.copy_(gout)
             gY = like(0)
-            gW1 = like(1) if need_w1 else None
-            gW2 = like(2) if need_w2 else None
-            _dev_call("DR2L1W_TV_batched_vjp_dev", g, M, N, batch, row_major, max_iters, tape, g, gY, gW1, gW2)
-            return (gY if need_y else None), gW1, gW2, None
-
-    class DR2(torch.autograd.Function):
-        """apply(xin, w, w_t, geom) of _dr2_solve.  backward: proxtv_DR2_TV_vjp_dev_*, the exact vector-Jacobian product of the
-        unrolled iteration; glam per image and axis."""
-        @staticmethod
-        def forward(ctx, xin, w, w_t, geom):
-            M, N, batch, _, max_iters = geom
-            tape = torch.empty(int(require_device().proxtv_DR2_TV_tape_bytes(M, N, batch, max_iters)), dtype=torch.uint8, device=xin.device)
-            out = _dr2_solve(xin, w, geom, tape)
-            ctx.save_for_backward(tape)
-            ctx.geom, ctx.layout = geom, (out.shape, out.stride(), out.dtype)
-            ctx.w_like = (w_t.dtype, w_t.device, ()) if w_t is not None else None
-            return out
-
-        @staticmethod
-        @once_differentiable
-        def backward(ctx, gout):
-            (tape,) = ctx.saved_tensors
-            M, N, batch, row_major, max_iters = ctx.geom
-            shape, stride, dt = ctx.layout
-            need_x, _, need_w_t, _ = ctx.needs_input_grad
-            g = torch.empty_strided(shape, stride, dtype=dt, device=tape.device)      # the upstream gradient in the output's layout
-            g.copy_(gout)
-            gY = torch.empty_strided(shape, stride, dtype=dt, device=tape.device)
+            lead = (max_iters, tape) if dr else (tape, out)
+            if ctx.layouts[1] is not None:
+                gW1 = like(1) if need_w1 else None
+                gW2 = like(2) if need_w2 else None
+                _dev_call(ctx.entry + "_vjp_dev", g, M, N, batch, row_major, *lead, g, gY, gW1, gW2, *(() if dr else (None,)))
+                return (gY if need_x else None), gW1, gW2, None, None, None, None
             glam = torch.empty(2 * batch, dtype=torch.float64, device=tape.device) if need_w_t else None
-            _dev_call("DR2_TV_vjp_dev", g, M, N, batch, row_major, max_iters, tape, g, gY, glam)
+            _dev_call(ctx.entry + "_vjp_dev", g, M, N, batch, row_major, *lead, g, gY, glam)
             g_w = _penalty_grad(glam, ctx.w_like) if need_w_t else None
-            return (gY if need_x else None), None, g_w, None
+            return (gY if need_x else None), None, None, None, g_w, None, None
 
     class ND(torch.autograd.Function):
-        """apply(xin, ws_t, solver, nsa, dsa, lama, max_iters[, batch]) of _nd_solve; ctx also keeps the iteration count the solve ran
-        (the Dykstra solvers' stop rule picks it; batch >= 1: each item's K).  backward: proxtv_<solver>_vjp_dev_*; the gradient of ws_t
-        is npen * glam for PDR_TV and PD_TV (glam: the gradients of the scaled penalties), glam for PD2_TV.  batch >= 1:
+        """apply(xin, ws_t, solver, nsa, dsa, lama, max_iters, owner, batch) of _nd_solve; ctx also keeps the iteration count the solve
+        ran (the Dykstra solvers' stop rule picks it; batch >= 1: each item's K).  backward: proxtv_<solver>_vjp_dev_*; the gradient of
+        ws_t is npen * glam for PDR_TV and PD_TV (glam: the gradients of the scaled penalties), glam for PD2_TV.  batch >= 1:
         proxtv_<solver>_batched_vjp_dev_*, whose per-item glam is of the penalties as given for both solvers, summed over the items."""
         @staticmethod
-        def forward(ctx, xin, ws_t, solver, nsa, dsa, lama, max_iters, batch=0):
+        def forward(ctx, xin, ws_t, solver, nsa, dsa, lama, max_iters, owner, batch):
             lib = require_device()
             if batch:
                 tape_bytes = getattr(lib, "proxtv_%s_batched_tape_bytes" % solver)
@@ -1057,7 +938,7 @@ def _autograd():
                 tape_bytes = getattr(lib, "proxtv_%s_tape_bytes" % solver)
                 nb = int(tape_bytes(_ptr(nsa), len(nsa), len(lama), max_iters))  # 0: too large; the record call refuses it
             tape = torch.empty(max(nb, 256), dtype=torch.uint8, device=xin.device)
-            out, info = _nd_solve(xin, solver, nsa, dsa, lama, max_iters, tape, batch)
+            out, info = _nd_solve(xin, solver, nsa, dsa, lama, max_iters, owner, batch, tape)
             ctx.save_for_backward(tape)
             iters = info[:, 0].astype(np.int64) if batch else int(info[0])
             ctx.geom, ctx.layout = (solver, nsa, dsa, max_iters, iters, batch), (out.shape, out.stride(), out.dtype)
@@ -1086,42 +967,4 @@ def _autograd():
             g_ws = _penalty_grad(glam if solver == "PD2_TV" else glam * float(npen), ctx.ws_like) if need_ws else None
             return (gY if need_x else None), g_ws, *rest
 
-    class CP2(torch.autograd.Function):
-        """apply(xin, W1, W2, w, w_t, geom) of _cp2_solve (W1 None: the penalty w, read from w_t when that is a tensor).  backward:
-        proxtv_CP2_TV_vjp_dev_* / proxtv_CP2W_TV_vjp_dev_*, the Jacobian of the converged prox at the recorded partition -- gx = the
-        cluster means of the upstream gradient, per-edge weight gradients (NULL for a map that needs none), glam per image and axis."""
-        @staticmethod
-        def forward(ctx, xin, W1, W2, w, w_t, geom):
-            M, N, batch = geom[:3]
-            tape = torch.empty(int(require_device().proxtv_CP2_TV_tape_bytes(M, N, batch)), dtype=torch.uint8, device=xin.device)
-            out = _cp2_solve(xin, W1, W2, w, geom, tape)
-            ctx.save_for_backward(tape, out)
-            ctx.geom = geom
-            ctx.layouts = [(t.shape, t.stride(), t.dtype) if t is not None else None for t in (out, W1, W2)]
-            ctx.w_like = (w_t.dtype, w_t.device, ()) if w_t is not None else None
-            return out
-
-        @staticmethod
-        @once_differentiable
-        def backward(ctx, gout):
-            tape, out = ctx.saved_tensors
-            M, N, batch, row_major = ctx.geom[:4]
-            need_x, need_w1, need_w2, _, need_w_t, _ = ctx.needs_input_grad
-
-            def like(i):
-                shape, stride, dt = ctx.layouts[i]
-                return torch.empty_strided(shape, stride, dtype=dt, device=tape.device)
-            g = like(0)                                   # the upstream gradient in the output's layout
-            g.copy_(gout)
-            gY = like(0)
-            if ctx.layouts[1] is not None:
-                gW1 = like(1) if need_w1 else None
-                gW2 = like(2) if need_w2 else None
-                _dev_call("CP2W_TV_vjp_dev", g, M, N, batch, row_major, tape, out, g, gY, gW1, gW2, None)
-                return (gY if need_x else None), gW1, gW2, None, None, None
-            glam = torch.empty(2 * batch, dtype=torch.float64, device=tape.device) if need_w_t else None
-            _dev_call("CP2_TV_vjp_dev", g, M, N, batch, row_major, tape, out, g, gY, glam)
-            g_w = _penalty_grad(glam, ctx.w_like) if need_w_t else None
-            return (gY if need_x else None), None, None, None, g_w, None
-
-    return types.SimpleNamespace(ProxRows=ProxRows, DRW=DRW, DR2=DR2, ND=ND, CP2=CP2)
+    return types.SimpleNamespace(ProxRows=ProxRows, TV2=TV2, ND=ND)
