@@ -656,8 +656,9 @@ template <typename T> struct PdrvPtrs { T* gz[64]; };
 // The backward workspace of the three solvers, in order: npen arrays a.gz (PD2_TV: gp, and gq when npen = 2), Sk (PD_TV: Gk; PD2_TV
 // with npen = 1: gq), h, sc, gw (only when glam is wanted), the VJP scratch of the largest term, the double sums.  Returns its size
 // and, unless ws is nullptr, splits ws into *L.
-// batch >= 1 (section 16): every array holds the whole batch, the double sums one set of REDUCE_BLOCKS per item, then the device copies of
-// the slot table and of the slot map.
+// batch = 0 (the single-item entry points): the double sums are REDUCE_BLOCKS + 8 doubles, and PD_TV / PD2_TV's one item keeps its slot
+// table and slot map in the last 8.  batch >= 1 (section 16): every array holds the whole batch, the double sums one set of
+// REDUCE_BLOCKS per item, then the device copies of the slot table and of the slot map.
 template <typename T> struct NdVjpWs {
     PdrvPtrs<T> a;
     T *Sk, *h, *sc, *gw;
@@ -682,8 +683,13 @@ template <typename T> static size_t nd_vjp_ws(const NdTerms& t, int npen, bool w
     L->gw = want_glam ? (T*)take(ab) : nullptr;
     L->vscr = take(al256(vs));
     L->scratch = (double*)take(batch > 0 ? al256((size_t)batch * REDUCE_BLOCKS * sizeof(double)) : DR2V_SCRATCH);
-    L->dslots = batch > 0 ? (int*)take(al256((size_t)batch * sizeof(int))) : nullptr;
-    L->dmap = batch > 0 ? (int*)take(al256((size_t)batch * sizeof(int))) : nullptr;
+    if (batch > 0) {
+        L->dslots = (int*)take(al256((size_t)batch * sizeof(int)));
+        L->dmap = (int*)take(al256((size_t)batch * sizeof(int)));
+    } else {
+        L->dslots = ws ? (int*)(L->scratch + REDUCE_BLOCKS) : nullptr;
+        L->dmap = ws ? L->dslots + 1 : nullptr;
+    }
     return off;
 }
 template <typename T> size_t ws_bytes_nd_vjp(const NdTerms& t, int npen, bool want_glam, int batch) {
@@ -728,32 +734,25 @@ __global__ void k_pdrv(PdrvPtrs<T> a, int npen, int i, bool start, bool more, co
 // PD_TV (pd_device, k = npen terms, kk = (T)k, lam_i scaled by k), all K npen passes reach out (pass p = j npen + i):
 //     z_i = Y ;  j = 0..K-1:  p_i = P_i(z_i) ; x = ((0 + p_0 / kk) + p_1 / kk) + ... ; z_i = z_i + (x - p_i)       out = x (j = K-1)
 //   backward, in T (sums term by term, i in order):
-//     a_i = 0 ; gk = G / kk ; h = gk - a_0                                                                  (k_pdv, start)
+//     a_i = 0 ; gk = G / kk ; h = gk - 0                                                    (the start values, nd_vjp_items)
 //     j = K-1..0:  i = 0..k-1:  a_i = a_i + S_{j,i}(h) ; h = gk - a_{i+1}     (one VJP pass, then k_pdv; after the last term:
 //                  s = (a_0 + a_1) + ... ; j > 0: gk = s / kk, h = gk - a_0 ; j = 0: gY = s)
 // PD2_TV (pd2_device, npen <= 2, penalties as given), passes 2j (z = P_0(x + p)) and 2j + 1 (x' = P_1(z + q)); npen = 1: one
 // iteration, x' = z, pass 0.  Backward with the adjoints (gx, gp, gq) of (x', p', q') = (G, 0, 0); after the first step gx == gp, so
 // one array gp holds both:
-//     gp = 0 ; gq = 0 ; h = G - 0                                                                           (k_pd2v, mode 0)
-//     j = K-1..0:  [npen = 2: gv = S_1(h) ; gq = gq + gv ; h = gq - gp                                      (mode 1)]
+//     gp = 0 ; gq = 0 ; h = G - 0                                                           (the start values, nd_vjp_items)
+//     j = K-1..0:  [npen = 2: gv = S_1(h) ; gq = gq + gv ; h = gq - gp                                      (k_pd2v, mode 1)]
 //                  gu = S_0(h) ; gp = gp + gu ; j > 0: h = gp - gq ; j = 0: gY = gp                           (mode 2)
 // Penalty gradients: glam_i = 0.0 ; glam_i = glam_i + sum(gw) per pass of term i in backward order, gw the pass's edge gradients for
 // its upstream gradient h, each sum img_sums' fixed two-stage double sum.  No atomics.
 
-// start: every a_l = 0, gk = G / kk, h = gk - a_0.  Else the step after term i's VJP pass (result sc): a_i = a_i + sc, then h = gk - a_{i+1}
-// for the next term; after the last term s = (a_0 + a_1) + ... ; more: gk = s / kk, h = gk - a_0 ; else gY = s.
+// The step after term i's VJP pass (result sc): a_i = a_i + sc, then h = gk - a_{i+1} for the next term; after the last term
+// s = (a_0 + a_1) + ... ; more: gk = s / kk, h = gk - a_0 ; else gY = s.
 template <typename T>
-__global__ void k_pdv(PdrvPtrs<T> a, int npen, int i, bool start, bool more, const T* __restrict__ G, const T* __restrict__ sc,
-                      T* __restrict__ Gk, T* __restrict__ h, T* __restrict__ gY, long long n) {
+__global__ void k_pdv(PdrvPtrs<T> a, int npen, int i, bool more, const T* __restrict__ sc, T* __restrict__ Gk, T* __restrict__ h,
+                      T* __restrict__ gY, long long n) {
     const T kk = (T)npen;
     GRID_STRIDE(q, n) {
-        if (start) {
-            for (int l = 0; l < npen; l++) a.gz[l][q] = T(0);
-            const T gk = G[q] / kk;
-            Gk[q] = gk;
-            h[q] = gk - T(0);
-            continue;
-        }
         const T v = a.gz[i][q] + sc[q];
         a.gz[i][q] = v;
         if (i + 1 < npen) { h[q] = Gk[q] - a.gz[i + 1][q]; continue; }
@@ -769,16 +768,13 @@ __global__ void k_pdv(PdrvPtrs<T> a, int npen, int i, bool start, bool more, con
     }
 }
 
-// mode 0: gp = 0, gq = 0, h = G - 0.  1 (after P_1's VJP, sc = gv): gq = gq + gv, h = gq - gp.  2 (after P_0's VJP, sc = gu): gp = gp + gu;
-// more: h = gp - gq ; else gY = gp.
+// mode 1 (after P_1's VJP, sc = gv): gq = gq + gv, h = gq - gp.  2 (after P_0's VJP, sc = gu): gp = gp + gu; more: h = gp - gq ; else
+// gY = gp.
 template <typename T>
-__global__ void k_pd2v(int mode, bool more, const T* __restrict__ G, const T* __restrict__ sc, T* __restrict__ gp, T* __restrict__ gq,
-                       T* __restrict__ h, T* __restrict__ gY, long long n) {
+__global__ void k_pd2v(int mode, bool more, const T* __restrict__ sc, T* __restrict__ gp, T* __restrict__ gq, T* __restrict__ h,
+                       T* __restrict__ gY, long long n) {
     GRID_STRIDE(q, n) {
-        if (mode == 0) {
-            gp[q] = T(0); gq[q] = T(0);
-            h[q] = G[q] - T(0);
-        } else if (mode == 1) {
+        if (mode == 1) {
             const T v = gq[q] + sc[q];
             gq[q] = v;
             h[q] = v - gp[q];
@@ -803,17 +799,16 @@ __global__ void k_item_final(const double* __restrict__ partial, int nblk, const
 }
 __global__ void k_scale(double* __restrict__ a, long long n, double f) { GRID_STRIDE(q, n) a[q] = a[q] * f; }
 
-// Batched PD_TV / PD2_TV (section 16): the recurrences above per item, item b over its own K_b = Kb[b].  The adjoint arrays keep the
-// forward's slot order (nd_slots); going down from the largest K, the items with K_b = j + 1 join at iteration j with the start values
-// (PD_TV: a_i = 0, gk = G_b / kk, h = gk - 0; PD2_TV: gp = gq = 0, h = G_b - 0), the others moving to their new slots through sc.  Each
-// pass's edge gradients are summed per item with the single-item call's blocks; glam[b npen + i] of the penalties as given.
+// PD_TV / PD2_TV, single-item (batch = 1) or batched (section 16): the recurrences above per item, item b over its own K_b = Kb[b].
+// tb: the tape's first pass.  The adjoint arrays keep the forward's slot order (nd_slots); going down from the largest K, the items with
+// K_b = j + 1 join at iteration j with the start values, the others moving to their new slots through sc.  Each pass's edge gradients
+// are summed per item, into glam[b npen + i] (PD_TV: of the scaled penalties).
 template <typename T>
-static cudaError_t nd_vjp_items(NdSolver s, const NdTerms& t, int npen, int batch, const int* Kb, const void* tape, const T* gout, T* gY,
+static cudaError_t nd_vjp_items(NdSolver s, const NdTerms& t, int npen, int batch, const int* Kb, const char* tb, const T* gout, T* gY,
                                 double* glam, const NdVjpWs<T>& L, cudaStream_t st) {
 #define RTRY(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) return e__; } while (0)
     const long long n = t.n;
     const size_t sb = ptvv::vjp_tape_set_bytes(n * batch);
-    const char* tb = (const char*)tape + nd_tape_head_bytes(batch);
     const T kk = (T)npen;
     int Kmax = 0;
     for (int b = 0; b < batch; b++) if (Kb[b] > Kmax) Kmax = Kb[b];
@@ -858,6 +853,7 @@ static cudaError_t nd_vjp_items(NdSolver s, const NdTerms& t, int npen, int batc
             RTRY(cudaMemcpyAsync(L.dmap, map.data(), (size_t)m2 * sizeof(int), cudaMemcpyHostToDevice, st));
             RTRY(cudaMemcpyAsync(L.dslots, slots.data(), (size_t)m2 * sizeof(int), cudaMemcpyHostToDevice, st));
             for (int a = 0; a < narr; a++) {
+                if (!m) { RTRY(ew_slot_gather<T>(nullptr, arr[a], L.dmap, m2, n, init[a], gout, kk, st)); continue; }   // start values only
                 RTRY(ew_slot_gather<T>(arr[a], L.sc, L.dmap, m2, n, init[a], gout, kk, st));
                 RTRY(cudaMemcpyAsync(arr[a], L.sc, (size_t)m2 * n * sizeof(T), cudaMemcpyDeviceToDevice, st));
             }
@@ -868,26 +864,21 @@ static cudaError_t nd_vjp_items(NdSolver s, const NdTerms& t, int npen, int batc
             for (int i = 0; i < npen; i++) {
                 RTRY(pass((long long)j * npen + i, i));
                 KernelSpan sp(KC_ELEMENTWISE, 1, st);
-                k_pdv<T><<<ge, 256, 0, st>>>(L.a, npen, i, false, j > 0, gout, L.sc, L.Sk, L.h, gY, nm);
+                k_pdv<T><<<ge, 256, 0, st>>>(L.a, npen, i, j > 0, L.sc, L.Sk, L.h, gY, nm);
                 RTRY(cudaGetLastError());
             }
         } else {
             if (npen >= 2) {
                 RTRY(pass(2LL * j + 1, 1));
                 KernelSpan sp(KC_ELEMENTWISE, 1, st);
-                k_pd2v<T><<<ge, 256, 0, st>>>(1, true, gout, L.sc, gp, gq, L.h, gY, nm);
+                k_pd2v<T><<<ge, 256, 0, st>>>(1, true, L.sc, gp, gq, L.h, gY, nm);
                 RTRY(cudaGetLastError());
             }
             RTRY(pass(npen >= 2 ? 2LL * j : 0, 0));
             KernelSpan sp(KC_ELEMENTWISE, 1, st);
-            k_pd2v<T><<<ge, 256, 0, st>>>(2, j > 0, gout, L.sc, gp, gq, L.h, gY, nm);
+            k_pd2v<T><<<ge, 256, 0, st>>>(2, j > 0, L.sc, gp, gq, L.h, gY, nm);
             RTRY(cudaGetLastError());
         }
-    }
-    if (glam && s == ND_PD) {                            // d/d of the penalties as given: PD_TV solved with npen lam_i
-        KernelSpan sp(KC_ELEMENTWISE, 1, st);
-        k_scale<<<ew_grid((long long)batch * npen), 256, 0, st>>>(glam, (long long)batch * npen, (double)npen);
-        RTRY(cudaGetLastError());
     }
     return cudaSuccess;
 #undef RTRY
@@ -898,20 +889,23 @@ cudaError_t nd_vjp_device(NdSolver s, const NdTerms& t, int npen, int maxIters, 
                           double* glam, void* ws, cudaStream_t st, int batch, const int* Kb) {
 #define RTRY(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) return e__; } while (0)
     const long long n = t.n;
-    if (batch > 0) {
-        if (glam) RTRY(cudaMemsetAsync(glam, 0, (size_t)batch * npen * sizeof(double), st));
-        if (n == 0) return cudaSuccess;
-        NdVjpWs<T> L;
-        nd_vjp_ws<T>(t, npen, glam != nullptr, (char*)ws, &L, batch);
-        return nd_vjp_items<T>(s, t, npen, batch, Kb, tape, gout, gY, glam, L, st);
-    }
-    const int K = nd_K(s, maxIters, iters);
-    if (glam) RTRY(cudaMemsetAsync(glam, 0, (size_t)npen * sizeof(double), st));
-    if (n == 0 || K <= 0) return cudaSuccess;
+    const int nb = batch > 0 ? batch : 1;
+    if (glam) RTRY(cudaMemsetAsync(glam, 0, (size_t)nb * npen * sizeof(double), st));
+    const int K = batch > 0 ? 0 : nd_K(s, maxIters, iters);
+    if (n == 0 || (batch == 0 && K <= 0)) return cudaSuccess;
     NdVjpWs<T> L;
-    nd_vjp_ws<T>(t, npen, glam != nullptr, (char*)ws, &L);
+    nd_vjp_ws<T>(t, npen, glam != nullptr, (char*)ws, &L, batch);
+    const char* tb = (const char*)tape + nd_tape_head_bytes(batch);
+    if (s != ND_PDR) {
+        RTRY(nd_vjp_items<T>(s, t, npen, nb, batch > 0 ? Kb : &K, tb, gout, gY, glam, L, st));
+        if (batch > 0 && glam && s == ND_PD) {           // d/d of the penalties as given: PD_TV solved with npen lam_i
+            KernelSpan sp(KC_ELEMENTWISE, 1, st);
+            k_scale<<<ew_grid((long long)batch * npen), 256, 0, st>>>(glam, (long long)batch * npen, (double)npen);
+            RTRY(cudaGetLastError());
+        }
+        return cudaSuccess;
+    }
     const size_t sb = ptvv::vjp_tape_set_bytes(n);
-    const char* tb = (const char*)tape + 256;
     const unsigned ge = ew_grid(n);
     // the VJP of pass p (term i) for the upstream h into sc, and its edge gradients into glam[i]
     auto pass = [&](long long p, int i) -> cudaError_t {
@@ -922,48 +916,17 @@ cudaError_t nd_vjp_device(NdSolver s, const NdTerms& t, int npen, int maxIters, 
         if (glam) RTRY(img_sums<T>(L.gw, g.nf * (long long)(g.len - 1), 1, L.scratch, nullptr, glam, i, 1.0, st));
         return cudaSuccess;
     };
-    if (s == ND_PDR) {
-        auto step = [&](bool start, int i, bool more) -> cudaError_t {
-            KernelSpan sp(KC_ELEMENTWISE, 1, st);
-            k_pdrv<T><<<ge, 256, 0, st>>>(L.a, npen, i, start, more, gout, L.sc, L.Sk, L.h, gY, n);
-            return cudaGetLastError();
-        };
-        RTRY(step(true, npen - 1, K >= 2));
-        for (int j = K - 2; j >= 0; j--)
-            for (int i = 0; i < npen; i++) {
-                RTRY(pass((long long)j * npen + i, i));
-                RTRY(step(false, i, j > 0));
-            }
-    } else if (s == ND_PD) {
-        auto step = [&](bool start, int i, bool more) -> cudaError_t {
-            KernelSpan sp(KC_ELEMENTWISE, 1, st);
-            k_pdv<T><<<ge, 256, 0, st>>>(L.a, npen, i, start, more, gout, L.sc, L.Sk, L.h, gY, n);
-            return cudaGetLastError();
-        };
-        RTRY(step(true, 0, true));
-        for (int j = K - 1; j >= 0; j--)
-            for (int i = 0; i < npen; i++) {
-                RTRY(pass((long long)j * npen + i, i));
-                RTRY(step(false, i, j > 0));
-            }
-    } else {
-        T* gp = L.a.gz[0];
-        T* gq = npen >= 2 ? L.a.gz[1] : L.Sk;
-        auto step = [&](int mode, bool more) -> cudaError_t {
-            KernelSpan sp(KC_ELEMENTWISE, 1, st);
-            k_pd2v<T><<<ge, 256, 0, st>>>(mode, more, gout, L.sc, gp, gq, L.h, gY, n);
-            return cudaGetLastError();
-        };
-        RTRY(step(0, true));
-        for (int j = K - 1; j >= 0; j--) {
-            if (npen >= 2) {
-                RTRY(pass(2LL * j + 1, 1));
-                RTRY(step(1, true));
-            }
-            RTRY(pass(npen >= 2 ? 2LL * j : 0, 0));
-            RTRY(step(2, j > 0));
+    auto step = [&](bool start, int i, bool more) -> cudaError_t {
+        KernelSpan sp(KC_ELEMENTWISE, 1, st);
+        k_pdrv<T><<<ge, 256, 0, st>>>(L.a, npen, i, start, more, gout, L.sc, L.Sk, L.h, gY, n);
+        return cudaGetLastError();
+    };
+    RTRY(step(true, npen - 1, K >= 2));
+    for (int j = K - 2; j >= 0; j--)
+        for (int i = 0; i < npen; i++) {
+            RTRY(pass((long long)j * npen + i, i));
+            RTRY(step(false, i, j > 0));
         }
-    }
     return cudaSuccess;
 #undef RTRY
 }

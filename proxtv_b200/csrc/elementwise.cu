@@ -134,120 +134,26 @@ template <typename T> cudaError_t ew_dr_reflect_bcast(const T* t, const T* x1, T
     KernelSpan span(KC_ELEMENTWISE, 1, st);
     k_dr_reflect_bcast<T><<<grid_for(n, 256), 256, 0, st>>>(t, x1, s, n, per_image, len, inc); return cudaGetLastError(); }
 
-// ---- stop criterion: mean |a - b|  (src/TV2Dopt.cpp:273-277) ----
-template <typename T> __global__ void k_absdiff_partial(const T* __restrict__ a, const T* __restrict__ b, long long n, double* __restrict__ partial) {
-    double acc = 0;
-    for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x)
-        acc += fabs((double)a[q] - (double)b[q]);
-    acc = block_sum(acc);
-    if (threadIdx.x == 0) partial[blockIdx.x] = acc;
-}
+// sums the nblk partials of one reduction in a fixed order: *result = that / n
 __global__ void k_final_mean(const double* __restrict__ partial, int nblk, long long n, double* __restrict__ result) {
     double acc = 0;
     for (int q = threadIdx.x; q < nblk; q += blockDim.x) acc += partial[q];
     acc = block_sum(acc);
     if (threadIdx.x == 0) *result = acc / (double)n;
 }
-template <typename T> cudaError_t ew_mean_abs_diff(const T* a, const T* b, long long n, double* scratch, double* result, cudaStream_t st) {
-    KernelSpan span(KC_ELEMENTWISE, 2, st);
-    int nblk = (int)grid_for(n, 256, 8); if (nblk > REDUCE_BLOCKS) nblk = REDUCE_BLOCKS;
-    k_absdiff_partial<T><<<nblk, 256, 0, st>>>(a, b, n, scratch);
-    k_final_mean<<<1, 256, 0, st>>>(scratch, nblk, n, result);
-    return cudaGetLastError();
-}
 
-// ---- parallel proximal Dykstra combine (src/TVNDopt.cpp:212-227): x = sum_i p_i/k ; z_i += x - p_i ; stop = mean|x - x_old| ----
-template <typename T> __global__ void k_pd_combine(T* const* __restrict__ p, T* const* __restrict__ z, int k, T* __restrict__ x,
-                                                  long long n, double* __restrict__ partial) {
-    double acc = 0;
-    const T kk = (T)k;
-    for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
-        T xo = x[q], xn = T(0);
-        for (int i = 0; i < k; i++) xn += p[i][q] / kk;
-        for (int i = 0; i < k; i++) z[i][q] += xn - p[i][q];
-        x[q] = xn;
-        acc += fabs((double)xn - (double)xo);
-    }
-    acc = block_sum(acc);
-    if (threadIdx.x == 0) partial[blockIdx.x] = acc;
-}
-// Same arithmetic, K known at compile time, the 2K array pointers passed by value and 16-byte vector accesses: the generic kernel
-// above chases 2K pointers through memory and moves 4-8 bytes per access.
-template <typename T, int K> struct PdPtrs { T* p[K]; T* z[K]; };
-template <typename T, int K>
-__global__ void __launch_bounds__(256) k_pd_combine_vec(PdPtrs<T, K> a, T* __restrict__ x, long long n, double* __restrict__ partial) {
-    constexpr int V = 16 / (int)sizeof(T);
-    struct alignas(16) Vec { T v[V]; };
-    double acc = 0;
-    const T kk = (T)K;
-    const long long nv = n / V;
-    for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < nv; q += (long long)gridDim.x * blockDim.x) {
-        Vec xo = reinterpret_cast<const Vec*>(x)[q], pv[K], zv[K], xn;
-#pragma unroll
-        for (int i = 0; i < K; i++) { pv[i] = reinterpret_cast<const Vec*>(a.p[i])[q]; zv[i] = reinterpret_cast<const Vec*>(a.z[i])[q]; }
-#pragma unroll
-        for (int e = 0; e < V; e++) {
-            T s = T(0);
-#pragma unroll
-            for (int i = 0; i < K; i++) s += pv[i].v[e] / kk;
-#pragma unroll
-            for (int i = 0; i < K; i++) zv[i].v[e] += s - pv[i].v[e];
-            xn.v[e] = s;
-            acc += fabs((double)s - (double)xo.v[e]);
-        }
-#pragma unroll
-        for (int i = 0; i < K; i++) reinterpret_cast<Vec*>(a.z[i])[q] = zv[i];
-        reinterpret_cast<Vec*>(x)[q] = xn;
-    }
-    if (blockIdx.x == 0 && threadIdx.x == 0)                       // the < V trailing elements
-        for (long long q = nv * V; q < n; q++) {
-            T xo = x[q], s = T(0);
-            for (int i = 0; i < K; i++) s += a.p[i][q] / kk;
-            for (int i = 0; i < K; i++) a.z[i][q] += s - a.p[i][q];
-            x[q] = s; acc += fabs((double)s - (double)xo);
-        }
-    acc = block_sum(acc);
-    if (threadIdx.x == 0) partial[blockIdx.x] = acc;
-}
-template <typename T, int K>
-static void launch_pd_vec(T* const* hp, T* const* hz, T* x, long long n, double* scratch, int nblk, cudaStream_t st) {
-    PdPtrs<T, K> a;
-    for (int i = 0; i < K; i++) { a.p[i] = hp[i]; a.z[i] = hz[i]; }
-    k_pd_combine_vec<T, K><<<nblk, 256, 0, st>>>(a, x, n, scratch);
-}
-
-// dp, dz: device copies of the pointer arrays (generic kernel); hp, hz: the same pointers on the host (vector kernel, K <= 4)
-template <typename T> cudaError_t ew_pd_combine(T* const* dp, T* const* dz, T* const* hp, T* const* hz, int k, T* x, long long n,
-                                                double* scratch, double* result, cudaStream_t st) {
-    KernelSpan span(KC_ELEMENTWISE, 2, st);
-    bool aligned = (((uintptr_t)x) & 15) == 0;
-    for (int i = 0; i < k && aligned; i++) aligned = ((((uintptr_t)hp[i]) | ((uintptr_t)hz[i])) & 15) == 0;
-    int nblk;
-    if (aligned && k >= 1 && k <= 4) {
-        nblk = (int)grid_for(n, 256, 16 / (int)sizeof(T) * 2); if (nblk > REDUCE_BLOCKS) nblk = REDUCE_BLOCKS;
-        switch (k) {
-            case 1: launch_pd_vec<T, 1>(hp, hz, x, n, scratch, nblk, st); break;
-            case 2: launch_pd_vec<T, 2>(hp, hz, x, n, scratch, nblk, st); break;
-            case 3: launch_pd_vec<T, 3>(hp, hz, x, n, scratch, nblk, st); break;
-            default: launch_pd_vec<T, 4>(hp, hz, x, n, scratch, nblk, st); break;
-        }
-    } else {
-        nblk = (int)grid_for(n, 256, 4); if (nblk > REDUCE_BLOCKS) nblk = REDUCE_BLOCKS;
-        k_pd_combine<T><<<nblk, 256, 0, st>>>(dp, dz, k, x, n, scratch);
-    }
-    k_final_mean<<<1, 256, 0, st>>>(scratch, nblk, n, result);
-    return cudaGetLastError();
-}
-
-// ---- the per-item forms of the two stop reductions (batched PD_TV / PD2_TV, DESIGN.md section 16) ----
+// ---- the proximal Dykstra solvers' combine and stop value (PD_TV / PD2_TV, src/TVNDopt.cpp:212-227, src/TV2Dopt.cpp:273-277), for
+//      `items` running items at once (DESIGN.md section 16; a single-item call is one item) ----
 // A 2D grid: blockIdx.y = slot s0 + y of the running items, each item n elements at s * n; blockIdx.x = one of the nblk reduction blocks
-// the single-item call uses for n elements, with the same element-to-thread assignment inside the item (element indices, not
-// addresses: a slot that is not 16-byte aligned sums in the order of the aligned single-item call).  partial[s * nblk + x].
+// an item of n elements gets.  The element-to-thread assignment inside an item goes by element index, not address, so an item sums in
+// the same order in every slot and in every batch.  partial[s * nblk + x].
 constexpr int MAX_GRID_Y = 65535;
 
-// PD_TV's combine: K 1..4, the vector kernel's assignment (V = 16 / sizeof(T) consecutive elements per thread step, the trailing n % V by
-// block 0's thread 0 after its loop); VLD: the slots are 16-byte aligned, so the V elements load as one vector.  k_pd_combine_items_gen:
-// the generic kernel's assignment (one element per step), k terms, the pointer tables in device memory.
+// PD_TV's combine, x = sum_i p_i/k ; z_i += x - p_i ; stop = mean|x - x_old|.  k_pd_combine_items: K 1..4 known at compile time, the 2K
+// array pointers passed by value, V = 16 / sizeof(T) consecutive elements per thread step, the trailing n % V by block 0's thread 0
+// after its loop; VLD: every item's arrays are 16-byte aligned, so the V elements move as one vector.  k_pd_combine_items_gen: any k,
+// one element per step, the pointer tables in device memory.
+template <typename T, int K> struct PdPtrs { T* p[K]; T* z[K]; };
 template <typename T>
 __global__ void k_pd_combine_items_gen(T* const* __restrict__ p, T* const* __restrict__ z, int k, T* __restrict__ x, long long n, int s0,
                                        double* __restrict__ partial) {
@@ -337,7 +243,7 @@ __global__ void __launch_bounds__(256, 1) k_pd_combine_items(PdPtrs<T, K> a, T* 
     acc = block_sum(acc);
     if (threadIdx.x == 0) partial[(long long)(s0 + blockIdx.y) * gridDim.x + blockIdx.x] = acc;
 }
-// PD2_TV's stop value: k_absdiff_partial per item
+// PD2_TV's stop value, mean |a - b|
 template <typename T> __global__ void k_absdiff_items(const T* __restrict__ a, const T* __restrict__ b, long long n, int s0,
                                                       double* __restrict__ partial) {
     const long long base = (long long)(s0 + blockIdx.y) * n;
@@ -347,7 +253,7 @@ template <typename T> __global__ void k_absdiff_items(const T* __restrict__ a, c
     acc = block_sum(acc);
     if (threadIdx.x == 0) partial[(long long)(s0 + blockIdx.y) * gridDim.x + blockIdx.x] = acc;
 }
-// k_final_mean per item: block s sums its nblk partials in the single-item order, result[s] = that / n
+// k_final_mean per item: block s sums its nblk partials, result[s] = that / n
 __global__ void k_final_mean_items(const double* __restrict__ partial, int nblk, long long n, double* __restrict__ result) {
     double acc = 0;
     for (int q = threadIdx.x; q < nblk; q += blockDim.x) acc += partial[(long long)blockIdx.x * nblk + q];
@@ -362,12 +268,15 @@ static void launch_pd_items(T* const* hp, T* const* hz, bool vld, T* x, long lon
     if (vld) k_pd_combine_items<T, K, true><<<dim3(nblk, ny), 256, 0, st>>>(a, x, n, s0, scratch);
     else k_pd_combine_items<T, K, false><<<dim3(nblk, ny), 256, 0, st>>>(a, x, n, s0, scratch);
 }
+// dp, dz: device copies of the pointer arrays (generic kernel); hp, hz: the same pointers on the host (K <= 4)
 template <typename T> cudaError_t ew_pd_combine_items(T* const* dp, T* const* dz, T* const* hp, T* const* hz, int k, T* x, long long n,
                                                       int items, double* scratch, double* result, cudaStream_t st) {
     KernelSpan span(KC_ELEMENTWISE, 1 + (items + MAX_GRID_Y - 1) / MAX_GRID_Y, st);
-    // the single-item call's choice for an aligned x and workspace: the vector kernel for 1..4 terms
-    const bool vec = k >= 1 && k <= 4;
-    const bool vld = ((n * (long long)sizeof(T)) & 15) == 0;            // every slot 16-byte aligned (the arrays are)
+    // the vector assignment for 1..4 terms when x and every p_i / z_i are 16-byte aligned (a batch's arrays are workspace, so always);
+    // VLD when every slot is aligned too: n * sizeof(T) a multiple of 16, or slot 0 alone
+    bool vec = k >= 1 && k <= 4 && (((uintptr_t)x) & 15) == 0;
+    for (int i = 0; i < k && vec; i++) vec = ((((uintptr_t)hp[i]) | ((uintptr_t)hz[i])) & 15) == 0;
+    const bool vld = items == 1 || ((n * (long long)sizeof(T)) & 15) == 0;
     int nblk = vec ? (int)grid_for(n, 256, 16 / (int)sizeof(T) * 2) : (int)grid_for(n, 256, 4);
     if (nblk > REDUCE_BLOCKS) nblk = REDUCE_BLOCKS;
     for (int s0 = 0; s0 < items; s0 += MAX_GRID_Y) {
@@ -396,22 +305,29 @@ template <typename T> cudaError_t ew_mean_abs_diff_items(const T* a, const T* b,
 }
 
 // Moves whole n-element slots: dst slot s = src slot map[s] when map[s] >= 0; map[s] = -1 - b: item b joins, with the start value init
-// 0: 0 ; 1: G_b / kk ; 2: G_b / kk - 0 ; 3: G_b - 0 (G_b = G + b n, the expressions of the backward's start steps, dr2_vjp.cu).
+// 0: 0 ; 1: G_b / kk ; 2: G_b / kk - 0 ; 3: G_b - 0 (G_b = G + b n, the start values of the PD_TV / PD2_TV backward, dr2_vjp.cu).
+// src is not read when every map[s] < 0.
 template <typename T> __global__ void k_slot_gather(const T* __restrict__ src, T* __restrict__ dst, const int* __restrict__ map, long long n,
-                                                    long long total, int init, const T* __restrict__ G, T kk) {
-    for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < total; q += (long long)gridDim.x * blockDim.x) {
-        const long long s = q / n, e = q - s * n;
+                                                    int slots, int init, const T* __restrict__ G, T kk) {
+    for (int s = blockIdx.y; s < slots; s += gridDim.y) {          // slots along y: no division per element
         const int m = map[s];
-        if (m >= 0) { dst[q] = src[(long long)m * n + e]; continue; }
-        const T g = init ? G[(long long)(-1 - m) * n + e] : T(0);
-        dst[q] = init == 0 ? T(0) : init == 1 ? g / kk : init == 2 ? g / kk - T(0) : g - T(0);
+        T* d = dst + (long long)s * n;
+        for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x) {
+            if (m >= 0) { d[e] = src[(long long)m * n + e]; continue; }
+            const T g = init ? G[(long long)(-1 - m) * n + e] : T(0);
+            d[e] = init == 0 ? T(0) : init == 1 ? g / kk : init == 2 ? g / kk - T(0) : g - T(0);
+        }
     }
 }
 template <typename T> cudaError_t ew_slot_gather(const T* src, T* dst, const int* map, int slots, long long n, int init, const T* G, T kk,
                                                  cudaStream_t st) {
     KernelSpan span(KC_ELEMENTWISE, 1, st);
-    const long long total = (long long)slots * n;
-    k_slot_gather<T><<<grid_for(total, 256), 256, 0, st>>>(src, dst, map, n, total, init, G, kk);
+    const unsigned gx = grid_for(n, 256);
+    unsigned gy = 132u * 32 / gx;                                   // grid_for's block budget, shared by the slots
+    if (gy > (unsigned)slots) gy = (unsigned)slots;
+    if (gy > (unsigned)MAX_GRID_Y) gy = MAX_GRID_Y;
+    if (gy < 1) gy = 1;
+    k_slot_gather<T><<<dim3(gx, gy), 256, 0, st>>>(src, dst, map, n, slots, init, G, kk);
     return cudaGetLastError();
 }
 
@@ -544,8 +460,6 @@ template <typename T> cudaError_t ew_mean_abs_step(const T* y, long long n, doub
     template cudaError_t ew_dr_final_rows<T>(const T*, const T*, const T*, T*, long long, cudaStream_t); \
     template cudaError_t ew_dual_update<T>(T*, const T*, const T*, long long, cudaStream_t); \
     template cudaError_t ew_dr_reflect_bcast<T>(const T*, const T*, T*, long long, long long, int, long long, cudaStream_t); \
-    template cudaError_t ew_mean_abs_diff<T>(const T*, const T*, long long, double*, double*, cudaStream_t); \
-    template cudaError_t ew_pd_combine<T>(T* const*, T* const*, T* const*, T* const*, int, T*, long long, double*, double*, cudaStream_t); \
     template cudaError_t ew_pdr_combine<T>(T* const*, T* const*, T* const*, T* const*, int, T*, long long, double*, double*, cudaStream_t); \
     template cudaError_t ew_pd_combine_items<T>(T* const*, T* const*, T* const*, T* const*, int, T*, long long, int, double*, double*, cudaStream_t); \
     template cudaError_t ew_mean_abs_diff_items<T>(const T*, const T*, long long, int, double*, double*, cudaStream_t); \

@@ -89,10 +89,6 @@ template <typename T> cudaError_t ew_dr_reflect_bcast(const T* t, const T* x1, T
                                                       long long inc, cudaStream_t st);
 template <typename T> cudaError_t prox_const_fibers(const T* c, long long c_stride, int batch, int n, T lam, T* x1, cudaStream_t st);
 template <typename T> cudaError_t ew_dual_update(T* p, const T* a, const T* b, long long n, cudaStream_t st);  // p += a - b
-template <typename T> cudaError_t ew_mean_abs_diff(const T* a, const T* b, long long n, double* scratch, double* result,
-                                                   cudaStream_t st);                  // *result = mean|a-b| (device)
-template <typename T> cudaError_t ew_pd_combine(T* const* dp, T* const* dz, T* const* hp, T* const* hz, int k, T* x, long long n,
-                                                double* scratch, double* result, cudaStream_t st);
 template <typename T> cudaError_t ew_pdr_combine(T* const* dp, T* const* dz, T* const* hp, T* const* hz, int k, T* x, long long n,
                                                  double* scratch, double* result, cudaStream_t st);
 template <typename T> cudaError_t ew_div_scalar(const T* y, T* x, long long n, T k, cudaStream_t st);             // x = y / k
@@ -100,9 +96,9 @@ template <typename T> cudaError_t ew_mean_abs_step(const T* y, long long n, doub
 template <typename T> cudaError_t ew_dr_first(const T* Y, const T* t, T* U, T* D, long long n, cudaStream_t st);  // D = t - t ; U = Y - (2 D - t)
 constexpr int REDUCE_BLOCKS = 1184;    // fixed, not the device's SM count (~9 per SM on a 132-SM H100): partial sums are combined in
                                        // the same fixed order on every GPU (deterministic)
-// The per-item stop values of a batched PD_TV / PD2_TV solve (DESIGN.md section 16): `items` running items of n elements in slots 0..items-1
-// of each array; result[s] = the value the single-item call (ew_pd_combine with aligned arrays / ew_mean_abs_diff) computes for slot s,
-// bit for bit.  scratch: items * REDUCE_BLOCKS doubles.
+// PD_TV's combine and PD2_TV's mean|a - b| with a stop value per item (DESIGN.md section 16): `items` running items of n elements in
+// slots 0..items-1 of each array (a single-item solve: one item); result[s] = slot s's stop value, the same bits whichever slot the
+// item sits in.  scratch: items * REDUCE_BLOCKS doubles.
 template <typename T> cudaError_t ew_pd_combine_items(T* const* dp, T* const* dz, T* const* hp, T* const* hz, int k, T* x, long long n,
                                                       int items, double* scratch, double* result, cudaStream_t st);
 template <typename T> cudaError_t ew_mean_abs_diff_items(const T* a, const T* b, long long n, int items, double* scratch, double* result,

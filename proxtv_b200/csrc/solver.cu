@@ -513,20 +513,23 @@ int nd_slots(const int* K, int batch, int j, int* slots) {
 // The fibers of `items` items of one term's geometry g: an item is the slowest axis, so its fibers are a contiguous range
 static FiberGeom items_geom(const FiberGeom& g, int items) { return FiberGeom{g.nf * items, g.len, g.inc}; }
 
-// The items of a batched PD_TV / PD2_TV solve (DESIGN.md section 16).  K[b] is INT_MAX while item b runs, then the iterations it ran; the
-// running items sit in the slots nd_slots gives them, slots[0..m).  Each iteration's stop values come back in one read-back; an item
-// that stops gets its info row and its x copied to its place in the output, and the others' state arrays move to their new slots through
-// a staging array (the moves of one array overlap, so they cannot be made in place).
+// The items of a PD_TV / PD2_TV solve (DESIGN.md section 16); a single-item call is one item.  K[b] is INT_MAX while item b runs, then
+// the iterations it ran; the running items sit in the slots nd_slots gives them, slots[0..m).  Each iteration's stop values come back in
+// one read-back; an item that stops gets its info row and its x copied to its place in the output, and the others' state arrays move to
+// their new slots through a staging array (the moves of one array overlap, so they cannot be made in place).
 template <typename T> struct NdItems {
     int batch = 0, m = 0; long long n = 0; T* out = nullptr; double* info = nullptr;
     std::vector<int> K, slots, next, map; std::vector<double> stop;
     T* x = nullptr; double* partial = nullptr; double* dstop = nullptr; int* dmap = nullptr;
-    // w: the workspace past the single-item layout of the whole batch (ws_bytes_pd)
-    void split(int b, long long n_, T* out_, double* info_, char* w) {
-        batch = b; m = b; n = n_; out = out_; info = info_;
-        K.assign(b, INT_MAX); slots.resize(b); next.resize(b); map.resize(b); stop.resize(b);
+    NdItems(int b, long long n_, T* out_, double* info_)
+        : batch(b), m(b), n(n_), out(out_), info(info_), K(b, INT_MAX), slots(b), next(b), map(b), stop(b) {
         nd_slots(K.data(), b, 0, slots.data());
-        if (!w) return;
+    }
+    // The device arrays.  w: a batch's, the workspace past the single-item layout of the whole batch (ws_bytes_pd).  nullptr: one item,
+    // which iterates in its output and reduces in the single-item layout's scratch and dres, so its workspace is the single-item one.
+    void split(char* w, double* scratch, double* dres) {
+        if (!w) { x = out; partial = scratch; dstop = dres; return; }
+        const int b = batch;
         x = (T*)w; w += align256((size_t)(n * b) * sizeof(T));
         partial = (double*)w; w += align256((size_t)b * REDUCE_BLOCKS * sizeof(double));
         dstop = (double*)w; w += align256((size_t)b * sizeof(double));
@@ -546,6 +549,7 @@ template <typename T> struct NdItems {
             if (go(stop[s])) continue;
             const int b = slots[s];
             K[b] = iters; row(b, iters, stop[s]); gone++;
+            if (x + (size_t)s * n == out + (size_t)b * n) continue;
             e = cudaMemcpyAsync(out + (size_t)b * n, x + (size_t)s * n, (size_t)n * sizeof(T), cudaMemcpyDeviceToDevice, st);
             if (e != cudaSuccess) return e;
         }
@@ -563,7 +567,7 @@ template <typename T> struct NdItems {
         slots.swap(next); m = m2;
         return cudaSuccess;
     }
-    // items that never ran (no elements, no terms): the single-item call's info
+    // items that never ran (no elements, no terms)
     void rest(int iters) { for (int b = 0; b < batch; b++) if (K[b] == INT_MAX) row(b, iters, DBL_MAX); }
 };
 
@@ -588,8 +592,11 @@ static int read_stop(const double* dres, double* stop, cudaStream_t st) {
     return e == cudaSuccess;
 }
 
-// tape != nullptr (the recorded forward, dr2_vjp.cu): after each pass the segmentation tape of its output is written -- z as pass
-// 2 iters, x as pass 2 iters + 1 (npen = 1: z as pass 0); nothing else changes.
+// The iteration of pd2_device and pd_device, over the running items of NdItems.  batch = 0 (the single-item entry points): one item that
+// iterates in x_out with the single-item workspace (ws_bytes_pd(n, npen)), info nullptr allowed.  batch >= 1: a batch iterates in the
+// workspace, and an item's x goes out when it stops.
+// PD2_TV.  tape != nullptr (the recorded forward, dr2_vjp.cu): after each pass the segmentation tape of its output is written -- z as
+// pass 2 iters, x as pass 2 iters + 1 (npen = 1: z as pass 0); nothing else changes.
 template <typename T>
 int pd2_device(const T* y, const double* lambdas, const double* dims, T* x_out, double* info, const int* ns, int nds, int npen,
                int maxIters, void* ws, Engine eng, cudaStream_t st, void* tape, int batch) {
@@ -602,23 +609,25 @@ int pd2_device(const T* y, const double* lambdas, const double* dims, T* x_out, 
     if (maxIters <= 0) maxIters = MAX_ITERS_PD;
     if (npen >= 1) eng = lane_guard<T>(eng, y, n * nb, npen >= 2 && lambdas[1] > lambdas[0] ? lambdas[1] : lambdas[0], st);
     if (npen < 1 || why) { printf("PD2_TV: invalid penalty dimensions\n"); if (info) info[INFO_RC] = RC_ERROR; return 0; }
-    double stop = DBL_MAX; int iters = 0;
-    NdItems<T> I;
+    double row1[3];
+    if (!info) info = row1;
+    NdItems<T> I(nb, n, x_out, info);
+    int iters = 0;
     if (n > 0) {
         const long long nt = n * nb;
         char* w = (char*)ws; const size_t ab = align256((size_t)nt * sizeof(T));
         T* p = (T*)w; w += ab; T* q = (T*)w; w += ab; T* z = (T*)w; w += ab; T* xl = (T*)w; w += ab;
         T* scr = (T*)w; w += 3 * ab;                 // staging of strided passes: 2 arrays + per-chunk masks / entering values
-        double* scratch = (double*)w; double* dres = scratch + REDUCE_BLOCKS;
-        if (batch) I.split(batch, n, x_out, info, (char*)ws + ws_bytes_pd<T>(nt, npen));
-        T* x = batch ? I.x : x_out;                  // a batch iterates in the workspace: an item's x goes out when it stops
+        double* scratch = (double*)w;
+        I.split(batch ? (char*)ws + ws_bytes_pd<T>(nt, npen) : nullptr, scratch, scratch + REDUCE_BLOCKS);
+        T* x = I.x;
         char* tp = tape ? (char*)tape + nd_tape_head_bytes(batch) : nullptr;
         T* const state[3] = {x, p, q};
         PTV_TRY(cudaMemcpyAsync(x, y, (size_t)nt * sizeof(T), cudaMemcpyDeviceToDevice, st));         // :132-137
         PTV_TRY(cudaMemsetAsync(p, 0, (size_t)nt * sizeof(T), st));
         PTV_TRY(cudaMemsetAsync(q, 0, (size_t)nt * sizeof(T), st));
-        while (batch ? I.m > 0 : stop > STOP_PD && (npen > 1 || !iters) && iters < maxIters) {        // :157
-            const int m = batch ? I.m : 1;
+        while (I.m > 0) {                                                                             // :157 per item
+            const int m = I.m;
             const long long nm = n * m;
             const FiberGeom g0 = items_geom(t.g[0], m), g1 = npen >= 2 ? items_geom(t.g[1], m) : g0;
             PTV_TRY(cudaMemcpyAsync(xl, x, (size_t)nm * sizeof(T), cudaMemcpyDeviceToDevice, st));
@@ -632,21 +641,14 @@ int pd2_device(const T* y, const double* lambdas, const double* dims, T* x_out, 
             } else {
                 PTV_TRY(cudaMemcpyAsync(x, z, (size_t)nm * sizeof(T), cudaMemcpyDeviceToDevice, st)); // :266-269
             }
-            if (batch) {                                                                              // :273-277 per item
-                PTV_TRY(ew_mean_abs_diff_items<T>(x, xl, n, m, I.partial, I.dstop, st));
-                iters++;
-                PTV_TRY(I.step(iters, [&](double s) { return s > STOP_PD && npen > 1 && iters < maxIters; }, state, npen >= 2 ? 3 : 2,
-                               scr, st));
-                continue;
-            }
-            PTV_TRY(ew_mean_abs_diff<T>(x, xl, n, scratch, dres, st));                                // :273-277
-            if (!read_stop(dres, &stop, st)) { PTV_TRY(cudaGetLastError()); PTV_TRY(cudaErrorUnknown); }
+            PTV_TRY(ew_mean_abs_diff_items<T>(x, xl, n, m, I.partial, I.dstop, st));                 // :273-277 per item
             iters++;
+            // the loop condition (:157), one iteration only with one term; info rows (:283-295)
+            PTV_TRY(I.step(iters, [&](double s) { return s > STOP_PD && npen > 1 && iters < maxIters; }, state, npen >= 2 ? 3 : 2,
+                           scr, st));
         }
     }
-    if (batch) { if (!I.batch) I.split(batch, 0, x_out, info, nullptr); I.rest(0); return 1; }
-    if (info) { info[INFO_ITERS] = iters; info[INFO_GAP] = stop;
-                info[INFO_RC] = iters >= MAX_ITERS_PD ? RC_ITERS : RC_OK; }                           // :283-295
+    I.rest(0);
     return 1;
 }
 
@@ -683,8 +685,8 @@ template <typename T> static cudaError_t pd_ws(void* ws, long long n, int npen, 
     return e;
 }
 
-// tape != nullptr (the recorded forward, dr2_vjp.cu): after each pass the segmentation tape of its output p_i is written as pass
-// iters * npen + i; nothing else changes.
+// PD_TV, with pd2_device's items and workspaces.  tape != nullptr (the recorded forward, dr2_vjp.cu): after each pass the segmentation
+// tape of its output p_i is written as pass iters * npen + i; nothing else changes.
 template <typename T>
 int pd_device(const T* y, const double* lam, const double* dims, T* x_out, double* info, const int* ns, int nds, int npen,
               int maxIters, void* ws, Engine eng, cudaStream_t st, void* tape, int batch) {
@@ -693,41 +695,36 @@ int pd_device(const T* y, const double* lam, const double* dims, T* x_out, doubl
     NdTerms t;
     if (!pd_start<T>("PD_TV", y, lam, dims, info, ns, nds, npen, &t, &eng, st, nb)) return 0;
     const long long n = t.n, nt = n * nb;
-    double stop = DBL_MAX; int iters = 0;
-    NdItems<T> I;
+    double row1[3];
+    if (!info) info = row1;
+    NdItems<T> I(nb, n, x_out, info);
+    int iters = 0;
     if (n > 0 && npen > 0) {
         PdWs<T> W;
         PTV_TRY(pd_ws<T>(ws, nt, npen, &W, st));
-        if (batch) I.split(batch, n, x_out, info, (char*)ws + ws_bytes_pd<T>(nt, npen));
-        T* x = batch ? I.x : x_out;                  // a batch iterates in the workspace: an item's x goes out when it stops
+        I.split(batch ? (char*)ws + ws_bytes_pd<T>(nt, npen) : nullptr, W.scratch, W.dres);
+        T* x = I.x;
         char* tp = tape ? (char*)tape + nd_tape_head_bytes(batch) : nullptr;
         T* state[65] = {x};
         for (int i = 0; i < npen; i++) state[1 + i] = W.hz[i];
         PTV_TRY(cudaMemsetAsync(x, 0, (size_t)nt * sizeof(T), st));                                   // :125-130
         for (int i = 0; i < npen; i++) PTV_TRY(cudaMemcpyAsync(W.hz[i], y, (size_t)nt * sizeof(T), cudaMemcpyDeviceToDevice, st));
-        while (batch ? I.m > 0 : stop > STOP_PD && iters < maxIters) {                               // :151
-            const int m = batch ? I.m : 1;
+        while (I.m > 0) {                                                                             // :151 per item
+            const int m = I.m;
             for (int i = 0; i < npen; i++) {
                 const FiberGeom g = items_geom(t.g[i], m);
                 PTV_TRY(prox_fibers<T>(W.hz[i], nullptr, IN_A, W.hp[i], 0, g, (T)lam[i], nullptr, eng, W.scr, st, 3 * n * m));  // :171-208
                 if (tp) PTV_TRY(nd_tape_pass<T>(tp, nt, (long long)iters * npen + i, W.hp[i], g, (T)lam[i], st));
             }
-            if (batch) {                                                                              // :212-227 per item
-                PTV_TRY(ew_pd_combine_items<T>(W.dp, W.dz, W.hp, W.hz, npen, x, n, m, I.partial, I.dstop, st));
-                iters++;
-                PTV_TRY(I.step(iters, [&](double s) { return s > STOP_PD && iters < maxIters; }, state, 1 + npen, W.scr, st));
-                continue;
-            }
-            PTV_TRY(ew_pd_combine<T>(W.dp, W.dz, W.hp, W.hz, npen, x, n, W.scratch, W.dres, st));             // :212-227
-            if (!read_stop(W.dres, &stop, st)) { PTV_TRY(cudaGetLastError()); PTV_TRY(cudaErrorUnknown); }
+            PTV_TRY(ew_pd_combine_items<T>(W.dp, W.dz, W.hp, W.hz, npen, x, n, m, I.partial, I.dstop, st));   // :212-227 per item
             iters++;
+            // the loop condition; info rows (:233-245)
+            PTV_TRY(I.step(iters, [&](double s) { return s > STOP_PD && iters < maxIters; }, state, 1 + npen, W.scr, st));
         }
     } else if (n > 0) {
         PTV_TRY(cudaMemsetAsync(x_out, 0, (size_t)nt * sizeof(T), st));
     }
-    if (batch) { if (!I.batch) I.split(batch, 0, x_out, info, nullptr); I.rest(0); return 1; }
-    if (info) { info[INFO_ITERS] = iters; info[INFO_GAP] = stop;
-                info[INFO_RC] = iters >= MAX_ITERS_PD ? RC_ITERS : RC_OK; }                           // :233-245
+    I.rest(0);
     return 1;
 }
 
