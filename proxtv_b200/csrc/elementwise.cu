@@ -435,18 +435,40 @@ template <typename T> cudaError_t ew_dr_first(const T* Y, const T* t, T* U, T* D
     return cudaGetLastError();
 }
 
-// mean |y[e + 1] - y[e]| over n consecutive elements: one block, fixed summation order (the lane-engine suitability test, solver.cu)
-template <typename T> __global__ void k_mean_abs_step(const T* __restrict__ y, long long n, double* __restrict__ out) {
-    __shared__ double sh[256];
+// mean |y[e + 1] - y[e]| over n consecutive elements (the lane-engine suitability test, solver.cu), in a fixed summation order: the
+// terms of e = j, j + 256, j + 512, ... are summed in that order into s_j, and the 256 sums s_j are combined by a pairwise tree.
+// Block j of k_abs_step_lanes forms s_j: its 256 threads load the terms (all loads in flight at once) into shared memory, one thread
+// adds them up; the serial chain is then shared-memory adds only, not one dependent global round trip per term as in a single block
+// of 256 threads walking the array (~400 us for 256k float64 elements on an H100, on every call of a solver under engine auto).
+constexpr int ABS_STEP_LANES = 256, ABS_STEP_CHUNK = 1024;
+template <typename T> __global__ void __launch_bounds__(256) k_abs_step_lanes(const T* __restrict__ y, long long n, double* __restrict__ part) {
+    __shared__ double term[ABS_STEP_CHUNK];
+    const long long j = blockIdx.x;
+    const long long cnt = n - 1 > j ? (n - 2 - j) / ABS_STEP_LANES + 1 : 0;          // e = j + k 256 with e + 1 < n
     double s = 0.0;
-    for (long long e = threadIdx.x; e + 1 < n; e += blockDim.x) s += fabs((double)y[e + 1] - (double)y[e]);
-    sh[threadIdx.x] = s;
+    for (long long k0 = 0; k0 < cnt; k0 += ABS_STEP_CHUNK) {
+        const int m = cnt - k0 < ABS_STEP_CHUNK ? (int)(cnt - k0) : ABS_STEP_CHUNK;
+        for (int k = threadIdx.x; k < m; k += blockDim.x) {
+            const long long e = j + (k0 + k) * ABS_STEP_LANES;
+            term[k] = fabs((double)y[e + 1] - (double)y[e]);
+        }
+        __syncthreads();
+        if (threadIdx.x == 0)
+            for (int k = 0; k < m; k++) s += term[k];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) part[j] = s;
+}
+__global__ void k_abs_step_tree(const double* __restrict__ part, long long n, double* __restrict__ out) {
+    __shared__ double sh[ABS_STEP_LANES];
+    sh[threadIdx.x] = part[threadIdx.x];
     __syncthreads();
-    for (int k = 128; k > 0; k >>= 1) { if ((int)threadIdx.x < k) sh[threadIdx.x] += sh[threadIdx.x + k]; __syncthreads(); }
+    for (int k = ABS_STEP_LANES / 2; k > 0; k >>= 1) { if ((int)threadIdx.x < k) sh[threadIdx.x] += sh[threadIdx.x + k]; __syncthreads(); }
     if (threadIdx.x == 0) out[0] = n > 1 ? sh[0] / (double)(n - 1) : 0.0;
 }
 template <typename T> cudaError_t ew_mean_abs_step(const T* y, long long n, double* out, cudaStream_t st) {
-    k_mean_abs_step<T><<<1, 256, 0, st>>>(y, n, out);
+    k_abs_step_lanes<T><<<ABS_STEP_LANES, 256, 0, st>>>(y, n, out + 1);
+    k_abs_step_tree<<<1, ABS_STEP_LANES, 0, st>>>(out + 1, n, out);
     return cudaGetLastError();
 }
 

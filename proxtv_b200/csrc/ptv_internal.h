@@ -92,7 +92,7 @@ template <typename T> cudaError_t ew_dual_update(T* p, const T* a, const T* b, l
 template <typename T> cudaError_t ew_pdr_combine(T* const* dp, T* const* dz, T* const* hp, T* const* hz, int k, T* x, long long n,
                                                  double* scratch, double* result, cudaStream_t st);
 template <typename T> cudaError_t ew_div_scalar(const T* y, T* x, long long n, T k, cudaStream_t st);             // x = y / k
-template <typename T> cudaError_t ew_mean_abs_step(const T* y, long long n, double* out, cudaStream_t st);       // out[0] = mean |y[e+1] - y[e]|
+template <typename T> cudaError_t ew_mean_abs_step(const T* y, long long n, double* out, cudaStream_t st);       // out[0] = mean |y[e+1] - y[e]|; out[1..256]: scratch
 template <typename T> cudaError_t ew_dr_first(const T* Y, const T* t, T* U, T* D, long long n, cudaStream_t st);  // D = t - t ; U = Y - (2 D - t)
 constexpr int REDUCE_BLOCKS = 1184;    // fixed, not the device's SM count (~9 per SM on a 132-SM H100): partial sums are combined in
                                        // the same fixed order on every GPU (deterministic)

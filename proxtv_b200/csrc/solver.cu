@@ -165,7 +165,7 @@ Engine lane_guard(Engine eng, const T* y, long long n, double lam, cudaStream_t 
     {   // evaluated on every call: the same buffer (the C ABI's own staging area, a caller's frame buffer) holds different data each time
         cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
         if (cudaStreamIsCapturing(st, &cap) != cudaSuccess || cap != cudaStreamCaptureStatusNone) { cudaGetLastError(); return eng; }
-        if (!G.dev && cudaMalloc(&G.dev, sizeof(double)) != cudaSuccess) { cudaGetLastError(); G.dev = nullptr; return ENGINE_CHUNKED; }
+        if (!G.dev && cudaMalloc(&G.dev, 257 * sizeof(double)) != cudaSuccess) { cudaGetLastError(); G.dev = nullptr; return ENGINE_CHUNKED; }
         double step = 0.0;
         const long long ns = n < (1LL << 18) ? n : (1LL << 18);               // the first 256k elements: a few fibers' worth
         if (ew_mean_abs_step<T>(y, ns, G.dev, st) != cudaSuccess ||
