@@ -435,6 +435,44 @@ int proxtv_PD2_TV_batched_record_dev_f32(const float *y, const double *lambdas, 
 int proxtv_PD2_TV_batched_vjp_dev_f32(const int *ns, int nds, int npen, const double *dims, int batch, int maxIters, const void *tape,
                                   const float *gout, float *gY, double *glam, void *stream);
 
+/* Per-item penalties (DESIGN.md section 16.1): the _batched_ entry points above with `lambdas` holding batch x npen doubles, item-major --
+ * item b's penalties in dims order at lambdas + b npen, as given (PD_TV applies its factor npen to a copy of each row; lambdas is never
+ * written).  Item b is solved as the single-item call with its own row solves it: under the seq and chunked engines its x and info row
+ * equal proxtv_PD*_TV_dev_* on that item with that row (into an aligned buffer) bit for bit; under auto / lane the engine is picked for
+ * the whole batch (the lane guard looks at the largest penalty of the table).  A pass whose running items all have the same penalty for
+ * its term runs the kernels of the shared-row call, so equal rows give the _batched_ call's result and info bit for bit on every engine.
+ * The record form writes an ordinary batched tape (same size, same format): proxtv_PD*_TV_batched_vjp_dev_* reads it, and its glam rows
+ * are the gradients of each item's own penalties as given.  Refusals: those of the _batched_ counterpart in the same order, plus lambdas
+ * == NULL; the record form refuses a negative penalty anywhere in the table. */
+int proxtv_PD_TV_batched_items_dev_f64(const double *y, const double *lambdas, const double *dims, double *x, double *info, const int *ns,
+                                       int nds, int npen, int batch, int maxIters, void *stream);
+int proxtv_PD_TV_batched_items_f64(const double *y, const double *lambdas, const double *dims, double *x, double *info, const int *ns, int nds,
+                                   int npen, int batch, int maxIters);                 /* host pointers */
+int proxtv_PD_TV_batched_items_record_dev_f64(const double *y, const double *lambdas, const double *dims, double *x, double *info,
+                                              const int *ns, int nds, int npen, int batch, int maxIters, void *tape, size_t tape_bytes,
+                                              void *stream);
+int proxtv_PD_TV_batched_items_dev_f32(const float *y, const double *lambdas, const double *dims, float *x, double *info, const int *ns,
+                                       int nds, int npen, int batch, int maxIters, void *stream);
+int proxtv_PD_TV_batched_items_f32(const float *y, const double *lambdas, const double *dims, float *x, double *info, const int *ns, int nds,
+                                   int npen, int batch, int maxIters);                 /* host pointers */
+int proxtv_PD_TV_batched_items_record_dev_f32(const float *y, const double *lambdas, const double *dims, float *x, double *info,
+                                              const int *ns, int nds, int npen, int batch, int maxIters, void *tape, size_t tape_bytes,
+                                              void *stream);
+int proxtv_PD2_TV_batched_items_dev_f64(const double *y, const double *lambdas, const double *dims, double *x, double *info, const int *ns,
+                                        int nds, int npen, int batch, int maxIters, void *stream);
+int proxtv_PD2_TV_batched_items_f64(const double *y, const double *lambdas, const double *dims, double *x, double *info, const int *ns, int nds,
+                                    int npen, int batch, int maxIters);                /* host pointers */
+int proxtv_PD2_TV_batched_items_record_dev_f64(const double *y, const double *lambdas, const double *dims, double *x, double *info,
+                                               const int *ns, int nds, int npen, int batch, int maxIters, void *tape, size_t tape_bytes,
+                                               void *stream);
+int proxtv_PD2_TV_batched_items_dev_f32(const float *y, const double *lambdas, const double *dims, float *x, double *info, const int *ns,
+                                        int nds, int npen, int batch, int maxIters, void *stream);
+int proxtv_PD2_TV_batched_items_f32(const float *y, const double *lambdas, const double *dims, float *x, double *info, const int *ns, int nds,
+                                    int npen, int batch, int maxIters);                /* host pointers */
+int proxtv_PD2_TV_batched_items_record_dev_f32(const float *y, const double *lambdas, const double *dims, float *x, double *info,
+                                               const int *ns, int nds, int npen, int batch, int maxIters, void *tape, size_t tape_bytes,
+                                               void *stream);
+
 /* Launch accounting and optional CUDA-event timing per kernel class (0: prox over contiguous fibers, 1: prox over strided
  * fibers, 2: elementwise/reduction helpers).  Launch counters always run; event timing only while enabled.  read():
  * arrays of 3; ms = summed event time, launches = kernels launched, spans = timed brackets; synchronises the events. */
@@ -463,6 +501,22 @@ int proxtv_lane_prox_dev_f64(int op, const double *A, const double *B, const dou
                              long long inc, double lam, void *stream);
 int proxtv_lane_prox_dev_f32(int op, const float *A, const float *B, const float *C, float *X, long long nf, int len,
                              long long inc, float lam, void *stream);
+/* The batched 1D prox above (plain, unweighted) with one penalty per group of fpi fibers: fiber j's penalty is lamf[j / fpi], lamf a
+ * device array of nf / fpi values.  Honours proxtv_set_engine; every fiber's result equals, bit for bit, the uniform pass with its own
+ * penalty on the kernel family that ran it (seq and chunked: the reference's linearized taut string; lane: the slope-form scan).  The
+ * lane engine takes a table only when every entry is > 0 (the call reads the table back once to know, and to give auto's lane guard
+ * its largest entry); a table with a zero runs on the chunked kernels.  Refused without writing anything: fpi < 1, nf not a multiple
+ * of fpi, lamf NULL, nf < 0, len < 0, inc < 1.  The tape form: proxtv_fiber_tape_dev_* with fiber j's penalty lamf[j / fpi] (an edge
+ * is fused only where its fiber's penalty is > 0), bit for bit the uniform tape of each fiber with its own penalty; refusals of
+ * proxtv_fiber_tape_dev_* (lamf in place of the penalty), then fpi < 1, nf not a multiple of fpi, fpi not a multiple of inc. */
+int proxtv_prox_fibers_lamf_dev_f64(const double *in, double *out, long long nf, int len, long long inc, const double *lamf, long long fpi,
+                                    void *stream);
+int proxtv_prox_fibers_lamf_dev_f32(const float *in, float *out, long long nf, int len, long long inc, const float *lamf, long long fpi,
+                                    void *stream);
+int proxtv_fiber_tape_lamf_dev_f64(const double *y, long long nf, int len, long long inc, const double *lamf, long long fpi, unsigned *F,
+                                   unsigned *U, void *stream);
+int proxtv_fiber_tape_lamf_dev_f32(const float *y, long long nf, int len, long long inc, const float *lamf, long long fpi, unsigned *F,
+                                   unsigned *U, void *stream);
 /* same with a second result array (the ops that write two results: 3 = first half of a Douglas-Rachford iteration, transposed) */
 int proxtv_lane_prox2_dev_f64(int op, const double *A, const double *B, const double *C, double *X, double *X2, long long nf, int len,
                               long long inc, double lam, void *stream);

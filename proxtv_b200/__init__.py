@@ -722,37 +722,51 @@ def _ws_floats(ws):
     return [float(v) for v in np.asarray(ws, dtype=np.float64).ravel()], None
 
 
-def _nd_torch(solver, owner, x, lam, ws_t, ds, max_iters, batched=False):
+def _ws_rows(ws):
+    """ws as a float64 (rows, terms) ndarray when it has two dimensions (a nested list, an ndarray or a tensor: one row of penalties
+    per item), else None; ws is not written."""
+    if _is_torch(ws):
+        import torch
+        return ws.detach().to(device="cpu", dtype=torch.float64).numpy() if ws.dim() == 2 else None
+    a = np.asarray(ws, dtype=np.float64)
+    return a if a.ndim == 2 else None
+
+
+def _nd_torch(solver, owner, x, lam, ws_t, ds, max_iters, batched=False, items=False):
     """The torch path of tvgen_pdr, tvgen, tv1_2d(method='pd') and (batched) tvgen_batched; recorded by the Function when grad mode is
     on and x, or the penalty tensor ws_t, requires grad.  lam: the penalties as floats; ws_t: None, a 1-D tensor of them, or a 0-dim
-    tensor shared by every term.  Nothing the caller passed is written: the solve gets a float64 copy of lam, which PDR_TV and PD_TV
+    tensor shared by every term.  items (batched): lam holds one row of len(ds) penalties per item, item-major, and ws_t is None or
+    the (B, len(ds)) tensor of them.  Nothing the caller passed is written: the solve gets a float64 copy of lam, which PDR_TV and PD_TV
     scale in place.  Sets owner.last_info."""
     import torch
-    assert len(lam) == len(ds)
-    assert ws_t is None or tuple(ws_t.shape) in ((), (len(lam),)), "ws must be one penalty per term, or one 0-dim penalty for all"
+    rows = int(x.shape[0]) if items else 1
+    assert len(lam) == rows * len(ds)
+    assert ws_t is None or tuple(ws_t.shape) in (((rows, len(ds)),) if items else ((), (len(lam),))), \
+        "ws must be one penalty per term, or one 0-dim penalty for all"
     ns, dims, xin = _nd_layout(x, ds, batched)
     batch = int(x.shape[0]) if batched else 0
     if batched and batch == 0:
         owner.last_info = np.zeros((0, _N_INFO))
         return torch.empty_like(x)
     args = (solver, np.array(ns, dtype=np.int32), np.array(dims, dtype=np.float64), np.array(lam, dtype=np.float64), int(max_iters),
-            owner, batch)
+            owner, batch, items)
     if _needs_grad(x, ws_t):
         return _autograd().ND.apply(xin, ws_t, *args)
     return _nd_solve(xin, *args)[0]
 
 
-def _nd_solve(xin, solver, nsa, dsa, lama, max_iters, owner, batch=0, tape=None):
+def _nd_solve(xin, solver, nsa, dsa, lama, max_iters, owner, batch=0, items=False, tape=None):
     """proxtv_<solver>_dev_* (solver: "PDR_TV", "PD_TV" or "PD2_TV") on xin, column-major over nsa (see _nd_layout), or given a tape
     (a uint8 CUDA tensor, proxtv_<solver>_tape_bytes() long) proxtv_<solver>_record_dev_*, the same solve recording every prox pass's
     segmentation.  batch >= 1 (PD_TV / PD2_TV): xin holds `batch` items over nsa back to back, solved by proxtv_<solver>_batched_dev_* /
-    _batched_record_dev_*, and info is (batch, 3).  Sets owner.last_info; returns (result in xin's layout, info)."""
+    _batched_record_dev_* (items: lama holds one row per item, proxtv_<solver>_batched_items_*), and info is (batch, 3).  Sets
+    owner.last_info; returns (result in xin's layout, info)."""
     import torch
     out = torch.empty_strided(xin.shape, xin.stride(), dtype=xin.dtype, device=xin.device)
     info = np.zeros(_N_INFO * max(batch, 1))
     bat = (batch,) if batch else ()
-    kind = "_batched" if batch else ""
-    args = (xin, lama, dsa, out, info, nsa, len(nsa), len(lama)) + bat + (max_iters,)
+    kind = ("_batched_items" if items else "_batched") if batch else ""
+    args = (xin, lama, dsa, out, info, nsa, len(nsa), len(dsa)) + bat + (max_iters,)
     if tape is None:
         _dev_call(solver + kind + "_dev", xin, *args, info=info)
     else:
@@ -768,8 +782,12 @@ def tvgen_batched(x, ws, ds, ps, max_iters=0):
     ps, max_iters=max_iters)`` would solve it, with its own stop test.
 
     ``ds`` are 1-based axes of an item (1..len(s)); two terms go to PD2_TV and any other count to PD_TV, as in ``tvgen``; p = 1 terms
-    only (anything else raises NotImplementedError).  ``ws`` is shared by every item -- a list, an ndarray or a 1-D tensor -- and is
-    never written (``tvgen``'s in-place scaling of a float64 ndarray is not carried over).
+    only (anything else raises NotImplementedError).  ``ws`` is never written (``tvgen``'s in-place scaling of a float64 ndarray is not
+    carried over) and is either shared by every item -- a list, an ndarray, a 1-D tensor or a 0-dim tensor, whatever B is -- or holds
+    one row of penalties per item: a nested list, a 2-D ndarray or a 2-D tensor of shape (B, len(ds)), row b item b's penalties in
+    ``ds`` order, so that item b is solved as ``tvgen(x[b], ws[b], ds, ps, max_iters=max_iters)`` would solve it
+    (``proxtv_PD*_TV_batched_items_*``, DESIGN.md section 16.1).  Any other shape raises AssertionError before any device work.  Rows
+    that are all equal give the shared call's result bit for bit.
     Per-item stop rule: item b iterates while mean|x_b - x_b,last| > 1e-6 and it < ``max_iters`` (0: 35) -- PD2_TV with one term runs
     one iteration -- so an item's result does not depend on the rest of the batch, and an item that has stopped costs no more prox
     work.  ``tvgen_batched.last_info`` is a (B, 3) array, row b = [K_b, stop_b, RC_b] as ``tvgen.last_info`` gives it for that item.
@@ -785,17 +803,27 @@ def tvgen_batched(x, ws, ds, ps, max_iters=0):
     the batch axis slowest; anything else is made C-contiguous; the result has the solved tensor's layout.  Differentiable with
     respect to x and a ``ws`` tensor: the forward records the segmentation tape of every prox pass and each item's K, and the backward
     is, for every item, the exact vector-Jacobian product of the K_b iterations that item ran (``proxtv_PD*_TV_batched_vjp_dev_*``,
-    DESIGN.md section 16); the ``ws`` gradient is the per-item penalty gradients summed in float64.  K_b has no derivative: where a
+    DESIGN.md section 16); the gradient of a shared ``ws`` tensor is the per-item penalty gradients summed in float64, that of a
+    (B, len(ds)) one is row b = item b's penalty gradients (an expanded ``w.expand(B, npen)`` thus gives ``w`` their sum through
+    autograd), each cast to the tensor's dtype and device.  K_b has no derivative: where a
     perturbation changes it the map jumps.  The tape is allocated for ``max_iters`` iterations of the whole batch, B times the single
     capacity: PD_TV with 3 terms at 35 iterations takes about 1.64 GiB per 512 x 512 x 256 item.  Double backward is not supported.
     """
-    _nd_checks(ws, ds, ps, max_iters)
+    rows = _ws_rows(ws)
+    if rows is None:
+        _nd_checks(ws, ds, ps, max_iters)
+        lam, ws_t = _ws_floats(ws)
+        assert ws_t is None or tuple(ws_t.shape) in ((), (len(lam),)), "ws must be one penalty per term, or one 0-dim penalty for all"
+    else:
+        assert len(ds) == len(ps) and max_iters >= 0
+        assert len(np.shape(x)) >= 2 and rows.shape == (int(np.shape(x)[0]), len(ds)), \
+            "a 2-D ws must be (B, len(ds)): one row of penalties per item"
+        lam, ws_t = [float(v) for v in rows.ravel()], (ws if _is_torch(ws) else None)
     _p1(ps)
-    lam, ws_t = _ws_floats(ws)
-    assert ws_t is None or tuple(ws_t.shape) in ((), (len(lam),)), "ws must be one penalty per term, or one 0-dim penalty for all"
-    solver = _nd_solver(len(lam))
+    items = rows is not None
+    solver = _nd_solver(len(ds))
     if _is_torch(x):
-        return _nd_torch(solver, tvgen_batched, x, lam, ws_t, ds, max_iters, batched=True)
+        return _nd_torch(solver, tvgen_batched, x, lam, ws_t, ds, max_iters, batched=True, items=items)
     x = np.asarray(x)
     f32 = x.dtype == np.float32
     assert x.ndim >= 2
@@ -809,8 +837,8 @@ def tvgen_batched(x, ws, ds, ps, max_iters=0):
     info = np.zeros(_N_INFO * B)
     ns = np.array(x.shape[1:], dtype=np.int32)
     lama = np.array(lam, dtype=np.float64)
-    _host_call(solver + "_batched", xt, xt, lama, np.array(ds, dtype=np.float64), out, info, ns, len(ns), len(lama), B, int(max_iters),
-               info=info)
+    _host_call(solver + ("_batched_items" if items else "_batched"), xt, xt, lama, np.array(ds, dtype=np.float64), out, info, ns, len(ns),
+               len(ds), B, int(max_iters), info=info)
     tvgen_batched.last_info = info.reshape(B, _N_INFO)
     return np.transpose(out, rev)
 
@@ -924,24 +952,25 @@ def _autograd():
             return (gY if need_x else None), None, None, None, g_w, None, None
 
     class ND(torch.autograd.Function):
-        """apply(xin, ws_t, solver, nsa, dsa, lama, max_iters, owner, batch) of _nd_solve; ctx also keeps the iteration count the solve
-        ran (the Dykstra solvers' stop rule picks it; batch >= 1: each item's K).  backward: proxtv_<solver>_vjp_dev_*; the gradient of
-        ws_t is npen * glam for PDR_TV and PD_TV (glam: the gradients of the scaled penalties), glam for PD2_TV.  batch >= 1:
-        proxtv_<solver>_batched_vjp_dev_*, whose per-item glam is of the penalties as given for both solvers, summed over the items."""
+        """apply(xin, ws_t, solver, nsa, dsa, lama, max_iters, owner, batch, items) of _nd_solve; ctx also keeps the iteration count the
+        solve ran (the Dykstra solvers' stop rule picks it; batch >= 1: each item's K).  backward: proxtv_<solver>_vjp_dev_*; the gradient
+        of ws_t is npen * glam for PDR_TV and PD_TV (glam: the gradients of the scaled penalties), glam for PD2_TV.  batch >= 1:
+        proxtv_<solver>_batched_vjp_dev_*, whose per-item glam is of the penalties as given for both solvers: summed over the items for a
+        shared ws_t, the (batch, npen) rows themselves for a per-item one (items)."""
         @staticmethod
-        def forward(ctx, xin, ws_t, solver, nsa, dsa, lama, max_iters, owner, batch):
+        def forward(ctx, xin, ws_t, solver, nsa, dsa, lama, max_iters, owner, batch, items=False):
             lib = require_device()
             if batch:
                 tape_bytes = getattr(lib, "proxtv_%s_batched_tape_bytes" % solver)
-                nb = int(tape_bytes(_ptr(nsa), len(nsa), len(lama), batch, max_iters))
+                nb = int(tape_bytes(_ptr(nsa), len(nsa), len(dsa), batch, max_iters))
             else:
                 tape_bytes = getattr(lib, "proxtv_%s_tape_bytes" % solver)
-                nb = int(tape_bytes(_ptr(nsa), len(nsa), len(lama), max_iters))  # 0: too large; the record call refuses it
+                nb = int(tape_bytes(_ptr(nsa), len(nsa), len(dsa), max_iters))  # 0: too large; the record call refuses it
             tape = torch.empty(max(nb, 256), dtype=torch.uint8, device=xin.device)
-            out, info = _nd_solve(xin, solver, nsa, dsa, lama, max_iters, owner, batch, tape)
+            out, info = _nd_solve(xin, solver, nsa, dsa, lama, max_iters, owner, batch, items, tape)
             ctx.save_for_backward(tape)
             iters = info[:, 0].astype(np.int64) if batch else int(info[0])
-            ctx.geom, ctx.layout = (solver, nsa, dsa, max_iters, iters, batch), (out.shape, out.stride(), out.dtype)
+            ctx.geom, ctx.layout = (solver, nsa, dsa, max_iters, iters, batch, items), (out.shape, out.stride(), out.dtype)
             ctx.ws_like = (ws_t.dtype, ws_t.device, ws_t.shape) if ws_t is not None else None
             return out
 
@@ -949,7 +978,7 @@ def _autograd():
         @once_differentiable
         def backward(ctx, gout):
             (tape,) = ctx.saved_tensors
-            solver, nsa, dsa, max_iters, iters, batch = ctx.geom
+            solver, nsa, dsa, max_iters, iters, batch, items = ctx.geom
             shape, stride, dt = ctx.layout
             need_x, need_ws = ctx.needs_input_grad[:2]
             npen = len(dsa)
@@ -960,7 +989,10 @@ def _autograd():
             rest = (None,) * (len(ctx.needs_input_grad) - 2)
             if batch:
                 _dev_call(solver + "_batched_vjp_dev", g, nsa, len(nsa), npen, dsa, batch, max_iters, tape, g, gY, glam)
-                g_ws = _penalty_grad(glam.view(batch, npen).sum(0, dtype=torch.float64), ctx.ws_like) if need_ws else None
+                g_ws = None
+                if need_ws:
+                    per_item = glam.view(batch, npen)
+                    g_ws = _penalty_grad(per_item if items else per_item.sum(0, dtype=torch.float64), ctx.ws_like)
                 return (gY if need_x else None), g_ws, *rest
             it = () if solver == "PDR_TV" else (iters,)                               # PDR_TV runs exactly max_iters iterations
             _dev_call(solver + "_vjp_dev", g, nsa, len(nsa), npen, dsa, max_iters, *it, tape, g, gY, glam)

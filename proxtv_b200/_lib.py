@@ -145,10 +145,30 @@ SIGNATURES = {
     "proxtv_PD2_TV_batched_record_dev_f32": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp, C.c_size_t,
                                                      _vp]),
     "proxtv_PD2_TV_batched_vjp_dev_f32": (C.c_int, [_vp, C.c_int, C.c_int, _vp, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp]),
+    "proxtv_PD_TV_batched_items_dev_f64": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp]),
+    "proxtv_PD_TV_batched_items_f64": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "proxtv_PD_TV_batched_items_record_dev_f64": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp,
+                                                          C.c_size_t, _vp]),
+    "proxtv_PD_TV_batched_items_dev_f32": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp]),
+    "proxtv_PD_TV_batched_items_f32": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "proxtv_PD_TV_batched_items_record_dev_f32": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp,
+                                                          C.c_size_t, _vp]),
+    "proxtv_PD2_TV_batched_items_dev_f64": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp]),
+    "proxtv_PD2_TV_batched_items_f64": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "proxtv_PD2_TV_batched_items_record_dev_f64": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp,
+                                                          C.c_size_t, _vp]),
+    "proxtv_PD2_TV_batched_items_dev_f32": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp]),
+    "proxtv_PD2_TV_batched_items_f32": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "proxtv_PD2_TV_batched_items_record_dev_f32": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp,
+                                                          C.c_size_t, _vp]),
     "proxtv_PDR_TV_dev_f64": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, _vp]),
     "proxtv_PDR_TV_dev_f32": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, _vp]),
     "proxtv_lane_prox_dev_f64": (C.c_int, [C.c_int, _vp, _vp, _vp, _vp, C.c_longlong, C.c_int, C.c_longlong, C.c_double, _vp]),
     "proxtv_lane_prox_dev_f32": (C.c_int, [C.c_int, _vp, _vp, _vp, _vp, C.c_longlong, C.c_int, C.c_longlong, C.c_float, _vp]),
+    "proxtv_prox_fibers_lamf_dev_f64": (C.c_int, [_vp, _vp, C.c_longlong, C.c_int, C.c_longlong, _vp, C.c_longlong, _vp]),
+    "proxtv_prox_fibers_lamf_dev_f32": (C.c_int, [_vp, _vp, C.c_longlong, C.c_int, C.c_longlong, _vp, C.c_longlong, _vp]),
+    "proxtv_fiber_tape_lamf_dev_f64": (C.c_int, [_vp, C.c_longlong, C.c_int, C.c_longlong, _vp, C.c_longlong, _vp, _vp, _vp]),
+    "proxtv_fiber_tape_lamf_dev_f32": (C.c_int, [_vp, C.c_longlong, C.c_int, C.c_longlong, _vp, C.c_longlong, _vp, _vp, _vp]),
     "proxtv_lane_prox2_dev_f64": (C.c_int, [C.c_int, _vp, _vp, _vp, _vp, _vp, C.c_longlong, C.c_int, C.c_longlong, C.c_double, _vp]),
     "proxtv_lane_tuning": (None, [C.c_int, C.c_int, C.c_int]),
     "proxtv_lane_stats": (C.c_ulonglong, [C.c_int]),

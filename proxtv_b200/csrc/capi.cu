@@ -324,6 +324,43 @@ static int dev_vjp(const char* fn, const T* y, const T* g, T* gx, T* gw, long lo
     return no.cuda_ok(ptvv::vjp_fibers<T>(y, g, gx, gw, nf, len, inc, lam, lamv, scr, (cudaStream_t)stream));
 }
 
+// The batched 1D prox with fiber j's penalty lamf[j / fpi] (device table); refused calls write nothing.
+template <typename T>
+static int dev_prox_fibers_lamf(const char* fn, const T* in, T* out, long long nf, int len, long long inc, const T* lamf, long long fpi,
+                                void* stream) {
+    const Refuse no{fn};
+    if (fpi < 1 || nf % fpi != 0) return no("invalid penalty groups (need fpi >= 1 and nf a multiple of fpi)");
+    if (!lamf) return no("NULL array");
+    if (nf < 0 || len < 0 || inc < 1) return no("invalid fiber geometry (need nf >= 0, len >= 0, inc >= 1)");
+    if (!no.have_device()) return 0;
+    const cudaStream_t st = (cudaStream_t)stream;
+    WsGuard guard(st);
+    const long long se = nf <= 0 || len <= 0 || inc == 1 ? 0 : strided_scratch_elems(nf, len);
+    T* scr = se ? (T*)ws_get(al((size_t)se * sizeof(T))) : nullptr;
+    // the table's largest entry for the lane guard, and whether every entry is > 0 (the lane engine's condition): one read-back
+    std::vector<T> tab(nf > 0 ? (size_t)(nf / fpi) : 0);
+    if (!tab.empty() && !(no.cuda_ok(cudaMemcpyAsync(tab.data(), lamf, tab.size() * sizeof(T), cudaMemcpyDeviceToHost, st)) &&
+                          no.cuda_ok(cudaStreamSynchronize(st)))) return 0;
+    bool pos = true; double lmax = 0.0;
+    for (T v : tab) { pos = pos && v > T(0); if ((double)v > lmax) lmax = (double)v; }
+    const Engine eng = (nf >= 1024 && len >= 64) ? lane_guard<T>((Engine)g_engine, in, nf * (long long)len, lmax, st) : (Engine)g_engine;
+    return no.cuda_ok(prox_fibers_lamf<T>(in, nullptr, IN_A, out, FiberGeom{nf, len, inc}, lamf, fpi, pos, eng, scr, st, se));
+}
+
+// The segmentation tape with fiber j's penalty lamf[j / fpi]; the refusals of dev_tape, then the groups (fpi >= 1, nf a multiple of fpi,
+// fpi a multiple of inc: every group is whole slabs).
+template <typename T>
+static int dev_tape_lamf(const char* fn, const T* y, long long nf, int len, long long inc, const T* lamf, long long fpi, uint32_t* F,
+                         uint32_t* U, void* stream) {
+    const Refuse no{fn};
+    if (nf < 0 || len < 0 || inc < 1 || nf % inc != 0) return no("invalid fiber geometry (need nf >= 0, len >= 0, inc >= 1, nf a multiple of inc)");
+    if (!y || !F || !U || !lamf) return no("NULL array");
+    if (fpi < 1 || nf % fpi != 0 || fpi % inc != 0) return no("invalid penalty groups (need fpi >= 1, nf a multiple of fpi, fpi a multiple of inc)");
+    if (!no.have_device()) return 0;
+    WsGuard guard((cudaStream_t)stream);
+    return no.cuda_ok(ptvv::fiber_tape_lamf<T>(y, nf, len, inc, lamf, fpi, F, U, (cudaStream_t)stream));
+}
+
 // Segmentation tape of y over the fibers (nf, len, inc) (nf a multiple of inc); refused calls write nothing.
 template <typename T>
 static int dev_tape(const char* fn, const T* y, long long nf, int len, long long inc, T lam, const T* lamv, uint32_t* F, uint32_t* U,
@@ -481,12 +518,13 @@ static int dev_nd_vjp(const char* fn, NdSolver s, const int* ns, int nds, int np
 
 // ---- batched PD_TV / PD2_TV (DESIGN.md section 16): `batch` items of prod(ns) elements back to back, each with its own stop rule ----
 // Every refusal writes info[3 b + RC] = RC_ERROR for every item and nothing else; lambdas are never written (PD_TV's factor npen is
-// applied to a copy).
+// applied to a copy).  items: lambdas holds one row of npen penalties per item, item-major (section 16.1), else one row for all.
 
 // The solve (host_io: y and x are host arrays) or, given a tape, the recorded solve and then the tape's header and K table.
 template <typename T>
 static int run_pd_batched(const char* fn, NdSolver s, bool host_io, bool record, const T* y, const double* lambdas, const double* dims, T* x, double* info,
-                          const int* ns, int nds, int npen, int batch, int maxIters, void* tape, size_t tape_bytes, cudaStream_t st) {
+                          const int* ns, int nds, int npen, int batch, int maxIters, void* tape, size_t tape_bytes, cudaStream_t st,
+                          bool items = false) {
     static const char* const too_small[2] = {"tape_bytes smaller than proxtv_PD2_TV_batched_tape_bytes()",
                                              "tape_bytes smaller than proxtv_PD_TV_batched_tape_bytes()"};
     const Refuse no{fn, info, batch};
@@ -495,7 +533,7 @@ static int run_pd_batched(const char* fn, NdSolver s, bool host_io, bool record,
         if (!y || !x || !lambdas || !dims || !ns || !tape) return no("NULL array");
         if (batch < 1) return no("invalid batch (need batch >= 1)");
         if (const char* why = nd_args_check(s, ns, nds, npen, dims, &t)) return no(why);
-        for (int i = 0; i < npen; i++) if (!(lambdas[i] >= 0)) return no("negative penalty");
+        for (long long i = 0; i < (long long)npen * (items ? batch : 1); i++) if (!(lambdas[i] >= 0)) return no("negative penalty");
         const size_t need = nd_tape_bytes(s, ns, nds, npen, maxIters, batch);
         if (need == 0) return no("tape size does not fit in size_t (maxIters too large)");
         if (tape_bytes < need) return no(too_small[s]);
@@ -508,11 +546,14 @@ static int run_pd_batched(const char* fn, NdSolver s, bool host_io, bool record,
         if (s == ND_PD2 && npen > 2) return no("this algorithm can not work with more than 2 penalties");
         if (s == ND_PD2 && npen < 1) return no("invalid penalty dimensions");
         if (const char* why = nd_terms(ns, nds, npen, dims, &t)) return no(why);
+        if (items && !lambdas) return no("NULL array");
     }
     const long long n = t.n;
     WsGuard guard(st);
-    std::vector<double> lam(lambdas ? lambdas : nullptr, lambdas ? lambdas + (npen > 0 ? npen : 0) : nullptr);
-    scale_penalties(s, lam.data(), npen);
+    const int rows = items ? batch : 1;
+    std::vector<double> lam(lambdas ? lambdas : nullptr, lambdas ? lambdas + (npen > 0 ? (size_t)npen * rows : 0) : nullptr);
+    for (int b = 0; b < rows && npen > 0; b++) scale_penalties(s, lam.data() + (size_t)b * npen, npen);
+    const int lstride = items ? npen : 0;
     void* ws = ws_get(ws_bytes_pd<T>(n, npen, batch));
     if (!ws) return no("out of memory");
     std::vector<double> linfo(3 * (size_t)batch);      // the tape's K table needs the rows even when the caller passes no info
@@ -523,8 +564,8 @@ static int run_pd_batched(const char* fn, NdSolver s, bool host_io, bool record,
         io.in(y, nt); io.out(x, nt);
         if (!io.stage()) return 0;
     }
-    const int ok = s == ND_PD2 ? pd2_device<T>(y, lam.data(), dims, x, pinfo, ns, nds, npen, maxIters, ws, (Engine)g_engine, st, tape, batch)
-                               : pd_device<T>(y, lam.data(), dims, x, pinfo, ns, nds, npen, maxIters, ws, (Engine)g_engine, st, tape, batch);
+    const int ok = s == ND_PD2 ? pd2_device<T>(y, lam.data(), dims, x, pinfo, ns, nds, npen, maxIters, ws, (Engine)g_engine, st, tape, batch, lstride)
+                               : pd_device<T>(y, lam.data(), dims, x, pinfo, ns, nds, npen, maxIters, ws, (Engine)g_engine, st, tape, batch, lstride);
     if (!ok) return no("device solver failed");
     if (record && !no.cuda_ok(nd_tape_header_batched(s, tape, sizeof(T), ns, nds, npen, dims, maxIters, batch, pinfo, st))) return 0;
     return io.finish() ? 1 : 0;
@@ -957,5 +998,65 @@ int proxtv_PD2_TV_batched_vjp_dev_f32(const int* ns, int nds, int npen, const do
     return dev_nd_vjp_batched<float>("proxtv_PD2_TV_batched_vjp_dev_f32", ND_PD2, ns, nds, npen, dims, batch, maxIters, tape, gout, gY, glam, stream); }
 size_t proxtv_PD2_TV_batched_tape_bytes(const int* ns, int nds, int npen, int batch, int maxIters) {
     return nd_tape_bytes_batched(ND_PD2, ns, nds, npen, batch, maxIters); }
+
+// ---- per-item penalties (DESIGN.md section 16.1) ----
+int proxtv_PD_TV_batched_items_dev_f64(const double* y, const double* lambdas, const double* dims, double* x, double* info, const int* ns,
+                                     int nds, int npen, int batch, int maxIters, void* stream) {
+    return run_pd_batched<double>("proxtv_PD_TV_batched_items_dev_f64", ND_PD, false, false, y, lambdas, dims, x, info, ns, nds, npen, batch, maxIters,
+                                nullptr, 0, (cudaStream_t)stream, true); }
+int proxtv_PD_TV_batched_items_f64(const double* y, const double* lambdas, const double* dims, double* x, double* info, const int* ns, int nds,
+                                 int npen, int batch, int maxIters) {
+    return run_pd_batched<double>("proxtv_PD_TV_batched_items_f64", ND_PD, true, false, y, lambdas, dims, x, info, ns, nds, npen, batch, maxIters,
+                                nullptr, 0, 0, true); }
+int proxtv_PD_TV_batched_items_record_dev_f64(const double* y, const double* lambdas, const double* dims, double* x, double* info, const int* ns,
+                                            int nds, int npen, int batch, int maxIters, void* tape, size_t tape_bytes, void* stream) {
+    return run_pd_batched<double>("proxtv_PD_TV_batched_items_record_dev_f64", ND_PD, false, true, y, lambdas, dims, x, info, ns, nds, npen, batch,
+                                maxIters, tape, tape_bytes, (cudaStream_t)stream, true); }
+int proxtv_PD_TV_batched_items_dev_f32(const float* y, const double* lambdas, const double* dims, float* x, double* info, const int* ns,
+                                     int nds, int npen, int batch, int maxIters, void* stream) {
+    return run_pd_batched<float>("proxtv_PD_TV_batched_items_dev_f32", ND_PD, false, false, y, lambdas, dims, x, info, ns, nds, npen, batch, maxIters,
+                                nullptr, 0, (cudaStream_t)stream, true); }
+int proxtv_PD_TV_batched_items_f32(const float* y, const double* lambdas, const double* dims, float* x, double* info, const int* ns, int nds,
+                                 int npen, int batch, int maxIters) {
+    return run_pd_batched<float>("proxtv_PD_TV_batched_items_f32", ND_PD, true, false, y, lambdas, dims, x, info, ns, nds, npen, batch, maxIters,
+                                nullptr, 0, 0, true); }
+int proxtv_PD_TV_batched_items_record_dev_f32(const float* y, const double* lambdas, const double* dims, float* x, double* info, const int* ns,
+                                            int nds, int npen, int batch, int maxIters, void* tape, size_t tape_bytes, void* stream) {
+    return run_pd_batched<float>("proxtv_PD_TV_batched_items_record_dev_f32", ND_PD, false, true, y, lambdas, dims, x, info, ns, nds, npen, batch,
+                                maxIters, tape, tape_bytes, (cudaStream_t)stream, true); }
+int proxtv_PD2_TV_batched_items_dev_f64(const double* y, const double* lambdas, const double* dims, double* x, double* info, const int* ns,
+                                     int nds, int npen, int batch, int maxIters, void* stream) {
+    return run_pd_batched<double>("proxtv_PD2_TV_batched_items_dev_f64", ND_PD2, false, false, y, lambdas, dims, x, info, ns, nds, npen, batch, maxIters,
+                                nullptr, 0, (cudaStream_t)stream, true); }
+int proxtv_PD2_TV_batched_items_f64(const double* y, const double* lambdas, const double* dims, double* x, double* info, const int* ns, int nds,
+                                 int npen, int batch, int maxIters) {
+    return run_pd_batched<double>("proxtv_PD2_TV_batched_items_f64", ND_PD2, true, false, y, lambdas, dims, x, info, ns, nds, npen, batch, maxIters,
+                                nullptr, 0, 0, true); }
+int proxtv_PD2_TV_batched_items_record_dev_f64(const double* y, const double* lambdas, const double* dims, double* x, double* info, const int* ns,
+                                            int nds, int npen, int batch, int maxIters, void* tape, size_t tape_bytes, void* stream) {
+    return run_pd_batched<double>("proxtv_PD2_TV_batched_items_record_dev_f64", ND_PD2, false, true, y, lambdas, dims, x, info, ns, nds, npen, batch,
+                                maxIters, tape, tape_bytes, (cudaStream_t)stream, true); }
+int proxtv_PD2_TV_batched_items_dev_f32(const float* y, const double* lambdas, const double* dims, float* x, double* info, const int* ns,
+                                     int nds, int npen, int batch, int maxIters, void* stream) {
+    return run_pd_batched<float>("proxtv_PD2_TV_batched_items_dev_f32", ND_PD2, false, false, y, lambdas, dims, x, info, ns, nds, npen, batch, maxIters,
+                                nullptr, 0, (cudaStream_t)stream, true); }
+int proxtv_PD2_TV_batched_items_f32(const float* y, const double* lambdas, const double* dims, float* x, double* info, const int* ns, int nds,
+                                 int npen, int batch, int maxIters) {
+    return run_pd_batched<float>("proxtv_PD2_TV_batched_items_f32", ND_PD2, true, false, y, lambdas, dims, x, info, ns, nds, npen, batch, maxIters,
+                                nullptr, 0, 0, true); }
+int proxtv_PD2_TV_batched_items_record_dev_f32(const float* y, const double* lambdas, const double* dims, float* x, double* info, const int* ns,
+                                            int nds, int npen, int batch, int maxIters, void* tape, size_t tape_bytes, void* stream) {
+    return run_pd_batched<float>("proxtv_PD2_TV_batched_items_record_dev_f32", ND_PD2, false, true, y, lambdas, dims, x, info, ns, nds, npen, batch,
+                                maxIters, tape, tape_bytes, (cudaStream_t)stream, true); }
+int proxtv_prox_fibers_lamf_dev_f64(const double* in, double* out, long long nf, int len, long long inc, const double* lamf, long long fpi, void* stream) {
+    return dev_prox_fibers_lamf<double>("proxtv_prox_fibers_lamf_dev_f64", in, out, nf, len, inc, lamf, fpi, stream); }
+int proxtv_fiber_tape_lamf_dev_f64(const double* y, long long nf, int len, long long inc, const double* lamf, long long fpi, unsigned* F, unsigned* U,
+                                   void* stream) {
+    return dev_tape_lamf<double>("proxtv_fiber_tape_lamf_dev_f64", y, nf, len, inc, lamf, fpi, F, U, stream); }
+int proxtv_prox_fibers_lamf_dev_f32(const float* in, float* out, long long nf, int len, long long inc, const float* lamf, long long fpi, void* stream) {
+    return dev_prox_fibers_lamf<float>("proxtv_prox_fibers_lamf_dev_f32", in, out, nf, len, inc, lamf, fpi, stream); }
+int proxtv_fiber_tape_lamf_dev_f32(const float* y, long long nf, int len, long long inc, const float* lamf, long long fpi, unsigned* F, unsigned* U,
+                                   void* stream) {
+    return dev_tape_lamf<float>("proxtv_fiber_tape_lamf_dev_f32", y, nf, len, inc, lamf, fpi, F, U, stream); }
 
 }  // extern "C"

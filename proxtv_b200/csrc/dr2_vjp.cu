@@ -561,9 +561,11 @@ size_t nd_tape_bytes(NdSolver s, const int* ns, int nds, int npen, int maxIters,
     return head + (size_t)(passes * set2);
 }
 
-template <typename T> cudaError_t nd_tape_pass(void* passes, long long cap_n, long long p, const T* y, FiberGeom g, T lam, cudaStream_t st) {
+template <typename T> cudaError_t nd_tape_pass(void* passes, long long cap_n, long long p, const T* y, FiberGeom g, T lam, cudaStream_t st,
+                                               const T* lamf, long long fpi) {
     const size_t sb = ptvv::vjp_tape_set_bytes(cap_n);
     uint32_t* F = (uint32_t*)((char*)passes + (size_t)p * 2 * sb);
+    if (lamf) return ptvv::fiber_tape_lamf<T>(y, g.nf, g.len, g.inc, lamf, fpi, F, F + sb / 4, st);
     return ptvv::fiber_tape<T>(y, g.nf, g.len, g.inc, lam, nullptr, F, F + sb / 4, st);
 }
 template <typename T> cudaError_t pdr_tape_pass(void* tape, long long n, long long p, const T* y, FiberGeom g, T lam, cudaStream_t st) {
@@ -933,7 +935,7 @@ cudaError_t nd_vjp_device(NdSolver s, const NdTerms& t, int npen, int maxIters, 
 
 #define INST(T) \
     template cudaError_t pdr_tape_pass<T>(void*, long long, long long, const T*, FiberGeom, T, cudaStream_t); \
-    template cudaError_t nd_tape_pass<T>(void*, long long, long long, const T*, FiberGeom, T, cudaStream_t); \
+    template cudaError_t nd_tape_pass<T>(void*, long long, long long, const T*, FiberGeom, T, cudaStream_t, const T*, long long); \
     template size_t ws_bytes_nd_vjp<T>(const NdTerms&, int, bool, int); \
     template cudaError_t nd_vjp_device<T>(NdSolver, const NdTerms&, int, int, int, const void*, const T*, T*, double*, void*, cudaStream_t, \
                                           int, const int*); \

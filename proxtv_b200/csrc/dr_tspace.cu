@@ -20,7 +20,8 @@ namespace ptv {
 
 template <typename T>
 cudaError_t prox_fibers_chunked_contig(const T* A, const T* B, const T* C, InOp op, T* X, int out_op, FiberGeom g, T lam,
-                                       const T* lamv, cudaStream_t st, T* X2 = nullptr, long long inc2 = 0);
+                                       const T* lamv, cudaStream_t st, T* X2 = nullptr, long long inc2 = 0,
+                                       const T* lamf = nullptr, long long fpi = 1);
 template <typename T> cudaError_t gather_fibers(const T* A, const T* B, InOp op, T* out, FiberGeom g, cudaStream_t st);
 template <typename T> cudaError_t scatter_fibers(const T* in, T* X, FiberGeom g, cudaStream_t st);
 

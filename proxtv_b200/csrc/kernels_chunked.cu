@@ -113,11 +113,13 @@ __device__ __forceinline__ void fill_batch(int c0, int nwin, int nchunks, int n,
 // CL: how the optional transposed second output X2 is produced.  0: plain 8-byte scattered stores (slow: partial-sector writes make
 // L2 read-modify-write every sector); >= 1: the finished fiber rows of CL consecutive CTAs (a thread-block cluster when CL > 1)
 // are exchanged through (distributed) shared memory so that fpb*CL adjacent fibers are written together as full 32-byte sectors.
-template <typename T, bool WEIGHTED, int MAXT, int CL, int CHT = CH>
+// LAMF: fiber j's penalty is lamf[j / fpi] (one per group of fpi fibers), the uniform scan with that value.
+template <typename T, bool WEIGHTED, int MAXT, int CL, int CHT = CH, bool LAMF = false>
 __global__ void __launch_bounds__(MAXT, MAXT <= 256 ? 2 : 1) k_prox_chunked_contig(const T* __restrict__ A, const T* __restrict__ B, const T* __restrict__ C, int in_op,
                                       T* __restrict__ X, int out_op,
                                       long long nf, int n, T lam, const T* __restrict__ lamv, int lpf, int fpb, int npad, int use_tma,
-                                      T* __restrict__ X2, long long inc2, uint32_t* __restrict__ Mk, T* __restrict__ Cv) {
+                                      T* __restrict__ X2, long long inc2, uint32_t* __restrict__ Mk, T* __restrict__ Cv,
+                                      const T* __restrict__ lamf, long long fpi) {
     __shared__ uint64_t mbar;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     RcpPair<T>* rcp = reinterpret_cast<RcpPair<T>*>(smem_raw);    // reciprocal table        [RCP_N]   (16-byte aligned)
@@ -198,6 +200,7 @@ __global__ void __launch_bounds__(MAXT, MAXT <= 256 ? 2 : 1) k_prox_chunked_cont
 #endif
     };
     if (WEIGHTED) phases(ArrayLam<T, SmemLd32<T>>{SmemLd32<T>{smem_u32(wsm + (size_t)fbc * npad)}});
+    else if (LAMF) phases(UniformLam<T>{lamf[(f0 + fbc) / fpi]});
     else phases(UniformLam<T>{in_register(lam)});
 
     // ---- value of the segment entering each chunk (gathered before any output is written: the store is the output) ----
@@ -269,8 +272,9 @@ __global__ void __launch_bounds__(MAXT, MAXT <= 256 ? 2 : 1) k_prox_chunked_cont
 // Returns cudaErrorInvalidConfiguration if the fibers do not fit in shared memory (caller falls back to the sequential kernel).
 template <typename T>
 static cudaError_t launch_chunked_contig(const T* A, const T* B, const T* C, InOp op, T* X, int out_op, FiberGeom g, T lam,
-                                         const T* lamv, cudaStream_t st, T* X2, long long inc2, uint32_t* Mk, T* Cv) {
-    if (g.inc != 1) return cudaErrorInvalidConfiguration;
+                                         const T* lamv, cudaStream_t st, T* X2, long long inc2, uint32_t* Mk, T* Cv,
+                                         const T* lamf = nullptr, long long fpi = 1) {
+    if (g.inc != 1 || (lamf && (lamv || X2))) return cudaErrorInvalidConfiguration;
     if (g.nf <= 0 || g.len <= 0) return cudaSuccess;
     const int n = g.len;
     // 16-sample chunks for weighted float64 fibers: their second staged row (the weights) limits residency to 3 CTAs of 128
@@ -292,7 +296,8 @@ static cudaError_t launch_chunked_contig(const T* A, const T* B, const T* C, InO
     // TMA staging needs 16-byte aligned rows: aligned base, row pitch a multiple of 16 bytes, single input array
     const int use_tma = (op == IN_A) && (((uintptr_t)A & 15) == 0) && (((size_t)n * sizeof(T)) % 16 == 0);
     constexpr int SECT = 32 / (int)sizeof(T);                 // fibers per 32-byte sector
-    using KernT = void (*)(const T*, const T*, const T*, int, T*, int, long long, int, T, const T*, int, int, int, int, T*, long long, uint32_t*, T*);
+    using KernT = void (*)(const T*, const T*, const T*, int, T*, int, long long, int, T, const T*, int, int, int, int, T*, long long, uint32_t*, T*,
+                           const T*, long long);
     KernT kern; int cl = 0;
     if (X2 && !lamv && threads <= 256 && inc2 > 0) {
         // sector-assembled transposed output: the CTA's own fibers suffice, or a cluster of SECT single-fiber CTAs
@@ -302,6 +307,7 @@ static cudaError_t launch_chunked_contig(const T* A, const T* B, const T* C, InO
     } else {
         // small CTAs (<= 256 threads) get a register budget of up to 128/thread so loop constants stay in registers
         if (half) kern = threads <= 256 ? k_prox_chunked_contig<T, true, 256, 0, 16> : k_prox_chunked_contig<T, true, 1024, 0, 16>;
+        else if (lamf) kern = threads <= 256 ? k_prox_chunked_contig<T, false, 256, 0, CH, true> : k_prox_chunked_contig<T, false, 1024, 0, CH, true>;
         else
         kern = threads <= 256 ? (lamv ? k_prox_chunked_contig<T, true, 256, 0> : k_prox_chunked_contig<T, false, 256, 0>)
                               : (lamv ? k_prox_chunked_contig<T, true, 1024, 0> : k_prox_chunked_contig<T, false, 1024, 0>);
@@ -317,34 +323,34 @@ static cudaError_t launch_chunked_contig(const T* A, const T* B, const T* C, InO
         at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = cl; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
         cfg.attrs = at; cfg.numAttrs = 1;
         const int in_op_i = (int)op; const int use_tma_i = use_tma;
-        uint32_t* mk0 = nullptr; T* cv0 = nullptr;
-        return cudaLaunchKernelEx(&cfg, kern, A, B, C, in_op_i, X, out_op, g.nf, n, lam, lamv, lpf, fpb, npad, use_tma_i, X2, inc2a, mk0, cv0);
+        uint32_t* mk0 = nullptr; T* cv0 = nullptr; const T* lf0 = nullptr; const long long fpi1 = 1;
+        return cudaLaunchKernelEx(&cfg, kern, A, B, C, in_op_i, X, out_op, g.nf, n, lam, lamv, lpf, fpb, npad, use_tma_i, X2, inc2a, mk0, cv0, lf0, fpi1);
     }
-    kern<<<blocks, threads, smem, st>>>(A, B, C, (int)op, X, out_op, g.nf, n, lam, lamv, lpf, fpb, npad, use_tma, X2, inc2a, Mk, Cv);
+    kern<<<blocks, threads, smem, st>>>(A, B, C, (int)op, X, out_op, g.nf, n, lam, lamv, lpf, fpb, npad, use_tma, X2, inc2a, Mk, Cv, lamf, fpi);
     return cudaGetLastError();
 }
 
 template <typename T>
 cudaError_t prox_fibers_chunked_contig(const T* A, const T* B, const T* C, InOp op, T* X, int out_op, FiberGeom g, T lam,
-                                       const T* lamv, cudaStream_t st, T* X2, long long inc2) {
-    return launch_chunked_contig<T>(A, B, C, op, X, out_op, g, lam, lamv, st, X2, inc2, nullptr, nullptr);
+                                       const T* lamv, cudaStream_t st, T* X2, long long inc2, const T* lamf, long long fpi) {
+    return launch_chunked_contig<T>(A, B, C, op, X, out_op, g, lam, lamv, st, X2, inc2, nullptr, nullptr, lamf, fpi);
 }
 // Plain prox (OUT_X) of A (op) B with a SPARSE result: X only holds each segment's value at its start; Mk[fiber][chunk] = start mask,
 // Cv[fiber][chunk] = value entering the chunk (chunks of 32 samples, (len + 31) / 32 per fiber).  See scatter_fibers_ex_sparse.
 template <typename T>
 cudaError_t prox_fibers_chunked_contig_sparse(const T* A, const T* B, InOp op, T* X, FiberGeom g, T lam, const T* lamv, uint32_t* Mk, T* Cv,
-                                              cudaStream_t st) {
-    return launch_chunked_contig<T>(A, B, nullptr, op, X, OUT_X, g, lam, lamv, st, nullptr, 0, Mk, Cv);
+                                              cudaStream_t st, const T* lamf, long long fpi) {
+    return launch_chunked_contig<T>(A, B, nullptr, op, X, OUT_X, g, lam, lamv, st, nullptr, 0, Mk, Cv, lamf, fpi);
 }
 template cudaError_t prox_fibers_chunked_contig_sparse<double>(const double*, const double*, InOp, double*, FiberGeom, double, const double*, uint32_t*,
-                                                               double*, cudaStream_t);
+                                                               double*, cudaStream_t, const double*, long long);
 template cudaError_t prox_fibers_chunked_contig_sparse<float>(const float*, const float*, InOp, float*, FiberGeom, float, const float*, uint32_t*, float*,
-                                                              cudaStream_t);
+                                                              cudaStream_t, const float*, long long);
 
 template cudaError_t prox_fibers_chunked_contig<double>(const double*, const double*, const double*, InOp, double*, int, FiberGeom,
-                                                        double, const double*, cudaStream_t, double*, long long);
+                                                        double, const double*, cudaStream_t, double*, long long, const double*, long long);
 template cudaError_t prox_fibers_chunked_contig<float>(const float*, const float*, const float*, InOp, float*, int, FiberGeom,
-                                                       float, const float*, cudaStream_t, float*, long long);
+                                                       float, const float*, cudaStream_t, float*, long long, const float*, long long);
 
 // ------------------------------------------------------------------------------------------------------------------
 // k_prox_chunked_strided: fibers with element stride `inc` whose neighbours are adjacent in memory (every dimension but

@@ -93,6 +93,7 @@ template <typename T> struct LaneArgs {
     unsigned long long* stats;      // [0] repair scans, [1] retired lanes
     unsigned long long* tlog;       // optional (tools): per task TLOG_WORDS words, see k_lane
     long long ntasks;
+    const T* lamf; long long fpi;   // per-fiber penalties (the LAMF instantiations): fiber j's is lamf[j / fpi], in place of lam
 };
 constexpr int TLOG_WORDS = 16;
 
@@ -253,7 +254,8 @@ __device__ __forceinline__ void run_dev(Lane<T>& L, const DevWin<T, W> dw, const
     L.in_rec = in_;
 }
 
-template <typename T, int W> struct DevEnv {
+// LAMF: the lane's own penalty; scan() then takes 2 lam, -2 lam from the lam2 it is given (the same values lamc would hold for it)
+template <typename T, int W, bool LAMF = false> struct DevEnv {
     Lane<T> L; int lane; DevWin<T, W> dw; const acc_t* lamc;      // lamc: {2 lam, -2 lam} in the kernel's parameter block (constant bank)
     template <class F> __device__ __forceinline__ void each(F f) { f(L, lane); }
     template <class F> __device__ __forceinline__ int rmin(F f) { return __reduce_min_sync(0xffffffffu, f(L, lane)); }
@@ -261,9 +263,14 @@ template <typename T, int W> struct DevEnv {
     template <class F> __device__ __forceinline__ bool any(F f) { return __any_sync(0xffffffffu, f(L, lane)); }
     __device__ __forceinline__ void sync() { __syncwarp(); }
     __device__ __forceinline__ void scan(Lane<T>& l, const Window<T, W>&, int, const TaskGeom& g, const acc_t*, acc_t lam2, bool ph1, int niter) {
-        if (ph1) run_dev<true, T, W>(l, dw, g, lamc[0], lamc[1], niter); else run_dev<false, T, W>(l, dw, g, lamc[0], lamc[1], niter);
+        if constexpr (LAMF) { if (ph1) run_dev<true, T, W>(l, dw, g, lam2, -lam2, niter); else run_dev<false, T, W>(l, dw, g, lam2, -lam2, niter); }
+        else { if (ph1) run_dev<true, T, W>(l, dw, g, lamc[0], lamc[1], niter); else run_dev<false, T, W>(l, dw, g, lamc[0], lamc[1], niter); }
     }
 };
+// a lane's own penalty, as warp_task takes it per lane (each thread of the warp is one lane)
+template <typename T> struct LaneLam { T v; __device__ __forceinline__ T operator()(int) const { return v; } };
+// the penalty of fiber j of a LAMF launch
+template <typename T> __device__ __forceinline__ T fiber_lam(const LaneArgs<T>& a, long long j) { return a.lamf[j / a.fpi]; }
 
 // ---------------------------------------------------------------- STRIDED layout: feed and drain
 template <typename T, int W, int RT, int OP> struct FeedStrided {
@@ -524,7 +531,7 @@ template <typename T, int W, int RT, int OP, int LAY, int NW> struct LaneSmem {
 // each repair scan the lanes copy the next NB rows of the fiber -- with the pass's input arithmetic applied -- into the warp's
 // window memory, and the scan reads them from there (a dependent global load per step would cost ~1 us each); rows beyond the
 // staged range fall back to global memory.  Lane 0 writes the results.  Rare: a handful of fibers per solve.
-template <typename T, int OP, int NB, int W>
+template <typename T, int OP, int NB, int W, bool LAMF = false>
 __device__ __noinline__ int repair_fiber(const LaneArgs<T>* a, const ChunkPlan pl, long long fiber, long long gbase, long long stride, long long tfib,
                                          long long nfp, T* buf, const acc_t* rcp, int lane) {
     const int* rec = a->rec;
@@ -539,7 +546,9 @@ __device__ __noinline__ int repair_fiber(const LaneArgs<T>* a, const ChunkPlan p
                                 buf_lo = pos; buf_n = pl.n - pos < NBS ? pl.n - pos : NBS;
                                 for (int j = lane; j < buf_n; j += 32) buf[j] = in_at(pos + j);
                                 __syncwarp(); };
-    return verify_repair_fiber<T>(pl, a->lam,
+    // LAMF: record index fiber = group * LANES + lane of a group (slab z, first column x0) is fiber z inc + x0 + lane
+    const long long grp = fiber / LANES;
+    return verify_repair_fiber<T>(pl, LAMF ? fiber_lam<T>(*a, (grp / a->gps) * a->inc + (grp % a->gps) * LANES + fiber % LANES) : a->lam,
         [&](int c) { return rec[(0 * cstride + c) * nfp + fiber]; },
         [&](int c) { return rec[(3 * cstride + c) * nfp + fiber]; },
         [&](int c) { return rec[(4 * cstride + c) * nfp + fiber]; },
@@ -564,7 +573,9 @@ __device__ __forceinline__ unsigned smid() { unsigned r; asm volatile("mov.u32 %
 // ring of LOP_DR_B lives in what the third CTA would have used).
 template <int OP, int NW> constexpr int lane_min_ctas() { return ((OpTraits<OP>::staged ? 8 : 12) + NW - 1) / NW; }
 
-template <typename T, int W, int RT, int TITER, int OP, int NW, int LAY, bool LOG>
+// LAMF: per-fiber penalties (plain op): each lane reads its fiber's penalty once, at task start, and uses it for the scan, the tail and
+// the repair of its fiber; a CONTIG warp's 32 fibers may belong to two penalty groups, a STRIDED warp's lie in one slab.
+template <typename T, int W, int RT, int TITER, int OP, int NW, int LAY, bool LOG, bool LAMF = false>
 __global__ void __launch_bounds__(NW * 32, lane_min_ctas<OP, NW>()) k_lane(const __grid_constant__ LaneArgs<T> a) {
     using SM = LaneSmem<T, W, RT, OP, LAY, NW>;
     extern __shared__ __align__(1024) unsigned char smem[];
@@ -609,23 +620,27 @@ __global__ void __launch_bounds__(NW * 32, lane_min_ctas<OP, NW>()) k_lane(const
     const long long nfp = (long long)a.slabs * a.gps * LANES;
     const long long fiber = group * LANES + lane;
 
-    DevEnv<T, W> env; env.lane = lane; env.lamc = a.lamc;
+    // LAMF: this lane's penalty (an invalid lane takes lane 0's)
+    const T lamf = LAMF ? fiber_lam<T>(a, (long long)z * a.inc + x0 + (valid ? lane : 0)) : T(0);
+    DevEnv<T, W, LAMF> env; env.lane = lane; env.lamc = a.lamc;
     env.dw.wbase = s32(win); env.dw.lane8 = lane * (uint32_t)sizeof(T); env.dw.flg = s32(flg) + lane * (uint32_t)Window<T, W>::FP; env.dw.rcp = s32(rcp);
     Window<T, W> w{win, flg};
-    env.L.init(w, lane, g, a.lam, valid);
+    if constexpr (LAMF) env.L.init(w, lane, g, lamf, valid); else env.L.init(w, lane, g, a.lam, valid);
     TaskStats ts{};
     TaskStats* const sp = LOG ? &ts : nullptr;
     const long long tc0 = LOG ? clock64() : 0;
     if constexpr (LAY == LAY_CONTIG) {
         FeedContig<T, W> feed{&a, win, bar, x0, g.p0 / FeedContig<T, W>::R, lane};
         DrainContig<T, W> drain{&a, stB, x0, lane, g.ce};
-        warp_task<T, W, TITER>(env, feed, drain, w, rcp, g, a.lam, TITER + TITER / 2 + FeedContig<T, W>::R, sp);
+        if constexpr (LAMF) warp_task<T, W, TITER>(env, feed, drain, w, rcp, g, LaneLam<T>{lamf}, TITER + TITER / 2 + FeedContig<T, W>::R, sp);
+        else warp_task<T, W, TITER>(env, feed, drain, w, rcp, g, a.lam, TITER + TITER / 2 + FeedContig<T, W>::R, sp);
     } else {
         DRing<T, W, OP> ring;
         FeedStrided<T, W, RT, OP> feed{&a, win, stB, stC, bar, x0, z, g.p0 / RT, lane, &ring};
         DrainStrided<T, W, OP> drain; drain.ring = &ring; drain.B = a.B; drain.C = a.C; drain.X = a.X; drain.X2 = a.X2; drain.gbase = gbase; drain.stride = a.inc;
         drain.pf_row = -1; drain.pol = policy_evict_first(); drain.ce = g.ce; drain.tbase = tgroup; drain.n = pl.n; drain.nvalid = (int)(a.per_slab - x0 < LANES ? a.per_slab - x0 : LANES);
-        warp_task<T, W, TITER>(env, feed, drain, w, rcp, g, a.lam, TITER + TITER / 2 + RT, sp);
+        if constexpr (LAMF) warp_task<T, W, TITER>(env, feed, drain, w, rcp, g, LaneLam<T>{lamf}, TITER + TITER / 2 + RT, sp);
+        else warp_task<T, W, TITER>(env, feed, drain, w, rcp, g, a.lam, TITER + TITER / 2 + RT, sp);
     }
     if (tl && lane == 0) {
         tl[1] = gtimer();
@@ -667,7 +682,7 @@ __global__ void __launch_bounds__(NW * 32, lane_min_ctas<OP, NW>()) k_lane(const
     while (m) {
         const int src = __ffs(m) - 1; m &= m - 1;
         const long long gb = __shfl_sync(0xffffffffu, gbase, src);
-        nrep += repair_fiber<T, OP, W * LANES, W>(&a, pl, group * LANES + src, gb, gstride, tgroup + (long long)src * pl.n, nfp, win, rcp, lane);
+        nrep += repair_fiber<T, OP, W * LANES, W, LAMF>(&a, pl, group * LANES + src, gb, gstride, tgroup + (long long)src * pl.n, nfp, win, rcp, lane);
     }
     if (nrep && lane == 0) atomicAdd(a.stats, (unsigned long long)nrep);
 }
@@ -722,10 +737,10 @@ static long long lane_scratch_bytes(long long groups_cap, long long nf, int len)
 }
 
 // launch one instantiation; with `slots` only report how many warp tasks the device can hold at once
-template <typename T, int W, int RT, int TITER, int OP, int NW, int LAY>
+template <typename T, int W, int RT, int TITER, int OP, int NW, int LAY, bool LAMF = false>
 static cudaError_t launch_v(LaneArgs<T>& a, cudaStream_t st, int* slots) {
     using SM = LaneSmem<T, W, RT, OP, LAY, NW>;
-    auto kern = k_lane<T, W, RT, TITER, OP, NW, LAY, false>;
+    auto kern = k_lane<T, W, RT, TITER, OP, NW, LAY, false, LAMF>;
     const size_t smem = SM::total;
     static int s_slots = 0;                      // per instantiation: resident warps on the current device
     if (!s_slots) {
@@ -740,20 +755,28 @@ static cudaError_t launch_v(LaneArgs<T>& a, cudaStream_t st, int* slots) {
     }
     if (slots) { *slots = s_slots; return cudaSuccess; }
     const unsigned blocks = (unsigned)((a.ntasks + NW - 1) / NW);
-    if (a.tlog) {                                // tools: the instrumented copy (same shared memory, same residency)
-        auto klog = k_lane<T, W, RT, TITER, OP, NW, LAY, true>;
-        cudaError_t e = cudaFuncSetAttribute(klog, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        cudaFuncSetAttribute(klog, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-        klog<<<blocks, NW * 32, smem, st>>>(a);
-    } else kern<<<blocks, NW * 32, smem, st>>>(a);
+    if constexpr (!LAMF) {
+        if (a.tlog) {                            // tools: the instrumented copy (same shared memory, same residency)
+            auto klog = k_lane<T, W, RT, TITER, OP, NW, LAY, true>;
+            cudaError_t e = cudaFuncSetAttribute(klog, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            if (e != cudaSuccess) return e;
+            cudaFuncSetAttribute(klog, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+            klog<<<blocks, NW * 32, smem, st>>>(a);
+            return cudaGetLastError();
+        }
+    }
+    kern<<<blocks, NW * 32, smem, st>>>(a);
     return cudaGetLastError();
 }
 
 // tuning variants (window rows, warps per CTA); 0 is the default: CTAs of 4 warps -- one per SM sub-partition -- three of which fit
 // an SM when the pass needs no staging (12 resident warps, 3 per sub-partition; single-warp CTAs only reach 11, unevenly spread)
-template <typename T, int OP, int LAY>
+template <typename T, int OP, int LAY, bool LAMF = false>
 static cudaError_t launch_variant(int variant, LaneArgs<T>& a, cudaStream_t st, int* slots) {
+    if constexpr (LAMF) {           // per-fiber penalties: the default variant of each storage type only (lane_prox picks 6 / 0)
+        if constexpr (sizeof(T) == 4) return launch_v<T, 128, 8, 32, OP, 4, LAY, true>(a, st, slots);
+        else return launch_v<T, 64, 8, 16, OP, 4, LAY, true>(a, st, slots);
+    }
     switch (variant) {
         case 1: return launch_v<T, 64, 8, 16, OP, 1, LAY>(a, st, slots);
         case 5: return launch_v<T, 128, 8, 16, OP, 1, LAY>(a, st, slots);
@@ -765,6 +788,8 @@ static cudaError_t launch_variant(int variant, LaneArgs<T>& a, cudaStream_t st, 
 }
 template <typename T>
 static cudaError_t launch_any(int lay, int op, int variant, LaneArgs<T>& a, cudaStream_t st, int* slots) {
+    if (a.lamf) return lay == LAY_CONTIG ? launch_variant<T, LOP_PLAIN, LAY_CONTIG, true>(variant, a, st, slots)
+                                         : launch_variant<T, LOP_PLAIN, LAY_STRIDED, true>(variant, a, st, slots);
     if (lay == LAY_CONTIG) return launch_variant<T, LOP_PLAIN, LAY_CONTIG>(variant, a, st, slots);
     switch (op) {
         case LOP_DR_B: return launch_variant<T, LOP_DR_B, LAY_STRIDED>(variant, a, st, slots);
@@ -783,10 +808,12 @@ static cudaError_t launch_any(int lay, int op, int variant, LaneArgs<T>& a, cuda
 //   f * len + r -- for the fibers of a 2D image that is the transposed image.
 // scratch: lane_scratch() (records, group counters).  Returns cudaErrorInvalidConfiguration when the shape does not suit TMA
 // tiling (unaligned base, row pitch not a multiple of 16 bytes, tiny fibers) -- the caller then uses the chunked engine.
+// lamf (plain op only): fiber j's penalty is lamf[j / fpi] (device table, every entry > 0: the caller's to ensure), lam unused.
 template <typename T>
 cudaError_t lane_prox(int op, const T* A, const T* B, const T* C, T* X, long long nf, int len, long long inc, T lam, void* scratch,
-                      cudaStream_t st, T* X2) {
-    if (nf <= 0 || len < 2 || !(lam > T(0)) || op < 0 || op > LOP_PLAIN_T) return cudaErrorInvalidConfiguration;
+                      cudaStream_t st, T* X2, const T* lamf, long long fpi) {
+    if (lamf && (op != LOP_PLAIN || fpi < 1)) return cudaErrorInvalidConfiguration;
+    if (nf <= 0 || len < 2 || !(lamf || lam > T(0)) || op < 0 || op > LOP_PLAIN_T) return cudaErrorInvalidConfiguration;
     const int lay = inc == 1 ? LAY_CONTIG : LAY_STRIDED;
     if (lay == LAY_CONTIG && op != LOP_PLAIN) return cudaErrorInvalidConfiguration;
     if (lay == LAY_STRIDED && nf % inc != 0) return cudaErrorInvalidConfiguration;
@@ -798,6 +825,7 @@ cudaError_t lane_prox(int op, const T* A, const T* B, const T* C, T* X, long lon
     LaneArgs<T> a;
     memset(&a, 0, sizeof(a));
     a.A = A; a.B = B; a.C = C; a.X = X; a.X2 = X2; a.lam = lam; a.lamc[0] = 2.0 * (acc_t)lam; a.lamc[1] = -a.lamc[0];
+    a.lamf = lamf; a.fpi = fpi;
     const int BR = 128 / (int)sizeof(T);
     if (lay == LAY_CONTIG) {
         if (nf > 0x7fffffff) return cudaErrorInvalidConfiguration;
@@ -886,7 +914,9 @@ unsigned long long lane_read_stats(int reset) {
     return v;
 }
 
-template cudaError_t lane_prox<double>(int, const double*, const double*, const double*, double*, long long, int, long long, double, void*, cudaStream_t, double*);
-template cudaError_t lane_prox<float>(int, const float*, const float*, const float*, float*, long long, int, long long, float, void*, cudaStream_t, float*);
+template cudaError_t lane_prox<double>(int, const double*, const double*, const double*, double*, long long, int, long long, double, void*, cudaStream_t, double*,
+                                       const double*, long long);
+template cudaError_t lane_prox<float>(int, const float*, const float*, const float*, float*, long long, int, long long, float, void*, cudaStream_t, float*,
+                                      const float*, long long);
 
 }  // namespace ptvl

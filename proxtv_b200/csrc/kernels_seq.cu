@@ -9,10 +9,11 @@
 
 namespace ptv {
 
-template <typename T, bool WEIGHTED>
+// LAMF: fiber j's penalty is lamf[j / fpi] (one per group of fpi fibers), the uniform scan with that value
+template <typename T, bool WEIGHTED, bool LAMF = false>
 __global__ void __launch_bounds__(32) k_prox_seq(const T* __restrict__ A, const T* __restrict__ B, const T* __restrict__ C, int op, T* __restrict__ X,
                                                  int out_op, FiberGeom g, T lam, const T* __restrict__ lamv,
-                                                 const int* __restrict__ list, long long nlist) {
+                                                 const int* __restrict__ list, long long nlist, const T* __restrict__ lamf, long long fpi) {
     long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (list) { if (j >= nlist) return; j = list[j]; }
     else if (j >= g.nf) return;
@@ -42,7 +43,7 @@ __global__ void __launch_bounds__(32) k_prox_seq(const T* __restrict__ A, const 
         auto ld = [&](int i) -> T { return lamv[wbase + (long long)i * inc]; };
         run(ArrayLam<T, decltype(ld)>{ld});
     } else {
-        run(UniformLam<T>{lam});
+        run(UniformLam<T>{LAMF ? lamf[j / fpi] : lam});
     }
 }
 
@@ -94,18 +95,19 @@ template cudaError_t prox_const_fibers<float>(const float*, long long, int, int,
 
 template <typename T>
 cudaError_t prox_fibers_seq(const T* A, const T* B, const T* C, InOp op, T* X, int out_op, FiberGeom g, T lam, const T* lamv,
-                            const int* list, long long nlist, cudaStream_t st) {
+                            const int* list, long long nlist, cudaStream_t st, const T* lamf, long long fpi) {
     long long cnt = list ? nlist : g.nf;
     if (cnt <= 0 || g.len <= 0) return cudaSuccess;
     unsigned blocks = (unsigned)((cnt + 31) / 32);
-    if (lamv) k_prox_seq<T, true><<<blocks, 32, 0, st>>>(A, B, C, (int)op, X, out_op, g, lam, lamv, list, nlist);
-    else      k_prox_seq<T, false><<<blocks, 32, 0, st>>>(A, B, C, (int)op, X, out_op, g, lam, lamv, list, nlist);
+    if (lamv) k_prox_seq<T, true><<<blocks, 32, 0, st>>>(A, B, C, (int)op, X, out_op, g, lam, lamv, list, nlist, nullptr, 1);
+    else if (lamf) k_prox_seq<T, false, true><<<blocks, 32, 0, st>>>(A, B, C, (int)op, X, out_op, g, lam, nullptr, list, nlist, lamf, fpi);
+    else      k_prox_seq<T, false><<<blocks, 32, 0, st>>>(A, B, C, (int)op, X, out_op, g, lam, lamv, list, nlist, nullptr, 1);
     return cudaGetLastError();
 }
 
 template cudaError_t prox_fibers_seq<double>(const double*, const double*, const double*, InOp, double*, int, FiberGeom, double, const double*,
-                                             const int*, long long, cudaStream_t);
+                                             const int*, long long, cudaStream_t, const double*, long long);
 template cudaError_t prox_fibers_seq<float>(const float*, const float*, const float*, InOp, float*, int, FiberGeom, float, const float*,
-                                            const int*, long long, cudaStream_t);
+                                            const int*, long long, cudaStream_t, const float*, long long);
 
 }  // namespace ptv

@@ -29,6 +29,7 @@
 // (or a segment too long for the window) is repaired by an exact sequential continuation from the last verified renewal state,
 // which stops as soon as it reproduces one of the chunk's recorded segment starts (its first three): a few rows, as a rule.
 #pragma once
+#include <type_traits>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <math.h>
@@ -258,12 +259,15 @@ PTV_HD long long task_clock() {
 #endif
 }
 
-template <typename T, int W, int TITER, class Env, class Feed, class Drain>
-PTV_HD void warp_task(Env& env, Feed& feed, Drain& drain, const Window<T, W>& w, const acc_t* __restrict__ rcp, const TaskGeom g, T lam,
+// lam: one penalty for every lane (a T), or per lane (a callable: lam(lane) -> that lane's penalty; Env::scan then gets 2 lam(lane))
+template <typename T, int W, int TITER, class Env, class Feed, class Drain, class Lam>
+PTV_HD void warp_task(Env& env, Feed& feed, Drain& drain, const Window<T, W>& w, const acc_t* __restrict__ rcp, const TaskGeom g, Lam lam,
                       int ahead, TaskStats* stats) {
     constexpr int R = Feed::R;
     constexpr int DMIN = 8;           // rows kept in front of a lane that overruns its chunk; epochs shorter than this count as starved
-    const acc_t lam2 = 2.0 * (acc_t)lam;
+    constexpr bool per_lane = !std::is_arithmetic<Lam>::value;
+    acc_t lam2 = 0.0;
+    if constexpr (!per_lane) lam2 = 2.0 * (acc_t)lam;
     int row_lo = g.p0;                // first row still held by the window
     int row_req = g.p0;               // rows below have been requested
     int row_hi = g.p0;                // rows below are in the window, ready for the scan
@@ -361,7 +365,10 @@ PTV_HD void warp_task(Env& env, Feed& feed, Drain& drain, const Window<T, W>& w,
                 // lanes that wait in front of the fiber's last sample: finish them once it is in the window
                 const bool movable = env.any([&](Lane<T>& L, int) { return !L.done && L.i < g.n - 1; });
                 if (!movable && row_hi >= g.n) {
-                    env.each([&](Lane<T>& L, int lane) { L.template finish_tail<W>(w, lane, g, lam); });
+                    env.each([&](Lane<T>& L, int lane) {
+                        if constexpr (per_lane) L.template finish_tail<W>(w, lane, g, (T)lam(lane));
+                        else L.template finish_tail<W>(w, lane, g, lam);
+                    });
                     env.sync();
                     if (stats) { stats->tail++; stats->c_stuck += task_clock() - tc; }
                     continue;
@@ -386,7 +393,9 @@ PTV_HD void warp_task(Env& env, Feed& feed, Drain& drain, const Window<T, W>& w,
             env.each([&](Lane<T>& L, int lane) {
                 const int d = lim_ - L.i;
                 if (!L.done && d >= 1) {
-                    env.scan(L, w, lane, g, rcp, lam2, ph1_, d < TITER ? d : TITER);      // Lane::run, or the kernel's equivalent device form
+                    // Lane::run, or the kernel's equivalent device form
+                    if constexpr (per_lane) env.scan(L, w, lane, g, rcp, 2.0 * (acc_t)lam(lane), ph1_, d < TITER ? d : TITER);
+                    else env.scan(L, w, lane, g, rcp, lam2, ph1_, d < TITER ? d : TITER);
                     L.template settle<W>(w, lane, g);
                 }
             });

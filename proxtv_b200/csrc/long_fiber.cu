@@ -16,7 +16,8 @@ namespace ptv {
 
 template <typename T>
 cudaError_t prox_fibers_chunked_contig(const T* A, const T* B, const T* C, InOp op, T* X, int out_op, FiberGeom g, T lam,
-                                       const T* lamv, cudaStream_t st, T* X2 = nullptr, long long inc2 = 0);
+                                       const T* lamv, cudaStream_t st, T* X2 = nullptr, long long inc2 = 0,
+                                       const T* lamf = nullptr, long long fpi = 1);
 
 constexpr int LF_TL = 8192, LF_HL = 512, LF_HR = 512, LF_W = LF_TL + LF_HL + LF_HR;
 

@@ -4,6 +4,12 @@
 //   strided fibers, with scratch (default)                        -> tiled gather (fused input op) + chunked kernel + tiled scatter (fused output form)
 //   strided fibers, ENGINE_CHUNKED_STRIDED or no scratch          -> chunked kernel staging FPB adjacent fibers directly
 //   everything else (tiny fibers, weighted strided, ENGINE_SEQ)   -> sequential lane-per-fiber kernel
+//
+// With a per-fiber penalty table (prox_fibers_lamf: fiber j's penalty is lamf[j / fpi]) the lane engine (its per-lane instantiation,
+// only for a table whose entries are all > 0, as the uniform route needs lam > 0), the chunked kernels (contiguous, and behind the
+// gather -> scan -> scatter route) and the sequential kernel take the table.  Two routes decline it and pass the fibers down: the
+// direct strided kernel of ENGINE_CHUNKED_STRIDED (to the gather route, or the sequential kernel without scratch) and the long-fiber
+// tiles (to the sequential kernel).  Every fiber's result is the uniform pass's with its own penalty on the kernel family that ran it.
 #include "ptv_internal.h"
 #include "chunk_core.cuh"
 
@@ -11,10 +17,11 @@ namespace ptv {
 
 template <typename T>
 cudaError_t prox_fibers_seq(const T* A, const T* B, const T* C, InOp op, T* X, int out_op, FiberGeom g, T lam, const T* lamv,
-                            const int* list, long long nlist, cudaStream_t st);
+                            const int* list, long long nlist, cudaStream_t st, const T* lamf = nullptr, long long fpi = 1);
 template <typename T>
 cudaError_t prox_fibers_chunked_contig(const T* A, const T* B, const T* C, InOp op, T* X, int out_op, FiberGeom g, T lam,
-                                       const T* lamv, cudaStream_t st, T* X2 = nullptr, long long inc2 = 0);
+                                       const T* lamv, cudaStream_t st, T* X2 = nullptr, long long inc2 = 0,
+                                       const T* lamf = nullptr, long long fpi = 1);
 template <typename T>
 cudaError_t prox_fibers_chunked_strided(const T* A, const T* B, const T* C, InOp op, T* X, int out_op, FiberGeom g, T lam, T* V,
                                         cudaStream_t st);
@@ -28,7 +35,7 @@ template <typename T>
 cudaError_t scatter_fibers_ex(const T* in, const T* A, const T* B, const T* C, InOp op, int out_op, T* X, FiberGeom g, cudaStream_t st);
 template <typename T>
 cudaError_t prox_fibers_chunked_contig_sparse(const T* A, const T* B, InOp op, T* X, FiberGeom g, T lam, const T* lamv, uint32_t* Mk, T* Cv,
-                                              cudaStream_t st);
+                                              cudaStream_t st, const T* lamf = nullptr, long long fpi = 1);
 template <typename T>
 cudaError_t scatter_fibers_sparse(const T* in, const uint32_t* Mk, const T* Cv, const T* A, const T* B, const T* C, InOp op, int out_op, T* X,
                                   FiberGeom g, cudaStream_t st);
@@ -42,18 +49,18 @@ int long_fiber_last() { const int d = device_slot(); const int v = d < 0 ? 0 : g
 
 template <typename T>
 cudaError_t prox_fibers_ex(const T* A, const T* B, const T* C, InOp op, T* X, int out_op, FiberGeom g, T lam, const T* lamv,
-                           Engine eng, T* scratch, cudaStream_t st, long long scratch_elems) {
+                           Engine eng, T* scratch, cudaStream_t st, long long scratch_elems, const T* lamf, long long fpi, bool lamf_pos) {
     if (g.nf <= 0 || g.len <= 0) return cudaSuccess;
     // plain unweighted prox over many fibers: the lane-per-fiber streaming engine (kernels_lane.cu), when the shape suits TMA tiling
     // and there are enough fibers to fill the machine without cutting them (a single long fiber stays with the chunked kernels,
     // which are also the bit-faithful ones behind the 1D entry points)
-    if ((eng == ENGINE_AUTO || eng == ENGINE_LANE || eng == ENGINE_LANE_T) && op == IN_A && out_op == OUT_X && !lamv && lam > T(0) && g.len >= 64 && g.nf >= 1024) {
+    if ((eng == ENGINE_AUTO || eng == ENGINE_LANE || eng == ENGINE_LANE_T) && op == IN_A && out_op == OUT_X && !lamv && (lamf ? lamf_pos : lam > T(0)) && g.len >= 64 && g.nf >= 1024) {
         const void* ptrs[2] = {A, X};
         if (ptvl::lane_shape_ok(g.nf, g.len, g.inc, sizeof(T), ptrs, 2)) {
             void* lscr = ptvl::lane_scratch(g.nf, g.len);
             if (lscr) {
                 KernelSpan span(g.inc == 1 ? KC_PROX_CONTIG : KC_PROX_STRIDED, 1, st);
-                cudaError_t e = ptvl::lane_prox<T>(ptvl::LANE_PLAIN, A, nullptr, nullptr, X, g.nf, g.len, g.inc, lam, lscr, st);
+                cudaError_t e = ptvl::lane_prox<T>(ptvl::LANE_PLAIN, A, nullptr, nullptr, X, g.nf, g.len, g.inc, lam, lscr, st, nullptr, lamf, fpi);
                 if (e != cudaErrorInvalidConfiguration) return e;
                 cudaGetLastError(); span.cancel();
             }
@@ -62,14 +69,14 @@ cudaError_t prox_fibers_ex(const T* A, const T* B, const T* C, InOp op, T* X, in
     if (eng != ENGINE_SEQ && g.len >= 2 * 32) {
         if (g.inc == 1) {
             KernelSpan span(KC_PROX_CONTIG, 1, st);
-            cudaError_t e = prox_fibers_chunked_contig<T>(A, B, C, op, X, out_op, g, lam, lamv, st);
+            cudaError_t e = prox_fibers_chunked_contig<T>(A, B, C, op, X, out_op, g, lam, lamv, st, nullptr, 0, lamf, fpi);
             if (e != cudaErrorInvalidConfiguration) return e;
             cudaGetLastError();
             span.cancel();                  // refused before launching: the launch counters count kernels that ran
             // too long for shared memory: overlapping tiles, verified stitching (long_fiber.cu); the scratch convention for
             // this case is lf_scratch_elems() elements, which the 1D host entry points provide
             // (plain results only: the agreement test of the stitching compares prox values, which the fused output forms would hide)
-            if (!lamv && out_op == OUT_X && scratch && scratch_elems >= lf_scratch_elems(g.nf, g.len)) {
+            if (!lamv && !lamf && out_op == OUT_X && scratch && scratch_elems >= lf_scratch_elems(g.nf, g.len)) {
                 KernelSpan lspan(KC_PROX_CONTIG, 1, st);
                 e = prox_long_fibers<T>(A, B, op, X, out_op, g, lam, scratch, lf_scratch_elems(g.nf, g.len), st);
                 if (e == cudaSuccess || e == cudaErrorNotReady) long_fiber_note(e == cudaSuccess ? 1 : 0);
@@ -84,7 +91,7 @@ cudaError_t prox_fibers_ex(const T* A, const T* B, const T* C, InOp op, T* X, in
             // kernels cost less than staging strided fibers directly at one CTA per SM; ENGINE_CHUNKED_STRIDED selects the
             // direct kernel (no transposed copy, FPB adjacent fibers per CTA) for comparison and for callers without scratch.
             const bool direct = (eng == ENGINE_CHUNKED_STRIDED) || !scratch || g.nf % g.inc != 0;
-            if (direct) {
+            if (direct && !lamf) {
                 KernelSpan span(KC_PROX_STRIDED, 1, st);
                 cudaError_t e = prox_fibers_chunked_strided<T>(A, B, C, op, X, out_op, g, lam,
                                                                (scratch && eng == ENGINE_CHUNKED_STRIDED) ? scratch : nullptr, st);
@@ -104,8 +111,9 @@ cudaError_t prox_fibers_ex(const T* A, const T* B, const T* C, InOp op, T* X, in
                 const long long lpf = ((long long)g.len + 31) / 32;
                 T* Cv = scratch + 2 * n; uint32_t* Mk = reinterpret_cast<uint32_t*>(Cv + g.nf * lpf);
                 { KernelSpan span(KC_PROX_STRIDED, 1, st);
-                  e = sparse ? prox_fibers_chunked_contig_sparse<T>(t1, nullptr, IN_A, t2, gc, lam, nullptr, Mk, Cv, st)
-                             : prox_fibers_chunked_contig<T>(t1, nullptr, nullptr, IN_A, t2, OUT_X, gc, lam, nullptr, st);
+                  // the gathered row of fiber j is row j: the penalty table applies unchanged
+                  e = sparse ? prox_fibers_chunked_contig_sparse<T>(t1, nullptr, IN_A, t2, gc, lam, nullptr, Mk, Cv, st, lamf, fpi)
+                             : prox_fibers_chunked_contig<T>(t1, nullptr, nullptr, IN_A, t2, OUT_X, gc, lam, nullptr, st, nullptr, 0, lamf, fpi);
                   if (e == cudaErrorInvalidConfiguration) span.cancel(); }
                 if (e == cudaSuccess) {
                     KernelSpan span(KC_ELEMENTWISE, 1, st);
@@ -119,7 +127,13 @@ cudaError_t prox_fibers_ex(const T* A, const T* B, const T* C, InOp op, T* X, in
         }
     }
     KernelSpan span(g.inc == 1 ? KC_PROX_CONTIG : KC_PROX_STRIDED, 1, st);
-    return prox_fibers_seq<T>(A, B, C, op, X, out_op, g, lam, lamv, nullptr, 0, st);
+    return prox_fibers_seq<T>(A, B, C, op, X, out_op, g, lam, lamv, nullptr, 0, st, lamf, fpi);
+}
+
+template <typename T>
+cudaError_t prox_fibers_lamf(const T* A, const T* B, InOp op, T* X, FiberGeom g, const T* lamf, long long fpi, bool pos, Engine eng, T* scratch,
+                             cudaStream_t st, long long scratch_elems) {
+    return prox_fibers_ex<T>(A, B, nullptr, op, X, OUT_X, g, T(0), nullptr, eng, scratch, st, scratch_elems, lamf, fpi, pos);
 }
 
 template <typename T>
@@ -129,7 +143,9 @@ cudaError_t prox_fibers(const T* A, const T* B, InOp op, T* X, int out_op, Fiber
 }
 
 #define INST(T) \
-    template cudaError_t prox_fibers_ex<T>(const T*, const T*, const T*, InOp, T*, int, FiberGeom, T, const T*, Engine, T*, cudaStream_t, long long); \
+    template cudaError_t prox_fibers_ex<T>(const T*, const T*, const T*, InOp, T*, int, FiberGeom, T, const T*, Engine, T*, cudaStream_t, long long, \
+                                           const T*, long long, bool); \
+    template cudaError_t prox_fibers_lamf<T>(const T*, const T*, InOp, T*, FiberGeom, const T*, long long, bool, Engine, T*, cudaStream_t, long long); \
     template cudaError_t prox_fibers<T>(const T*, const T*, InOp, T*, int, FiberGeom, T, const T*, Engine, T*, cudaStream_t, long long);
 INST(double)
 INST(float)

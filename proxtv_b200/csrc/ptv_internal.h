@@ -54,7 +54,14 @@ cudaError_t prox_fibers(const T* A, const T* B, InOp op, T* X, int out_op, Fiber
 // Same, with a third array C for the fused Douglas-Rachford row pass (out_op 3 / 4, see OutOp in chunk_core.cuh).
 template <typename T>
 cudaError_t prox_fibers_ex(const T* A, const T* B, const T* C, InOp op, T* X, int out_op, FiberGeom g, T lam, const T* lamv,
-                           Engine eng, T* scratch, cudaStream_t st, long long scratch_elems = 0);
+                           Engine eng, T* scratch, cudaStream_t st, long long scratch_elems = 0, const T* lamf = nullptr, long long fpi = 1,
+                           bool lamf_pos = false);
+// prox_fibers with out_op 0, no per-edge weights and one penalty per group of fpi fibers: fiber j's is lamf[j / fpi] (device table,
+// fpi >= 1), and its result equals bit for bit the uniform pass with that penalty on the kernel family that ran it (the routes that
+// decline a table: prox_dispatch.cu).  pos: every entry of the table is > 0 (the lane engine takes only such tables).
+template <typename T>
+cudaError_t prox_fibers_lamf(const T* A, const T* B, InOp op, T* X, FiberGeom g, const T* lamf, long long fpi, bool pos, Engine eng, T* scratch,
+                             cudaStream_t st, long long scratch_elems = 0);
 
 long long strided_scratch_elems(long long nf, long long len);   // scratch elements that enable the sparse strided route (else 2n: dense route)
 long long lf_scratch_elems(long long nf, long long len);     // scratch elements prox_fibers needs for contiguous fibers longer than shared memory
@@ -153,12 +160,15 @@ int nd_slots(const int* K, int batch, int j, int* slots);
 // batch = 0: one array (the single-item entry points).  batch >= 1: `batch` items of prod(ns) elements back to back in y and x, each
 // with its own stop rule and info row (info: 3 batch doubles), bit for bit the single-item call on that item under the seq and chunked
 // engines; tape: the batched layout (nd_tape_head_bytes(batch) bytes of header and K table, then passes of batch items each).
+// lstride: the penalties' row stride -- 0, one row lambdas[0..npen) for every item; npen (batch >= 1), item b's row at lambdas + b npen
+// (DESIGN.md section 16.1): item b is then solved with its own row, bit for bit as the single-item call with that row under the seq and
+// chunked engines.
 template <typename T> int pd2_device(const T* y, const double* lambdas, const double* dims, T* x, double* info, const int* ns,
                                      int nds, int npen, int maxIters, void* ws, Engine eng, cudaStream_t st, void* tape = nullptr,
-                                     int batch = 0);
+                                     int batch = 0, int lstride = 0);
 template <typename T> int pd_device(const T* y, const double* lambdas_scaled, const double* dims, T* x, double* info,
                                     const int* ns, int nds, int npen, int maxIters, void* ws, Engine eng, cudaStream_t st,
-                                    void* tape = nullptr, int batch = 0);
+                                    void* tape = nullptr, int batch = 0, int lstride = 0);
 // Engine choice under ENGINE_AUTO for data y (device pointer, n elements) and penalty lam: the lane engine keeps every open segment of
 // a fiber inside a 64-row (float64) / 128-row (float32) shared-memory window and sends fibers whose segments outgrow it through a
 // slow exact repair path, so it only pays while segments are short -- lam not larger than about the mean step |y[i+1] - y[i]| of the
@@ -216,7 +226,9 @@ size_t nd_tape_head_bytes(int batch);
 // the tape of pass p (output y over the fibers g, penalty lam) into a tape of n-element passes
 template <typename T> cudaError_t pdr_tape_pass(void* tape, long long n, long long p, const T* y, FiberGeom g, T lam, cudaStream_t st);
 // the same into the passes that start at `passes`, each sized for cap_n elements (y covers the first nf * len of them)
-template <typename T> cudaError_t nd_tape_pass(void* passes, long long cap_n, long long p, const T* y, FiberGeom g, T lam, cudaStream_t st);
+// lamf != nullptr: fiber j's penalty is lamf[j / fpi] instead of lam (fiber_tape_lamf)
+template <typename T> cudaError_t nd_tape_pass(void* passes, long long cap_n, long long p, const T* y, FiberGeom g, T lam, cudaStream_t st,
+                                               const T* lamf = nullptr, long long fpi = 1);
 // writes the 256-byte header after the solve (arguments checked by the caller; axes = dims - 1)
 cudaError_t nd_tape_header(NdSolver s, void* tape, size_t elem, const int* ns, int nds, int npen, const double* dims, int maxIters, int iters,
                            cudaStream_t st);
@@ -272,7 +284,7 @@ enum { LANE_PLAIN = 0, LANE_DR_B = 1, LANE_DR_B_FINAL = 2, LANE_DRA = 3, LANE_DR
 // prox over the fibers (nf, len, inc); returns cudaErrorInvalidConfiguration when the shape does not suit (caller falls back)
 template <typename T>
 cudaError_t lane_prox(int op, const T* A, const T* B, const T* C, T* X, long long nf, int len, long long inc, T lam, void* scratch,
-                      cudaStream_t st, T* X2 = nullptr);
+                      cudaStream_t st, T* X2 = nullptr, const T* lamf = nullptr, long long fpi = 1);   // lamf: per-fiber penalties (plain op), all > 0
 void* lane_scratch(long long nf, int len);          // per-device records / counters (allocates: call outside stream capture)
 unsigned long long lane_scratch_generation();       // per device: allocations of that buffer so far (its layout changes with each)
 bool lane_shape_ok(long long nf, int len, long long inc, size_t elem, const void* const* ptrs, int nptrs);
@@ -295,6 +307,11 @@ cudaError_t vjp_fibers_tape(const uint32_t* F, const uint32_t* U, const T* g, T*
 // The segmentation tape of y over the fibers (nf, len, inc), nf a multiple of inc: F and U of vjp_tape_set_bytes(nf * len) bytes each.
 template <typename T>
 cudaError_t fiber_tape(const T* y, long long nf, int len, long long inc, T lam, const T* lamv, uint32_t* F, uint32_t* U, cudaStream_t st);
+// The same with fiber j's penalty lamf[j / fpi] (device table; fpi a multiple of inc, so that a group is a range of elements): bit for
+// bit the uniform tape of each fiber with its own penalty.
+template <typename T>
+cudaError_t fiber_tape_lamf(const T* y, long long nf, int len, long long inc, const T* lamf, long long fpi, uint32_t* F, uint32_t* U,
+                            cudaStream_t st);
 size_t vjp_scratch_bytes(long long nf, int len);
 int vjp_chunk_len(long long nf, int len);
 void vjp_set_tuning(int clen);

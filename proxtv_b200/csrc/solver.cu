@@ -10,6 +10,7 @@
 #include <float.h>
 #include <limits.h>
 #include <stdio.h>
+#include <string.h>
 #include <vector>
 
 namespace ptv {
@@ -30,14 +31,15 @@ static constexpr size_t SCRATCH_BYTES = (REDUCE_BLOCKS + 8) * sizeof(double);
 // Same kernels, same arithmetic, same results as the serial schedule; only the order of independent work changes.
 template <typename T>
 cudaError_t prox_fibers_chunked_contig(const T* A, const T* B, const T* C, InOp op, T* X, int out_op, FiberGeom g, T lam,
-                                       const T* lamv, cudaStream_t st, T* X2 = nullptr, long long inc2 = 0);
+                                       const T* lamv, cudaStream_t st, T* X2 = nullptr, long long inc2 = 0,
+                                       const T* lamf = nullptr, long long fpi = 1);
 template <typename T> cudaError_t gather_fibers_range(const T* A, const T* B, InOp op, T* out, FiberGeom g, int k_begin, int k_end, cudaStream_t st);
 template <typename T>
 cudaError_t scatter_fibers_ex_range(const T* in, const T* A, const T* B, const T* C, InOp op, int out_op, T* X, FiberGeom g,
                                     long long r_begin, long long r_end, cudaStream_t st);
 template <typename T>
 cudaError_t prox_fibers_chunked_contig_sparse(const T* A, const T* B, InOp op, T* X, FiberGeom g, T lam, const T* lamv, uint32_t* Mk, T* Cv,
-                                              cudaStream_t st);
+                                              cudaStream_t st, const T* lamf = nullptr, long long fpi = 1);
 template <typename T>
 cudaError_t scatter_fibers_ex_sparse_range(const T* in, const uint32_t* Mk, const T* Cv, const T* A, const T* B, const T* C, InOp op, int out_op,
                                            T* X, FiberGeom g, long long r_begin, long long r_end, cudaStream_t st);
@@ -497,7 +499,7 @@ int drw_device(size_t M, size_t N, int batch, int row_major, const T* Y, const T
 template <typename T> size_t ws_bytes_pd(long long n, int npen, int batch) {
     if (batch > 0) return ws_bytes_pd<T>(n * batch, npen, 0) + align256((size_t)(n * batch) * sizeof(T)) +
                           align256((size_t)batch * REDUCE_BLOCKS * sizeof(double)) + align256((size_t)batch * sizeof(double)) +
-                          align256((size_t)batch * sizeof(int));
+                          align256((size_t)batch * sizeof(int)) + align256((size_t)batch * (npen > 0 ? npen : 1) * sizeof(T));
     int arrays = 2 * npen + 4;   // PD_TV: p_i, z_i + 3 staging ; PD2_TV (npen <= 2): p, q, z, xl + 3 staging
     if (arrays < 8) arrays = 8;
     return (size_t)arrays * align256((size_t)n * sizeof(T)) + SCRATCH_BYTES + align256(2 * 64 * sizeof(void*));
@@ -520,7 +522,7 @@ static FiberGeom items_geom(const FiberGeom& g, int items) { return FiberGeom{g.
 template <typename T> struct NdItems {
     int batch = 0, m = 0; long long n = 0; T* out = nullptr; double* info = nullptr;
     std::vector<int> K, slots, next, map; std::vector<double> stop;
-    T* x = nullptr; double* partial = nullptr; double* dstop = nullptr; int* dmap = nullptr;
+    T* x = nullptr; double* partial = nullptr; double* dstop = nullptr; int* dmap = nullptr; T* dlam = nullptr;
     NdItems(int b, long long n_, T* out_, double* info_)
         : batch(b), m(b), n(n_), out(out_), info(info_), K(b, INT_MAX), slots(b), next(b), map(b), stop(b) {
         nd_slots(K.data(), b, 0, slots.data());
@@ -533,7 +535,8 @@ template <typename T> struct NdItems {
         x = (T*)w; w += align256((size_t)(n * b) * sizeof(T));
         partial = (double*)w; w += align256((size_t)b * REDUCE_BLOCKS * sizeof(double));
         dstop = (double*)w; w += align256((size_t)b * sizeof(double));
-        dmap = (int*)w;
+        dmap = (int*)w; w += align256((size_t)b * sizeof(int));
+        dlam = (T*)w;
     }
     void row(int b, int iters, double s) {
         info[3 * (size_t)b + INFO_ITERS] = iters; info[3 * (size_t)b + INFO_GAP] = s;
@@ -571,6 +574,51 @@ template <typename T> struct NdItems {
     void rest(int iters) { for (int b = 0; b < batch; b++) if (K[b] == INT_MAX) row(b, iters, DBL_MAX); }
 };
 
+// The penalties of a PD_TV / PD2_TV solve, lam[b * stride + i] for item b and term i: stride 0, one row shared by every item; stride npen,
+// one row per item (DESIGN.md section 16.1).  A pass over the running items takes the uniform kernels with scalar(i) when they all have
+// the same penalty for term i, else the per-fiber kernels with table(i): their penalties in slot order, in the device table I.dlam
+// ([npen][batch]), uploaded by sync() whenever the running items change -- before the first pass and after each compaction, in the
+// stream order of the iteration's other work.
+template <typename T> struct NdPens {
+    const double* lam; int stride, npen, batch;
+    std::vector<T> host; std::vector<char> uni, pos; int m = -1;
+    NdPens(const double* l, int s, int np, int b) : lam(l), stride(s), npen(np), batch(b), host((size_t)np * b), uni(np, 1), pos(np, 0) {}
+    T at(int b, int i) const { return (T)lam[(size_t)b * stride + i]; }
+    // the largest penalty of the whole table (the lane guard's)
+    double max() const {
+        double v = 0.0;
+        for (int b = 0; b < (stride ? batch : 1); b++) for (int i = 0; i < npen; i++) if (lam[(size_t)b * stride + i] > v) v = lam[(size_t)b * stride + i];
+        return v;
+    }
+    cudaError_t sync(const NdItems<T>& I, cudaStream_t st) {
+        if (!stride || I.m == m) return cudaSuccess;
+        m = I.m;
+        bool all = true;
+        for (int i = 0; i < npen; i++) {
+            T* h = host.data() + (size_t)i * batch;
+            for (int s = 0; s < m; s++) h[s] = at(I.slots[s], i);
+            uni[i] = 1; pos[i] = 1;
+            for (int s = 1; s < m; s++) if (memcmp(&h[s], &h[0], sizeof(T))) { uni[i] = 0; break; }
+            for (int s = 0; s < m; s++) if (!(h[s] > T(0))) { pos[i] = 0; break; }     // a zero keeps the table off the lane engine
+            all = all && uni[i];
+        }
+        return all ? cudaSuccess : cudaMemcpyAsync(I.dlam, host.data(), host.size() * sizeof(T), cudaMemcpyHostToDevice, st);
+    }
+    T scalar(int i) const { return stride ? host[(size_t)i * batch] : at(0, i); }
+    const T* table(const NdItems<T>& I, int i) const { return stride && !uni[i] ? I.dlam + (size_t)i * batch : nullptr; }
+};
+
+// One prox pass of term i over the running items' fibers g (fpi fibers per item), with their penalties, and its tape pass p (tp set)
+template <typename T>
+static cudaError_t nd_pass(const T* A, const T* B, InOp op, T* X, FiberGeom g, long long fpi, const NdPens<T>& L, const NdItems<T>& I, int i,
+                           Engine eng, T* scr, long long scr_elems, char* tp, long long nt, long long p, cudaStream_t st) {
+    const T* lamf = L.table(I, i);
+    cudaError_t e = lamf ? prox_fibers_lamf<T>(A, B, op, X, g, lamf, fpi, L.pos[i], eng, scr, st, scr_elems)
+                         : prox_fibers<T>(A, B, op, X, 0, g, L.scalar(i), nullptr, eng, scr, st, scr_elems);
+    if (e == cudaSuccess && tp) e = nd_tape_pass<T>(tp, nt, p, X, g, L.scalar(i), st, lamf, fpi);
+    return e;
+}
+
 const char* nd_terms(const int* ns, int nds, int npen, const double* dims, NdTerms* t) {
     long long n = 1;
     for (int i = 0; i < nds; i++) n *= ns[i];
@@ -599,7 +647,7 @@ static int read_stop(const double* dres, double* stop, cudaStream_t st) {
 // pass 2 iters, x as pass 2 iters + 1 (npen = 1: z as pass 0); nothing else changes.
 template <typename T>
 int pd2_device(const T* y, const double* lambdas, const double* dims, T* x_out, double* info, const int* ns, int nds, int npen,
-               int maxIters, void* ws, Engine eng, cudaStream_t st, void* tape, int batch) {
+               int maxIters, void* ws, Engine eng, cudaStream_t st, void* tape, int batch, int lstride) {
     if (npen > 2) { printf("PD2_TV: this algorithm can not work with more than 2 penalties\n");      // :95-96
                     if (info) info[INFO_RC] = RC_ERROR; return 0; }
     NdTerms t;
@@ -607,7 +655,8 @@ int pd2_device(const T* y, const double* lambdas, const double* dims, T* x_out, 
     const long long n = t.n;
     const int nb = batch > 0 ? batch : 1;
     if (maxIters <= 0) maxIters = MAX_ITERS_PD;
-    if (npen >= 1) eng = lane_guard<T>(eng, y, n * nb, npen >= 2 && lambdas[1] > lambdas[0] ? lambdas[1] : lambdas[0], st);
+    NdPens<T> L(lambdas, lstride, npen >= 1 && npen <= 2 ? npen : 0, nb);
+    if (npen >= 1 && npen <= 2) eng = lane_guard<T>(eng, y, n * nb, L.max(), st);
     if (npen < 1 || why) { printf("PD2_TV: invalid penalty dimensions\n"); if (info) info[INFO_RC] = RC_ERROR; return 0; }
     double row1[3];
     if (!info) info = row1;
@@ -630,13 +679,12 @@ int pd2_device(const T* y, const double* lambdas, const double* dims, T* x_out, 
             const int m = I.m;
             const long long nm = n * m;
             const FiberGeom g0 = items_geom(t.g[0], m), g1 = npen >= 2 ? items_geom(t.g[1], m) : g0;
+            PTV_TRY(L.sync(I, st));
             PTV_TRY(cudaMemcpyAsync(xl, x, (size_t)nm * sizeof(T), cudaMemcpyDeviceToDevice, st));
-            PTV_TRY(prox_fibers<T>(x, p, IN_A_PLUS_B, z, 0, g0, (T)lambdas[0], nullptr, eng, scr, st, 3 * nm));      // :171-208
-            if (tp) PTV_TRY(nd_tape_pass<T>(tp, nt, 2LL * iters, z, g0, (T)lambdas[0], st));
+            PTV_TRY(nd_pass<T>(x, p, IN_A_PLUS_B, z, g0, t.g[0].nf, L, I, 0, eng, scr, 3 * nm, tp, nt, 2LL * iters, st));   // :171-208
             PTV_TRY(ew_dual_update<T>(p, x, z, nm, st));                                              // :211-213
             if (npen >= 2) {
-                PTV_TRY(prox_fibers<T>(z, q, IN_A_PLUS_B, x, 0, g1, (T)lambdas[1], nullptr, eng, scr, st, 3 * nm));  // :216-258
-                if (tp) PTV_TRY(nd_tape_pass<T>(tp, nt, 2LL * iters + 1, x, g1, (T)lambdas[1], st));
+                PTV_TRY(nd_pass<T>(z, q, IN_A_PLUS_B, x, g1, t.g[1].nf, L, I, 1, eng, scr, 3 * nm, tp, nt, 2LL * iters + 1, st));  // :216-258
                 PTV_TRY(ew_dual_update<T>(q, z, x, nm, st));                                          // :261-263
             } else {
                 PTV_TRY(cudaMemcpyAsync(x, z, (size_t)nm * sizeof(T), cudaMemcpyDeviceToDevice, st)); // :266-269
@@ -656,10 +704,11 @@ int pd2_device(const T* y, const double* lambdas, const double* dims, T* x_out, 
 // "<name>: <reason>" on stdout, info[RC] = RC_ERROR, false.
 template <typename T>
 static bool pd_start(const char* name, const T* y, const double* lam, const double* dims, double* info, const int* ns, int nds, int npen,
-                     NdTerms* t, Engine* eng, cudaStream_t st, int items = 1) {
+                     NdTerms* t, Engine* eng, cudaStream_t st, int items = 1, int lstride = 0) {
     const char* why = nd_terms(ns, nds, npen, dims, t);
     if (npen <= 64) {
-        double lmax = 0.0; for (int i = 0; i < npen; i++) if (lam[i] > lmax) lmax = lam[i];
+        double lmax = 0.0;
+        for (int b = 0; b < (lstride ? items : 1); b++) for (int i = 0; i < npen; i++) if (lam[(size_t)b * lstride + i] > lmax) lmax = lam[(size_t)b * lstride + i];
         *eng = lane_guard<T>(*eng, y, t->n * items, lmax, st);
     }
     if (why) { printf("%s: %s\n", name, why); if (info) info[INFO_RC] = RC_ERROR; return false; }
@@ -689,11 +738,11 @@ template <typename T> static cudaError_t pd_ws(void* ws, long long n, int npen, 
 // tape of its output p_i is written as pass iters * npen + i; nothing else changes.
 template <typename T>
 int pd_device(const T* y, const double* lam, const double* dims, T* x_out, double* info, const int* ns, int nds, int npen,
-              int maxIters, void* ws, Engine eng, cudaStream_t st, void* tape, int batch) {
+              int maxIters, void* ws, Engine eng, cudaStream_t st, void* tape, int batch, int lstride) {
     if (maxIters <= 0) maxIters = MAX_ITERS_PD;
     const int nb = batch > 0 ? batch : 1;
     NdTerms t;
-    if (!pd_start<T>("PD_TV", y, lam, dims, info, ns, nds, npen, &t, &eng, st, nb)) return 0;
+    if (!pd_start<T>("PD_TV", y, lam, dims, info, ns, nds, npen, &t, &eng, st, nb, lstride)) return 0;
     const long long n = t.n, nt = n * nb;
     double row1[3];
     if (!info) info = row1;
@@ -709,13 +758,13 @@ int pd_device(const T* y, const double* lam, const double* dims, T* x_out, doubl
         for (int i = 0; i < npen; i++) state[1 + i] = W.hz[i];
         PTV_TRY(cudaMemsetAsync(x, 0, (size_t)nt * sizeof(T), st));                                   // :125-130
         for (int i = 0; i < npen; i++) PTV_TRY(cudaMemcpyAsync(W.hz[i], y, (size_t)nt * sizeof(T), cudaMemcpyDeviceToDevice, st));
+        NdPens<T> L(lam, lstride, npen, nb);
         while (I.m > 0) {                                                                             // :151 per item
             const int m = I.m;
-            for (int i = 0; i < npen; i++) {
-                const FiberGeom g = items_geom(t.g[i], m);
-                PTV_TRY(prox_fibers<T>(W.hz[i], nullptr, IN_A, W.hp[i], 0, g, (T)lam[i], nullptr, eng, W.scr, st, 3 * n * m));  // :171-208
-                if (tp) PTV_TRY(nd_tape_pass<T>(tp, nt, (long long)iters * npen + i, W.hp[i], g, (T)lam[i], st));
-            }
+            PTV_TRY(L.sync(I, st));
+            for (int i = 0; i < npen; i++)                                                            // :171-208
+                PTV_TRY(nd_pass<T>(W.hz[i], nullptr, IN_A, W.hp[i], items_geom(t.g[i], m), t.g[i].nf, L, I, i, eng, W.scr, 3 * n * m, tp, nt,
+                                   (long long)iters * npen + i, st));
             PTV_TRY(ew_pd_combine_items<T>(W.dp, W.dz, W.hp, W.hz, npen, x, n, m, I.partial, I.dstop, st));   // :212-227 per item
             iters++;
             // the loop condition; info rows (:233-245)
@@ -776,9 +825,9 @@ int pdr_device(const T* y, const double* lam, const double* dims, T* x, double* 
     template struct DrwPasses<T>; \
     template size_t ws_bytes_pd<T>(long long, int, int); \
     template int pd2_device<T>(const T*, const double*, const double*, T*, double*, const int*, int, int, int, void*, Engine, cudaStream_t, \
-                               void*, int); \
+                               void*, int, int); \
     template int pd_device<T>(const T*, const double*, const double*, T*, double*, const int*, int, int, int, void*, Engine, cudaStream_t, \
-                              void*, int); \
+                              void*, int, int); \
     template int pdr_device<T>(const T*, const double*, const double*, T*, double*, const int*, int, int, int, void*, Engine, cudaStream_t, \
                                void*);
 INST(double)

@@ -251,16 +251,17 @@ cudaError_t vjp_fibers_tape(const uint32_t* F, const uint32_t* U, const T* g, T*
 }
 
 // The tape of y over the fibers (nf, len, inc) (nf a multiple of inc: the fibers cover the nf * len elements once): one warp per
-// 32-element word, the words of the 256-byte padding written as 0.
-template <typename T>
+// 32-element word, the words of the 256-byte padding written as 0.  LAMF: the penalty of fiber j is lamf[j / fpi] -- with fpi a
+// multiple of inc a group of fibers is a range of epi = fpi len elements, so element i's is lamf[i / epi].
+template <typename T, bool LAMF = false>
 __global__ void k_fiber_tape(const T* __restrict__ y, long long n, int len, long long inc, double lam, const T* __restrict__ w,
-                             uint32_t* __restrict__ F, uint32_t* __restrict__ U, long long nwords) {
+                             uint32_t* __restrict__ F, uint32_t* __restrict__ U, long long nwords, const T* __restrict__ lamf, long long epi) {
     const int lane = threadIdx.x & 31;
     const long long w0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5, ws = ((long long)gridDim.x * blockDim.x) >> 5;
     for (long long q = w0; q < nwords; q += ws) {
         const long long i = q * 32 + lane;
         uint32_t f = 0, u = 0;
-        if (i < n) vjp_tape_edge<T>(y, i, len, inc, lam, w, f, u);
+        if (i < n) vjp_tape_edge<T>(y, i, len, inc, LAMF ? (double)lamf[i / epi] : lam, w, f, u);
         const uint32_t bf = __ballot_sync(0xffffffffu, f), bu = __ballot_sync(0xffffffffu, u);
         if (lane == 0) { F[q] = bf; U[q] = bu; }
     }
@@ -274,7 +275,20 @@ cudaError_t fiber_tape(const T* y, long long nf, int len, long long inc, T lam, 
     long long blocks = (nwords * 32 + 255) / 256;
     if (blocks > 132LL * 16) blocks = 132LL * 16;
     KernelSpan span(ptv::KC_ELEMENTWISE, 1, st);
-    k_fiber_tape<T><<<(unsigned)blocks, 256, 0, st>>>(y, n, len, inc, (double)lam, lamv, F, U, nwords);
+    k_fiber_tape<T><<<(unsigned)blocks, 256, 0, st>>>(y, n, len, inc, (double)lam, lamv, F, U, nwords, nullptr, 1);
+    return cudaGetLastError();
+}
+
+template <typename T>
+cudaError_t fiber_tape_lamf(const T* y, long long nf, int len, long long inc, const T* lamf, long long fpi, uint32_t* F, uint32_t* U,
+                            cudaStream_t st) {
+    const long long n = nf * (long long)len;
+    const long long nwords = (long long)(vjp_tape_set_bytes(n) / 4);
+    if (nwords == 0) return cudaSuccess;
+    long long blocks = (nwords * 32 + 255) / 256;
+    if (blocks > 132LL * 16) blocks = 132LL * 16;
+    KernelSpan span(ptv::KC_ELEMENTWISE, 1, st);
+    k_fiber_tape<T, true><<<(unsigned)blocks, 256, 0, st>>>(y, n, len, inc, 0.0, nullptr, F, U, nwords, lamf, fpi * (long long)len);
     return cudaGetLastError();
 }
 
@@ -288,5 +302,7 @@ template cudaError_t vjp_fibers_tape<float>(const uint32_t*, const uint32_t*, co
                                             void*, cudaStream_t);
 template cudaError_t fiber_tape<double>(const double*, long long, int, long long, double, const double*, uint32_t*, uint32_t*, cudaStream_t);
 template cudaError_t fiber_tape<float>(const float*, long long, int, long long, float, const float*, uint32_t*, uint32_t*, cudaStream_t);
+template cudaError_t fiber_tape_lamf<double>(const double*, long long, int, long long, const double*, long long, uint32_t*, uint32_t*, cudaStream_t);
+template cudaError_t fiber_tape_lamf<float>(const float*, long long, int, long long, const float*, long long, uint32_t*, uint32_t*, cudaStream_t);
 
 }  // namespace ptvv
